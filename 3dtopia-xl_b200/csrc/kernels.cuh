@@ -69,5 +69,13 @@ size_t primsdf_grid_bytes(long long cap_entries);
 int launch_primsdf_grid_build(const float* srt, int K, void* ws, size_t ws_bytes, cudaStream_t st);
 int launch_primsdf_query_grid(const float* x, const float* srt, const float* feat, const void* ws, size_t ws_bytes, long long n, int K, int S, int dim_feat,
                               int inference, float* out, cudaStream_t st);
+int launch_primsdf_sdf_grid(const float* coords, int R, const float* srt, const float* feat, const void* ws, size_t ws_bytes, int K, int S, int dim_feat,
+                            int inference, float* grid, cudaStream_t st);
+
+// marching_cubes.cu : dense fp32 volume -> indexed triangle mesh (count, then emit on the same workspace)
+size_t mc_workspace_bytes(long long X, long long Y, long long Z);
+int launch_mc_count(const float* vol, long long X, long long Y, long long Z, float iso, void* ws, size_t ws_bytes, long long* counts, cudaStream_t st);
+int launch_mc_emit(const float* vol, long long X, long long Y, long long Z, float iso, const float origin[3], const float spacing[3], void* ws, size_t ws_bytes,
+                   float* verts, long long* faces, cudaStream_t st);
 
 }  // namespace tpx

@@ -14,19 +14,21 @@ constexpr int PS_THREADS = 256;
 constexpr int PS_CHUNK = 1024;   // primitives staged per pass (16 KB of float4)
 
 // ---- pieces shared by the exhaustive and the grid-binned kernels (identical arithmetic => identical results) ----------------------
-template <int DF>
+// DF is the per-primitive channel stride of feat, NC <= DF the number of leading channels accumulated: the SDF-grid kernel
+// accumulates channel 0 alone with exactly the channel-0 arithmetic of the full query.
+template <int NC>
 struct PointAcc {
-    float acc[DF];
+    float acc[NC];
     float wsum;
 };
 
 // visit primitive k for the point (px,py,pz): box weight, and — if it covers the point — its trilinear sample
-template <int DF>
-__device__ __forceinline__ void visit_prim(PointAcc<DF>& a, float px, float py, float pz, const float4 v /* scale, tx, ty, tz */, int k,
+template <int NC, int DF>
+__device__ __forceinline__ void visit_prim(PointAcc<NC>& a, float px, float py, float pz, const float4 v /* scale, tx, ty, tz */, int k,
                                            const float* __restrict__ feat, int S, int S3, float half_span) {
     const float inv = 1.0f / v.x;
     const float dx = px - v.y, dy = py - v.z, dz = pz - v.w;
-    float lx = dx * inv, ly = dy * inv, lz = dz * inv;
+    float lx = __fmul_rn(dx, inv), ly = __fmul_rn(dy, inv), lz = __fmul_rn(dz, inv);
     float w = 1.0f - fmaxf(fabsf(lx), fmaxf(fabsf(ly), fabsf(lz)));
     if (fabsf(w) < 1e-5f) {   // on the box boundary: decide with the reference's exact division, not the reciprocal
         lx = dx / v.x; ly = dy / v.x; lz = dz / v.x;
@@ -38,32 +40,35 @@ __device__ __forceinline__ void visit_prim(PointAcc<DF>& a, float px, float py, 
         const float fx = (lx + 1.0f) * half_span, fy = (ly + 1.0f) * half_span, fz = (lz + 1.0f) * half_span;
         const int x0 = min(static_cast<int>(fx), S - 2), y0 = min(static_cast<int>(fy), S - 2), z0 = min(static_cast<int>(fz), S - 2);
         const float ax = fx - x0, ay = fy - y0, az = fz - z0;
+        const float bx = 1.f - ax, by = 1.f - ay, bz = 1.f - az;
         const float* f = feat + static_cast<size_t>(k) * DF * S3 + (z0 * S + y0) * S + x0;
+        // Every product is rounded or fused as written (no compiler contraction), so the sdf channel comes out bit-identical
+        // whether one channel (the SDF grid) or all six (the point query) are accumulated: u (1 - t) + v t = fma(1 - t, u, t v).
 #pragma unroll
-        for (int c = 0; c < DF; ++c) {
+        for (int c = 0; c < NC; ++c) {
             const float* fc = f + c * S3;
-            const float c00 = fc[0] * (1.f - ax) + fc[1] * ax;
-            const float c01 = fc[S] * (1.f - ax) + fc[S + 1] * ax;
-            const float c10 = fc[S * S] * (1.f - ax) + fc[S * S + 1] * ax;
-            const float c11 = fc[S * S + S] * (1.f - ax) + fc[S * S + S + 1] * ax;
-            const float val = (c00 * (1.f - ay) + c01 * ay) * (1.f - az) + (c10 * (1.f - ay) + c11 * ay) * az;
+            const float c00 = __fmaf_rn(bx, fc[0], __fmul_rn(ax, fc[1]));
+            const float c01 = __fmaf_rn(bx, fc[S], __fmul_rn(ax, fc[S + 1]));
+            const float c10 = __fmaf_rn(bx, fc[S * S], __fmul_rn(ax, fc[S * S + 1]));
+            const float c11 = __fmaf_rn(bx, fc[S * S + S], __fmul_rn(ax, fc[S * S + S + 1]));
+            const float val = __fmaf_rn(bz, __fmaf_rn(by, c00, __fmul_rn(ay, c01)), __fmul_rn(az, __fmaf_rn(by, c10, __fmul_rn(ay, c11))));
             a.acc[c] = fmaf(w, val, a.acc[c]);
         }
     }
 }
 
-template <int DF>
-__device__ __forceinline__ void finish_point(const PointAcc<DF>& a, float px, float py, float pz, int best_k, const float* __restrict__ srt,
+template <int NC, int DF>
+__device__ __forceinline__ void finish_point(const PointAcc<NC>& a, float px, float py, float pz, int best_k, const float* __restrict__ srt,
                                              const float* __restrict__ feat, int K, int S, int S3, float half_span, int inference, float* __restrict__ o) {
     if (a.wsum > 0.f) {
         const float inv = 1.0f / (a.wsum + 1e-6f);
         o[0] = a.acc[0] * inv;
 #pragma unroll
-        for (int c = 1; c < DF; ++c) o[c] = fminf(fmaxf(a.acc[c] * inv, 0.f), 1.f);
+        for (int c = 1; c < NC; ++c) o[c] = fminf(fmaxf(a.acc[c] * inv, 0.f), 1.f);
         return;
     }
 #pragma unroll
-    for (int c = 0; c < DF; ++c) o[c] = 0.f;
+    for (int c = 0; c < NC; ++c) o[c] = 0.f;
     if (inference && K > 0) {
         // SDF of an uncovered point: nearest voxel of the nearest primitive, same sign, plus the L2 distance to it
         const float4 v = *reinterpret_cast<const float4*>(srt + 4 * static_cast<size_t>(best_k));
@@ -123,11 +128,11 @@ __global__ void __launch_bounds__(PS_THREADS) primsdf_query_kernel(const float* 
             const float dx = px - p.y, dy = py - p.z, dz = pz - p.w;
             const float d2 = dx * dx + dy * dy + dz * dz;
             if (d2 < best_d2) { best_d2 = d2; best_k = k0 + t; }
-            visit_prim<DF>(a, px, py, pz, p, k0 + t, feat, S, S3, half_span);
+            visit_prim<DF, DF>(a, px, py, pz, p, k0 + t, feat, S, S3, half_span);
         }
     }
     if (!live) return;
-    finish_point<DF>(a, px, py, pz, best_k, srt, feat, K, S, S3, half_span, inference, out + static_cast<size_t>(i) * DF);
+    finish_point<DF, DF>(a, px, py, pz, best_k, srt, feat, K, S, S3, half_span, inference, out + static_cast<size_t>(i) * DF);
 }
 
 // =====================================================================================================================
@@ -255,39 +260,41 @@ __global__ void __launch_bounds__(1024) grid_scan_kernel(const int* __restrict__
     }
 }
 
-template <int DF>
-__global__ void __launch_bounds__(PS_THREADS) primsdf_query_grid_kernel(const float* __restrict__ x, const float* __restrict__ srt,
-                                                                        const float* __restrict__ feat, const GridHdr* __restrict__ hdr,
-                                                                        const int* __restrict__ offsets, const int* __restrict__ entries, long long n, int K,
-                                                                        int S, int inference, float* __restrict__ out) {
-    const long long i = static_cast<long long>(blockIdx.x) * PS_THREADS + threadIdx.x;
-    if (i >= n) return;
-    const float px = x[3 * i], py = x[3 * i + 1], pz = x[3 * i + 2];
-    PointAcc<DF> a;
+// one point of the binned query; hdr == nullptr (no grid) takes the exhaustive loop
+template <int NC, int DF>
+__device__ __forceinline__ void query_point_binned(float px, float py, float pz, const float* __restrict__ srt, const float* __restrict__ feat,
+                                                   const GridHdr* __restrict__ hdr, const int* __restrict__ offsets, const int* __restrict__ entries, int K,
+                                                   int S, int inference, float* __restrict__ o) {
+    PointAcc<NC> a;
 #pragma unroll
-    for (int c = 0; c < DF; ++c) a.acc[c] = 0.f;
+    for (int c = 0; c < NC; ++c) a.acc[c] = 0.f;
     a.wsum = 0.f;
     float best_d2 = INFINITY;
     int best_k = 0;
     const int S3 = S * S * S;
     const float half_span = 0.5f * static_cast<float>(S - 1);
-    const float gx = (px - hdr->ox) * hdr->inv_h, gy = (py - hdr->oy) * hdr->inv_h, gz = (pz - hdr->oz) * hdr->inv_h;
-    const bool inside = gx >= 0.f && gy >= 0.f && gz >= 0.f && gx < static_cast<float>(PG_G) && gy < static_cast<float>(PG_G) && gz < static_cast<float>(PG_G);
-    if (!inside || hdr->overflow != 0) {          // exhaustive loop (rare: points outside the primitives' bounding box / oversized lists)
+    bool inside = false;
+    int cell = 0;
+    if (hdr != nullptr) {
+        const float gx = (px - hdr->ox) * hdr->inv_h, gy = (py - hdr->oy) * hdr->inv_h, gz = (pz - hdr->oz) * hdr->inv_h;
+        inside = gx >= 0.f && gy >= 0.f && gz >= 0.f && gx < static_cast<float>(PG_G) && gy < static_cast<float>(PG_G) && gz < static_cast<float>(PG_G) &&
+                 hdr->overflow == 0;
+        if (inside) cell = (static_cast<int>(gz) * PG_G + static_cast<int>(gy)) * PG_G + static_cast<int>(gx);
+    }
+    if (!inside) {          // exhaustive loop (rare: points outside the primitives' bounding box / oversized lists / no grid)
         for (int k = 0; k < K; ++k) {
             const float4 p = __ldg(reinterpret_cast<const float4*>(srt + 4 * static_cast<size_t>(k)));
             const float dx = px - p.y, dy = py - p.z, dz = pz - p.w;
             const float d2 = dx * dx + dy * dy + dz * dz;
             if (d2 < best_d2) { best_d2 = d2; best_k = k; }
-            visit_prim<DF>(a, px, py, pz, p, k, feat, S, S3, half_span);
+            visit_prim<NC, DF>(a, px, py, pz, p, k, feat, S, S3, half_span);
         }
     } else {
-        const int cell = (static_cast<int>(gz) * PG_G + static_cast<int>(gy)) * PG_G + static_cast<int>(gx);
         const int c0 = offsets[cell], c1 = offsets[cell + 1];
         for (int e = c0; e < c1; ++e) {
             const int k = entries[e];
             const float4 p = __ldg(reinterpret_cast<const float4*>(srt + 4 * static_cast<size_t>(k)));
-            visit_prim<DF>(a, px, py, pz, p, k, feat, S, S3, half_span);
+            visit_prim<NC, DF>(a, px, py, pz, p, k, feat, S, S3, half_span);
         }
         if (!(a.wsum > 0.f) && inference) {
             const int n0 = offsets[PG_CELLS + cell], n1 = offsets[PG_CELLS + cell + 1];
@@ -300,7 +307,30 @@ __global__ void __launch_bounds__(PS_THREADS) primsdf_query_grid_kernel(const fl
             }
         }
     }
-    finish_point<DF>(a, px, py, pz, best_k, srt, feat, K, S, S3, half_span, inference, out + static_cast<size_t>(i) * DF);
+    finish_point<NC, DF>(a, px, py, pz, best_k, srt, feat, K, S, S3, half_span, inference, o);
+}
+
+template <int DF>
+__global__ void __launch_bounds__(PS_THREADS) primsdf_query_grid_kernel(const float* __restrict__ x, const float* __restrict__ srt,
+                                                                        const float* __restrict__ feat, const GridHdr* __restrict__ hdr,
+                                                                        const int* __restrict__ offsets, const int* __restrict__ entries, long long n, int K,
+                                                                        int S, int inference, float* __restrict__ out) {
+    const long long i = static_cast<long long>(blockIdx.x) * PS_THREADS + threadIdx.x;
+    if (i >= n) return;
+    query_point_binned<DF, DF>(x[3 * i], x[3 * i + 1], x[3 * i + 2], srt, feat, hdr, offsets, entries, K, S, inference, out + static_cast<size_t>(i) * DF);
+}
+
+// sdf channel of the query on the R^3 lattice (coords[i], coords[j], coords[k]); grid[(i R + j) R + k] (inference.py:108-116:
+// meshgrid(indexing='ij'), reshape(R,R,R)); the points are never materialised
+__global__ void __launch_bounds__(PS_THREADS) primsdf_sdf_grid_kernel(const float* __restrict__ coords, int R, const float* __restrict__ srt,
+                                                                      const float* __restrict__ feat, const GridHdr* __restrict__ hdr,
+                                                                      const int* __restrict__ offsets, const int* __restrict__ entries, int K, int S,
+                                                                      int inference, float* __restrict__ grid) {
+    const long long idx = static_cast<long long>(blockIdx.x) * PS_THREADS + threadIdx.x;
+    const long long n = static_cast<long long>(R) * R * R;
+    if (idx >= n) return;
+    const int k = static_cast<int>(idx % R), j = static_cast<int>((idx / R) % R), i = static_cast<int>(idx / (static_cast<long long>(R) * R));
+    query_point_binned<1, 6>(coords[i], coords[j], coords[k], srt, feat, hdr, offsets, entries, K, S, inference, grid + idx);
 }
 }  // namespace
 
@@ -372,6 +402,21 @@ int launch_primsdf_query_grid(const float* x, const float* srt, const float* fea
     const long long blocks = (n + PS_THREADS - 1) / PS_THREADS;
     TPX_CHECK(blocks < (1LL << 31), TPX_ERR_SHAPE, "primsdf_query: too many points");
     primsdf_query_grid_kernel<6><<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(x, srt, feat, g.hdr, g.offsets, g.entries, n, K, S, inference, out);
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+int launch_primsdf_sdf_grid(const float* coords, int R, const float* srt, const float* feat, const void* ws, size_t ws_bytes, int K, int S, int dim_feat,
+                            int inference, float* grid, cudaStream_t st) {
+    TPX_CHECK(dim_feat == 6, TPX_ERR_SHAPE, "primsdf_sdf_grid: dim_feat %d (kernel covers the released 6-channel layout)", dim_feat);
+    TPX_CHECK(S >= 2 && S <= 32 && K >= 0 && (K > 0 || ws == nullptr), TPX_ERR_SHAPE, "primsdf_sdf_grid: bad primitive geometry (S %d, K %d)", S, K);
+    TPX_CHECK(R >= 1 && R <= 2048, TPX_ERR_SHAPE, "primsdf_sdf_grid: resolution %d (1..2048)", R);
+    TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0, TPX_ERR_ARG, "primsdf_sdf_grid: srt must be 16-B aligned");
+    GridPtrs g{nullptr, nullptr, nullptr, nullptr, 0};
+    if (ws != nullptr) g = grid_carve(const_cast<void*>(ws), ws_bytes);
+    ProfScope prof(PROF_VAE_MISC, st);
+    const long long blocks = (static_cast<long long>(R) * R * R + PS_THREADS - 1) / PS_THREADS;
+    primsdf_sdf_grid_kernel<<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(coords, R, srt, feat, g.hdr, g.offsets, g.entries, K, S, inference, grid);
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }

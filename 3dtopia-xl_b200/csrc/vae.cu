@@ -361,6 +361,14 @@ int tpx_primsdf_query_grid(const float* x, const float* srt, const float* feat, 
     return launch_primsdf_query_grid(x, srt, feat, grid_ws, grid_bytes, n, K, S, dim_feat, inference, out, static_cast<cudaStream_t>(stream));
 }
 
+int tpx_primsdf_sdf_grid(const float* coords, int R, const float* srt, const float* feat, const void* grid_ws, size_t grid_bytes, int K, int S, int dim_feat,
+                         int inference, float* grid_out, void* stream) {
+    TPX_CHECK(coords != nullptr && srt != nullptr && feat != nullptr && grid_out != nullptr, TPX_ERR_ARG, "primsdf_sdf_grid: null argument");
+    int rc = tpx_device_check();
+    if (rc != TPX_OK) return rc;
+    return launch_primsdf_sdf_grid(coords, R, srt, feat, grid_ws, grid_bytes, K, S, dim_feat, inference, grid_out, static_cast<cudaStream_t>(stream));
+}
+
 int tpx_groupnorm_silu(const void* x, const void* gamma, const void* beta, int P, int S3, int C, int groups, float eps, int apply_silu, void* out,
                        void* stream) {
     TPX_CHECK(x != nullptr && gamma != nullptr && beta != nullptr && out != nullptr, TPX_ERR_ARG, "groupnorm_silu: null argument");

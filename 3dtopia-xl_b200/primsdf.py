@@ -12,7 +12,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, mesh
 
 
 class PrimSDF(nn.Module):
@@ -48,16 +48,56 @@ class PrimSDF(nn.Module):
                 _lib.check(lib.tpx_primsdf_query(xx.data_ptr(), srt.data_ptr(), feat.data_ptr(), n, K, self.prim_shape, self.dim_feat,
                                                  0 if self.training else 1, out.data_ptr(), _lib.stream_ptr()), "tpx_primsdf_query")
             else:
-                key = (self.srt_param.data_ptr(), self.srt_param._version, K, str(xx.device))
-                if self._grid is None or self._grid[0] != key:
-                    nbytes = int(lib.tpx_primsdf_grid_bytes(self.grid_entries))
-                    ws = torch.empty(nbytes, dtype=torch.uint8, device=xx.device)
-                    _lib.check(lib.tpx_primsdf_grid_build(srt.data_ptr(), K, ws.data_ptr(), nbytes, _lib.stream_ptr()), "tpx_primsdf_grid_build")
-                    self._grid = (key, self.srt_param.data, ws)     # holding the tensor keeps its address from being recycled under the key
-                ws = self._grid[2]
+                ws = self._grid_workspace(srt, K, xx.device)
                 _lib.check(lib.tpx_primsdf_query_grid(xx.data_ptr(), srt.data_ptr(), feat.data_ptr(), ws.data_ptr(), ws.numel(), n, K, self.prim_shape,
                                                       self.dim_feat, 0 if self.training else 1, out.data_ptr(), _lib.stream_ptr()), "tpx_primsdf_query_grid")
         return {"sdf": out[:, 0:1], "tex": out[:, 1:4], "mat": out[:, 4:6]}
+
+    def _grid_workspace(self, srt: torch.Tensor, K: int, device) -> torch.Tensor:
+        """The binned lists of the current srt_param (tpx_primsdf_grid_build), rebuilt only when srt_param changes."""
+        lib = _lib.lib()
+        key = (self.srt_param.data_ptr(), self.srt_param._version, K, str(device))
+        if self._grid is None or self._grid[0] != key:
+            nbytes = int(lib.tpx_primsdf_grid_bytes(self.grid_entries))
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+            _lib.check(lib.tpx_primsdf_grid_build(srt.data_ptr(), K, ws.data_ptr(), nbytes, _lib.stream_ptr()), "tpx_primsdf_grid_build")
+            self._grid = (key, self.srt_param.data, ws)     # holding the tensor keeps its address from being recycled under the key
+        return self._grid[2]
+
+    def sdf_grid(self, resolution: int, bound: float = 1.0) -> torch.Tensor:
+        """sdf of the query on the resolution^3 lattice linspace(-bound, bound, resolution)^3: fp32 [R,R,R] on the module's device,
+        grid[i,j,k] at (x, y, z) = (xx[i], xx[j], xx[k]).  Bit-identical to the grid extract_texmesh builds from ``forward`` over the
+        meshgrid points (inference.py:107-116), without materialising them; the uncovered-point approximation follows
+        ``self.training`` as in ``forward``."""
+        R = int(resolution)
+        if R < 1:
+            raise ValueError(f"resolution must be >= 1, got {resolution}")
+        if not self.srt_param.is_cuda:
+            raise _lib.TpxError("PrimSDF query runs on CUDA only (no CPU path): move the module to the GPU")
+        lib = _lib.lib()
+        dev = self.srt_param.device
+        srt = self.srt_param.detach().float().contiguous()
+        feat = self.feat_param.detach().float().contiguous()
+        K = srt.shape[0]
+        grid = torch.empty(R, R, R, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            coords = torch.linspace(-bound, bound, R, device=dev)
+            ws = self._grid_workspace(srt, K, dev) if 1 <= K <= 4096 else None
+            _lib.check(lib.tpx_primsdf_sdf_grid(coords.data_ptr(), R, srt.data_ptr(), feat.data_ptr(), _lib.ptr(ws), 0 if ws is None else ws.numel(), K,
+                                                self.prim_shape, self.dim_feat, 0 if self.training else 1, grid.data_ptr(), _lib.stream_ptr()),
+                       "tpx_primsdf_sdf_grid")
+        return grid
+
+    def extract_mesh(self, resolution: int = 256, isovalue: float = 0.0, bound: float = 1.0):
+        """Surface of the sdf field on the GPU: ``sdf_grid`` + marching cubes, in world coordinates (origin -bound, spacing
+        2 bound / (R - 1)), i.e. inference.py:107-124 without the host copy.  Returns (verts fp32 [V,3], faces int64 [F,3]) on the
+        module's device.  The primitive noise filter of extract_texmesh (:90-103) stays with the caller."""
+        R = int(resolution)
+        if R < 2:
+            raise ValueError(f"resolution must be >= 2, got {resolution}")
+        grid = self.sdf_grid(R, bound)
+        step = 2.0 * bound / (R - 1)
+        return mesh._mesh(grid, isovalue, origin=(-bound,) * 3, spacing=(step,) * 3)
 
     def sdf2alpha(self, sdf):
         return torch.exp(-(sdf / self.sdf2alpha_var) ** 2)

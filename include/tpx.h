@@ -225,6 +225,33 @@ int tpx_raymarch_preview(const float* template_chlast, const float* primpos, con
 int tpx_primsdf_grid_build(const float* srt_dev, int K, void* grid_ws, size_t grid_bytes, void* stream);
 int tpx_primsdf_query_grid(const float* x_dev, const float* srt_dev, const float* feat_dev, const void* grid_ws, size_t grid_bytes, int64_t n, int K, int S,
                            int dim_feat, int inference, float* out_dev, void* stream);
+/* The sdf column of the same query on the R x R x R lattice (coords[i], coords[j], coords[k]) that extract_texmesh evaluates
+ * (inference.py:106-116: linspace / meshgrid(indexing='ij') points in 8192-point chunks, reshape(R,R,R)), without materialising the
+ * points: grid_out device fp32 [R,R,R], grid_out[i,j,k] = sdf at (x, y, z) = (coords[i], coords[j], coords[k]); coords device fp32 [R]
+ * (the caller's linspace).  Bit-identical to column 0 of tpx_primsdf_query_grid / tpx_primsdf_query on those points.  grid_ws as for
+ * tpx_primsdf_query_grid (built from the same srt), or NULL for the exhaustive loop. */
+int tpx_primsdf_sdf_grid(const float* coords_dev, int R, const float* srt_dev, const float* feat_dev, const void* grid_ws, size_t grid_bytes, int K, int S,
+                         int dim_feat, int inference, float* grid_out_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Marching cubes — the `mcubes.marching_cubes(grid, 0.0)` call of extract_texmesh (inference.py:106-124), which copies the SDF grid
+ * to the host for a CPU library.  vol device fp32 [X,Y,Z] C order, X, Y, Z >= 2, X*Y*Z < 2^31.  Output: an indexed triangle mesh with
+ * shared vertices, deterministic (no output position depends on scheduling):
+ *   inside iff value < iso (strict); one vertex per lattice edge whose ends classify differently; the edge p -> p + e_a is owned by
+ *   p; vertex ids ordered by the C-order linear index of p, then by a; position p + t e_a, t = (iso - f(p)) / (f(p+e_a) - f(p)) in
+ *   fp32, emitted as origin[d] + spacing[d] * pos[d] (component d = array axis d; origin 0 / spacing 1 = index units);
+ *   triangles ordered by the C-order linear index of the cell, then by the case table (csrc/mc_tables.cuh, generated by mc_table.py);
+ *   faces int64 [F,3]; (v1-v0) x (v2-v0) points toward increasing value (outward for an SDF that is negative inside).
+ * Lifecycle: ws = tpx_mc_workspace_bytes(X,Y,Z) bytes of 256-B aligned device memory (0 = volume too large or too small; about
+ * 6 bytes per grid point); tpx_mc_count writes counts_dev[0] = V, counts_dev[1] = F (device int64); the caller reads them back,
+ * allocates verts [V,3] fp32 and faces [F,3] int64 (NULL allowed for a zero count), and calls tpx_mc_emit on the same workspace
+ * with the same vol, X, Y, Z and iso, on the same stream.  Neither call synchronises.  If V or F is 2^31 or more, emit writes
+ * nothing; the caller must treat such counts as an error.
+ * ---------------------------------------------------------------------------------------------------------- */
+size_t tpx_mc_workspace_bytes(int64_t X, int64_t Y, int64_t Z);
+int tpx_mc_count(const float* vol_dev, int64_t X, int64_t Y, int64_t Z, float iso, void* ws, size_t ws_bytes, int64_t* counts_dev, void* stream);
+int tpx_mc_emit(const float* vol_dev, int64_t X, int64_t Y, int64_t Z, float iso, float ox, float oy, float oz, float sx, float sy, float sz, void* ws,
+                size_t ws_bytes, float* verts_dev, int64_t* faces_dev, void* stream);
 
 /* nn.GELU() (erf form) in place on an fp16 tensor of n elements (n % 8 == 0, 16-B aligned) — the activation of the DINOv2 MLP
  * (models/conditioner/dinov2/layers/mlp.py:33-39); the rest of that encoder (SURVEY.md §8f-2) is built from the entry points above. */
