@@ -9,7 +9,7 @@ import types
 
 from . import synth  # noqa: F401
 from . import _lib  # noqa: F401
-from . import diffusion, dinov2, dit, mesh, pipeline, primsdf, ray_marcher, shard, vae  # noqa: F401
+from . import bake, diffusion, dinov2, dit, mesh, pipeline, primsdf, ray_marcher, shard, vae  # noqa: F401
 from .diffusion import SpacedDiffusion, create_diffusion  # noqa: F401
 from .dit import DiT  # noqa: F401
 from .pipeline import LatentCodec, PrimXPipeline  # noqa: F401
@@ -20,14 +20,15 @@ from .vae import VAE  # noqa: F401
 __version__ = "0.1.0"
 
 
-def install(mcubes: bool = False) -> None:
+def install(mcubes: bool = False, nvdiffrast: bool = False) -> None:
     """Make the reference's import paths resolve to this implementation, so ``inference.py`` / ``app.py`` run
     unchanged:  ``models.dit_crossattn`` -> dit, ``models.vae3d_dib`` -> vae, ``models.diffusion`` -> diffusion,
     ``models.primsdf`` -> primsdf, ``models.conditioner.image_dinov2`` -> dinov2, ``dva.ray_marcher`` -> ray_marcher.
     (Equivalent to editing ``class_name`` in configs/inference_dit.yml:32,53; see INTEGRATION.md.)  If the reference's
     ``models`` package is importable it is imported first so its other members (conditioner, primsdf) keep working.
     ``mcubes=True`` also binds ``sys.modules["mcubes"]`` to a module whose ``marching_cubes`` is the GPU one of ``mesh``, so
-    extract_texmesh (inference.py:119) runs without PyMCubes; by default ``mcubes`` is left alone."""
+    extract_texmesh (inference.py:119) runs without PyMCubes; by default ``mcubes`` is left alone.  ``nvdiffrast=True`` likewise binds
+    ``sys.modules["nvdiffrast"]`` / ``["nvdiffrast.torch"]`` to the forward-only UV-space rasteriser of ``bake`` (inference.py:22,31,172-174)."""
     try:
         import models as ref_models  # the reference checkout, when it is on sys.path
     except Exception:
@@ -55,3 +56,5 @@ def install(mcubes: bool = False) -> None:
         pass
     if mcubes:
         sys.modules["mcubes"] = mesh.mcubes_module()
+    if nvdiffrast:
+        sys.modules["nvdiffrast"], sys.modules["nvdiffrast.torch"] = bake.nvdiffrast_modules()

@@ -78,6 +78,11 @@ SIGNATURES = {
     "tpx_mc_workspace_bytes": (_sz, [_i64, _i64, _i64]),
     "tpx_mc_count": (_i, [_vp, _i64, _i64, _i64, _f, _vp, _sz, _vp, _vp]),
     "tpx_mc_emit": (_i, [_vp, _i64, _i64, _i64, _f, _f, _f, _f, _f, _f, _f, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_uv_rasterize": (_i, [_vp, _i64, _vp, _i64, _i, _i, _vp, _vp, _vp]),
+    "tpx_rast_interpolate": (_i, [_vp, _i64, _i, _vp, _i64, _vp, _i, _i, _vp, _vp]),
+    "tpx_primsdf_bake": (_i, [_vp, _i, _i, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _sz, _i, _i, _i, _vp, _vp, _vp]),
+    "tpx_texture_inpaint_bytes": (_sz, [_i, _i]),
+    "tpx_texture_inpaint": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp, _vp]),
     "tpx_groupnorm_silu": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp, _vp]),
     "tpx_conv3d_k3": (_i, [_vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _i, _vp]),
 }

@@ -78,4 +78,14 @@ int launch_mc_count(const float* vol, long long X, long long Y, long long Z, flo
 int launch_mc_emit(const float* vol, long long X, long long Y, long long Z, float iso, const float origin[3], const float spacing[3], void* ws, size_t ws_bytes,
                    float* verts, long long* faces, cudaStream_t st);
 
+// primsdf.cu : fused texel query of the texture bake; feats [H,W,6] = 255 (R, G, B, 0, roughness, metallic), mask [H,W]
+int launch_primsdf_bake(const float* rast, int H, int W, const float* v, long long Nv, const int* f, long long F, const float* srt, const float* feat, const void* ws,
+                        size_t ws_bytes, int K, int S, int dim_feat, float* feats, uint8_t* mask, cudaStream_t st);
+
+// texture_bake.cu : UV-space rasteriser + attribute interpolation, nearest-texel seam padding
+int launch_uv_rasterize(const float* vt, long long Nt, const int* ft, long long F, int H, int W, float* rast, int* winner, cudaStream_t st);
+int launch_rast_interpolate(const float* attr, long long Nv, int C, const int* tri, long long F, const float* rast, int H, int W, float* out, cudaStream_t st);
+size_t texture_inpaint_bytes(int H, int W);
+int launch_texture_inpaint(float* feats, const uint8_t* mask, int H, int W, int C, int P, void* ws, size_t ws_bytes, int* src, cudaStream_t st);
+
 }  // namespace tpx

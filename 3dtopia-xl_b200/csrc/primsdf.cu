@@ -5,6 +5,7 @@
 // primitive once (box test in registers), samples only the few that cover it (trilinear, align_corners=True, from the
 // L2-resident feature volumes) and never materialises the weight matrix.  FP32 SIMT: this is gather/compare work,
 // not tensor-core work.
+#include "bake_interp.cuh"
 #include "kernels.cuh"
 
 namespace tpx {
@@ -332,6 +333,36 @@ __global__ void __launch_bounds__(PS_THREADS) primsdf_sdf_grid_kernel(const floa
     const int k = static_cast<int>(idx % R), j = static_cast<int>((idx / R) % R), i = static_cast<int>(idx / (static_cast<long long>(R) * R));
     query_point_binned<1, 6>(coords[i], coords[j], coords[k], srt, feat, hdr, offsets, entries, K, S, inference, grid + idx);
 }
+// fused texel query of the texture bake (inference.py:173-198: dr.interpolate of the positions, the masked PrimSDF.forward in 8192-point
+// chunks, the scatter through the mask, * 255): one thread per atlas texel reads its rast entry, interpolates the 3-D position with the
+// device function tpx_rast_interpolate uses, runs the 6-channel binned query forward runs (inference = 0: the nearest-primitive
+// fallback only defines the discarded sdf of uncovered points) and writes feats = 255 (R, G, B, 0, roughness, metallic) and the mask.
+__global__ void __launch_bounds__(PS_THREADS) primsdf_bake_kernel(const float4* __restrict__ rast, long long n, const float* __restrict__ v, long long Nv,
+                                                                  const int* __restrict__ f, long long F, const float* __restrict__ srt,
+                                                                  const float* __restrict__ feat, const GridHdr* __restrict__ hdr,
+                                                                  const int* __restrict__ offsets, const int* __restrict__ entries, int K, int S,
+                                                                  float* __restrict__ feats, uint8_t* __restrict__ mask) {
+    const long long p = static_cast<long long>(blockIdx.x) * PS_THREADS + threadIdx.x;
+    if (p >= n) return;
+    const float4 r = rast[p];
+    const int t = rast_triangle(r.w);
+    float o[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    uint8_t covered = 0;
+    if (t >= 0 && t < F) {
+        const long long i0 = f[3 * static_cast<long long>(t)], i1 = f[3 * static_cast<long long>(t) + 1], i2 = f[3 * static_cast<long long>(t) + 2];
+        if (i0 >= 0 && i1 >= 0 && i2 >= 0 && i0 < Nv && i1 < Nv && i2 < Nv) {
+            const float *a0 = v + 3 * i0, *a1 = v + 3 * i1, *a2 = v + 3 * i2;
+            query_point_binned<6, 6>(bary_interp(r.x, r.y, a0[0], a1[0], a2[0]), bary_interp(r.x, r.y, a0[1], a1[1], a2[1]),
+                                     bary_interp(r.x, r.y, a0[2], a1[2], a2[2]), srt, feat, hdr, offsets, entries, K, S, 0, o);
+            covered = 1;
+        }
+    }
+    float* out = feats + p * 6;
+    out[0] = __fmul_rn(o[1], 255.f); out[1] = __fmul_rn(o[2], 255.f); out[2] = __fmul_rn(o[3], 255.f);
+    out[3] = 0.f;
+    out[4] = __fmul_rn(o[4], 255.f); out[5] = __fmul_rn(o[5], 255.f);
+    mask[p] = covered;
+}
 }  // namespace
 
 int launch_primsdf_query(const float* x, const float* srt, const float* feat, long long n, int K, int S, int dim_feat, int inference, float* out,
@@ -417,6 +448,22 @@ int launch_primsdf_sdf_grid(const float* coords, int R, const float* srt, const 
     ProfScope prof(PROF_VAE_MISC, st);
     const long long blocks = (static_cast<long long>(R) * R * R + PS_THREADS - 1) / PS_THREADS;
     primsdf_sdf_grid_kernel<<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(coords, R, srt, feat, g.hdr, g.offsets, g.entries, K, S, inference, grid);
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+int launch_primsdf_bake(const float* rast, int H, int W, const float* v, long long Nv, const int* f, long long F, const float* srt, const float* feat, const void* ws,
+                        size_t ws_bytes, int K, int S, int dim_feat, float* feats, uint8_t* mask, cudaStream_t st) {
+    TPX_CHECK(dim_feat == 6, TPX_ERR_SHAPE, "primsdf_bake: dim_feat %d (kernel covers the released 6-channel layout)", dim_feat);
+    TPX_CHECK(S >= 2 && S <= 32 && K >= 0 && (K > 0 || ws == nullptr), TPX_ERR_SHAPE, "primsdf_bake: bad primitive geometry (S %d, K %d)", S, K);
+    TPX_CHECK(H >= 1 && W >= 1 && H <= 8192 && W <= 8192 && F >= 0 && Nv >= 0, TPX_ERR_SHAPE, "primsdf_bake: atlas %d x %d (1..8192 each), F %lld, Nv %lld", H, W, F, Nv);
+    TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0 && (reinterpret_cast<uintptr_t>(rast) & 15) == 0, TPX_ERR_ARG, "primsdf_bake: srt and rast must be 16-B aligned");
+    GridPtrs g{nullptr, nullptr, nullptr, nullptr, 0};
+    if (ws != nullptr) g = grid_carve(const_cast<void*>(ws), ws_bytes);
+    ProfScope prof(PROF_VAE_MISC, st);
+    const long long n = static_cast<long long>(H) * W;
+    primsdf_bake_kernel<<<static_cast<unsigned>((n + PS_THREADS - 1) / PS_THREADS), PS_THREADS, 0, st>>>(reinterpret_cast<const float4*>(rast), n, v, Nv, f, F, srt, feat, g.hdr,
+                                                                                                       g.offsets, g.entries, K, S, feats, mask);
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }

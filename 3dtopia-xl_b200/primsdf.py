@@ -12,7 +12,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from . import _lib, mesh
+from . import _lib, bake, mesh
 
 
 class PrimSDF(nn.Module):
@@ -98,6 +98,42 @@ class PrimSDF(nn.Module):
         grid = self.sdf_grid(R, bound)
         step = 2.0 * bound / (R - 1)
         return mesh._mesh(grid, isovalue, origin=(-bound,) * 3, spacing=(step,) * 3)
+
+    def bake_texture(self, v, f, vt, ft, resolution=1024, pad: int = 32):
+        """Texture atlas of the colour / material channels over a UV-unwrapped mesh, on the GPU: inference.py:163-211 in one call
+        (rasterise the UV layout, interpolate the 3-D position of every covered texel, query this field there, pad the seams).
+        ``v`` [Nv,3] / ``f`` [F,3] are the mesh, ``vt`` [Nt,2] in [0,1] / ``ft`` [F,3] its UV layout (``f`` and ``ft`` index different
+        vertex arrays), as inference.py:161-162 hold them after either unwrap branch; ``resolution`` is an int or (h, w).
+        Returns (feats fp32 [h,w,6] = 255 * (R, G, B, 0, roughness, metallic), mask bool [h,w] of the covered texels) on the module's
+        device; row 0 is v = 0.  feats / 255 at a covered texel is bit-identical to ``forward`` at the position ``bake.interpolate``
+        gives for it; ``pad`` = 0 leaves the uncovered texels zero."""
+        h, w = (resolution, resolution) if isinstance(resolution, int) else resolution
+        h, w = bake._size(h, w)
+        bake._check_rows(v, 3, "v")
+        bake._check_rows(vt, 2, "vt")
+        bake._check_triangles(f, "f")
+        bake._check_triangles(ft, "ft")
+        if f.shape[0] != ft.shape[0]:
+            raise ValueError(f"f and ft must list the same triangles, got {f.shape[0]} and {ft.shape[0]}")
+        if not self.srt_param.is_cuda:
+            raise _lib.TpxError("PrimSDF query runs on CUDA only (no CPU path): move the module to the GPU")
+        lib = _lib.lib()
+        dev = self.srt_param.device
+        v, vt = v.detach().float().contiguous().to(dev), vt.detach().float().contiguous().to(dev)
+        f, ft = bake._narrow(f.to(dev), "f"), bake._narrow(ft.to(dev), "ft")
+        srt = self.srt_param.detach().float().contiguous()
+        feat = self.feat_param.detach().float().contiguous()
+        K = srt.shape[0]
+        feats = torch.empty(h, w, 6, dtype=torch.float32, device=dev)
+        mask = torch.empty(h, w, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            rast, _ = bake._rasterize(vt, ft, h, w)
+            ws = self._grid_workspace(srt, K, dev) if 1 <= K <= 4096 else None
+            _lib.check(lib.tpx_primsdf_bake(rast.data_ptr(), h, w, v.data_ptr(), v.shape[0], f.data_ptr(), f.shape[0], srt.data_ptr(), feat.data_ptr(),
+                                            _lib.ptr(ws), 0 if ws is None else ws.numel(), K, self.prim_shape, self.dim_feat, feats.data_ptr(),
+                                            mask.data_ptr(), _lib.stream_ptr()), "tpx_primsdf_bake")
+            bake.inpaint(feats, mask, pad)
+        return feats, mask.view(torch.bool)
 
     def sdf2alpha(self, sdf):
         return torch.exp(-(sdf / self.sdf2alpha_var) ** 2)

@@ -139,3 +139,19 @@ def synth_inputs(B: int, N: int, Cin: int, M: int, Dc: int, seed: int = 42):
     x = torch.from_numpy(rs.standard_normal(size=(B, N, Cin)).astype(np.float32))
     y = torch.from_numpy(rs.standard_normal(size=(B, M, Dc)).astype(np.float32))
     return x, y
+
+
+def cell_atlas(num_faces: int, seed: int = 0, fill: float = 0.9):
+    """A seeded UV layout with one atlas cell per triangle (no unwrapper runs offline): the unit square is cut into ceil(sqrt(F))^2
+    cells and triangle t takes the lower-left half of cell t, each corner jittered inward by up to a tenth of the cell (about a
+    third of the atlas ends up covered).  Returns (vt fp32 [3F,2], ft int32 [F,3]) in the per-corner layout extract_texmesh's
+    fast-unwrap branch produces (inference.py:144-150)."""
+    n = max(int(math.ceil(math.sqrt(max(num_faces, 1)))), 1)
+    g = torch.Generator().manual_seed(seed)
+    t = torch.arange(num_faces)
+    origin = torch.stack([(t % n).float(), (t // n).float()], 1)[:, None, :]
+    corners = torch.tensor([[0.0, 0.0], [1.0, 0.0], [0.0, 1.0]])
+    inward = torch.tensor([[1.0, 1.0], [-1.0, 1.0], [1.0, -1.0]])
+    local = corners[None] + 0.1 * inward[None] * torch.rand(num_faces, 3, 2, generator=g)
+    vt = (origin + (1.0 - fill) / 2 + fill * local) / n
+    return vt.reshape(-1, 2).contiguous(), torch.arange(3 * num_faces, dtype=torch.int32).reshape(-1, 3)

@@ -253,6 +253,42 @@ int tpx_mc_count(const float* vol_dev, int64_t X, int64_t Y, int64_t Z, float is
 int tpx_mc_emit(const float* vol_dev, int64_t X, int64_t Y, int64_t Z, float iso, float ox, float oy, float oz, float sx, float sy, float sz, void* ws,
                 size_t ws_bytes, float* verts_dev, int64_t* faces_dev, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Texture bake — the back half of extract_texmesh (inference.py:163-211), device-resident.  All tensors contiguous, row-major;
+ * atlas H, W in 1..8192; index tensors int32.
+ *
+ * tpx_uv_rasterize stands behind dr.rasterize as called at inference.py:163-172 (positions (2 uv - 1, 0, 1), i.e. a UV-space
+ * rasterisation; nvdiffrast is a third-party extension that cannot be run here, so the contract is fixed below rather than
+ * measured).  vt device fp32 [Nt,2] in [0,1], ft device int32 [F,3] (F < 2^24: rast carries the id as a float), outputs
+ * rast device fp32 [H,W,4] = (u, v, 0, triangle_id + 1), zeros where nothing covers, and winner device int32 [H,W] = triangle_id or -1.
+ *   texel (row i, col j) is sampled at its centre ((j + 1/2) / W, (i + 1/2) / H) in uv: row 0 is v = 0, nvdiffrast's bottom-up rows;
+ *   a triangle covers a texel iff its three edge functions, oriented by the sign of its area, are >= 0 there (edges inclusive, both
+ *   windings, zero-area triangles and triangles with an index outside [0, Nt) skipped); an edge is evaluated identically for the
+ *   two triangles sharing it, so a shared edge leaves no hole; where several triangles cover a texel the lowest index wins;
+ *   (u, v) are the barycentric weights of vertices 0 and 1.  Deterministic: repeated calls give identical bits.
+ * tpx_rast_interpolate stands behind dr.interpolate (inference.py:173-174): out device fp32 [H,W,C] =
+ * u attr[tri[t,0]] + v attr[tri[t,1]] + (1 - u - v) attr[tri[t,2]] with t = rast[...,3] - 1; zeros where rast[...,3] == 0 or an index
+ * is outside [0, Nv).  attr device fp32 [Nv,C], tri device int32 [F,3] (may index a different vertex array than ft did).
+ * ---------------------------------------------------------------------------------------------------------- */
+int tpx_uv_rasterize(const float* vt_dev, int64_t Nt, const int32_t* ft_dev, int64_t F, int H, int W, float* rast_dev, int32_t* winner_dev, void* stream);
+int tpx_rast_interpolate(const float* attr_dev, int64_t Nv, int C, const int32_t* tri_dev, int64_t F, const float* rast_dev, int H, int W, float* out_dev,
+                         void* stream);
+/* The masked query of inference.py:173-198 in one launch: per texel of rast, the 3-D position interpolated from v device fp32 [Nv,3] /
+ * f device int32 [F,3] exactly as tpx_rast_interpolate computes it, the 6-channel grid-binned PrimSDF query (srt, feat, grid_ws, K, S,
+ * dim_feat as for tpx_primsdf_sdf_grid; grid_ws NULL = exhaustive loop), feats_dev fp32 [H,W,6] = 255 * (R, G, B, 0, roughness, metallic)
+ * and mask_dev uint8 [H,W] = 1 where a triangle covers the texel; uncovered texels get zeros.  feats / 255 is bit-identical to the
+ * tex / mat columns of tpx_primsdf_query_grid at those positions. */
+int tpx_primsdf_bake(const float* rast_dev, int H, int W, const float* v_dev, int64_t Nv, const int32_t* f_dev, int64_t F, const float* srt_dev,
+                     const float* feat_dev, const void* grid_ws, size_t grid_bytes, int K, int S, int dim_feat, float* feats_dev, uint8_t* mask_dev,
+                     void* stream);
+/* Seam padding (inference.py:200-211: binary_dilation x pad, binary_erosion x 3, kd-tree nearest neighbour, all on the host there):
+ * in place on feats_dev fp32 [H,W,C], every texel outside mask_dev (uint8 [H,W], non-zero = inside) whose 4-connected distance to the mask
+ * is <= pad (0..8192) takes the value of the Euclidean-nearest mask texel, the smallest (row, col) among equidistant ones; all other
+ * texels are untouched.  Exact (integer distances), deterministic.  src_dev (NULL allowed) int32 [H,W] receives the flat index of the
+ * source texel, -1 where nothing was written.  ws: tpx_texture_inpaint_bytes(H, W) bytes of device scratch. */
+size_t tpx_texture_inpaint_bytes(int H, int W);
+int tpx_texture_inpaint(float* feats_dev, const uint8_t* mask_dev, int H, int W, int C, int pad, void* ws, size_t ws_bytes, int32_t* src_dev, void* stream);
+
 /* nn.GELU() (erf form) in place on an fp16 tensor of n elements (n % 8 == 0, 16-B aligned) — the activation of the DINOv2 MLP
  * (models/conditioner/dinov2/layers/mlp.py:33-39); the rest of that encoder (SURVEY.md §8f-2) is built from the entry points above. */
 int tpx_gelu_erf(void* x_f16, int64_t n, void* stream);
