@@ -141,21 +141,6 @@ void build_required(tpx_dit* h) {
     h->seen.assign(r.size(), 0);
 }
 
-// tile width: minimise waves x BN over {128,256} (the widths whose consumer halves are whole 64-column bulk stores); ties go to
-// the wider tile (less operand re-read)
-int pick_bn(int M, int N) {
-    const int sms = gemm_num_sms();
-    const int tm = (M + 127) / 128;
-    int best = 128;
-    long best_cost = -1;
-    for (int bn : {128, 256}) {
-        const long tiles = static_cast<long>(tm) * ((N + bn - 1) / bn);
-        const long cost = ((tiles + sms - 1) / sms) * bn;
-        if (best_cost < 0 || cost < best_cost || (cost == best_cost && bn > best)) { best = bn; best_cost = cost; }
-    }
-    return best;
-}
-
 struct DitWs {
     float* xres;
     __half *h16, *q, *k, *v, *ao, *hid, *mod, *ts16, *fin;
@@ -215,7 +200,7 @@ int gemm_linear(const __half* A, int lda, const __half* W, int M, int N, int K, 
     p.A = A; p.a_mode = AMODE_LINEAR; p.lda = lda; p.W = W; p.M = M; p.N = N; p.K = K;
     p.epi = epi; p.args = args;
     TPX_CHECK(tile_n >= 0, TPX_ERR_ARG, "gemm: tile width %d (0 = automatic, or one of the instantiated widths)", tile_n);
-    p.BN = tile_n > 0 ? tile_n : pick_bn(M, N);
+    p.BN = tile_n > 0 ? tile_n : gemm_pick_bn(p);
     return launch_gemm(p, st);
 }
 }  // namespace

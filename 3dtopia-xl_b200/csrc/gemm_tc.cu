@@ -189,14 +189,36 @@ int make_tensor_map_2d(const void* ptr, long long rows, long long cols, long lon
     return map_2d(ptr, rows, cols, ld, box_rows, box_cols, out);
 }
 
+// The geometry the 24-column head-split bulk stores need at tile width bn (EPI_HEADS with heads_tma requested).
+static bool heads_bulk_ok(const GemmProblem& p, const GemmArgs& a, int bn) {
+    return p.epi == EPI_HEADS && a.heads_tma != 0 && p.a_mode == AMODE_LINEAR && gemm_wn(bn, p.a_mode) % 24 == 0 && p.N % bn == 0 && a.Dh % 24 == 0 &&
+           a.split_cols % 24 == 0 && a.Nseq % 32 == 0 && a.Nseq > 0 && p.M % a.Nseq == 0 && a.DhP % 8 == 0 && (a.vt_which_plus1 == 0 || a.vt_ld % 8 == 0);
+}
+
+// Automatic tile width of a linear GEMM: minimise rounds x width over the ping-pong widths {128, 144}, rounds = ceil(tiles / SMs), so
+// the last round leaves few SMs idle; 144 (two 72-wide heads, divides 1152 / 3456 / 4608) only where its epilogue is a bulk one (gated
+// residual; head split in 24-column groups).  Ties go to 144 (fewer tiles: less operand re-read).
+int gemm_pick_bn(const GemmProblem& p) {
+    const long sms = gemm_num_sms();
+    const long tm = (p.M + 127) / 128;
+    int best = 128;
+    long best_cost = -1;
+    for (int bn : {128, 144}) {
+        if (bn == 144 && !gemm_tma_epilogue(p.epi, bn) && !heads_bulk_ok(p, p.args, bn)) continue;
+        const long tiles = tm * ((p.N + bn - 1) / bn);
+        const long cost = ((tiles + sms - 1) / sms) * bn;
+        if (best_cost < 0 || cost <= best_cost) { best = bn; best_cost = cost; }
+    }
+    return best;
+}
+
 // Output tensor maps of the bulk-store epilogues (tc / td / te default to copies of the A map when unused).  Validates the geometry the
 // 24-column head-split stores need and clears a.heads_tma when it does not hold (the kernel then takes the per-thread path).
 static int make_output_maps(const GemmProblem& p, GemmArgs& a, const CUtensorMap& ta, CUtensorMap& tc, CUtensorMap& td, CUtensorMap& te) {
     int rc = TPX_OK;
     tc = ta; td = ta; te = ta;
     if (p.epi == EPI_HEADS && a.heads_tma != 0) {
-        const bool ok = p.a_mode == AMODE_LINEAR && gemm_wn(p.BN) % 24 == 0 && p.N % p.BN == 0 && a.Dh % 24 == 0 && a.split_cols % 24 == 0 && a.Nseq % 32 == 0 &&
-                        a.Nseq > 0 && p.M % a.Nseq == 0 && a.DhP % 8 == 0 && (a.vt_which_plus1 == 0 || a.vt_ld % 8 == 0);
+        const bool ok = heads_bulk_ok(p, a, p.BN);
         a.heads_tma = ok ? 1 : 0;
         if (ok) {
             const long long rows = static_cast<long long>(p.M / a.Nseq) * a.H * a.Nseq, rows_t = static_cast<long long>(p.M / a.Nseq) * a.H * a.DhP;
@@ -213,11 +235,13 @@ static int make_output_maps(const GemmProblem& p, GemmArgs& a, const CUtensorMap
     } else {
         a.heads_tma = 0;
     }
-    if (gemm_tma_epilogue(p.epi, gemm_wn(p.BN))) {
-        // fp16 [M, N] in 64-column x 32-row boxes, or the fp32 residual in 32 x 32 boxes
+    const int wn = gemm_wn(p.BN, p.a_mode);
+    if (gemm_tma_epilogue(p.epi, wn)) {
+        // fp16 [M, N] in 64-column x 32-row boxes, or the fp32 residual in 32 x 32 boxes (+ 16 x 32 for the last 16 columns of a 144 tile)
         if (p.epi == EPI_GATED) {
             TPX_CHECK(a.xres != nullptr && a.gate != nullptr, TPX_ERR_ARG, "gemm: gated epilogue without residual / gate");
             rc = map_2d(a.xres, p.M, p.N, a.ldx, 32, 32, &tc, 4);
+            if (rc == TPX_OK && wn % 32 != 0) rc = map_2d(a.xres, p.M, p.N, a.ldx, 32, 16, &td, 4);
         } else if (a.convt_store != 0) {
             // out0 already points at the (a,b,c) corner of the [P, 8, 8, 8, N] volume: the stride-2 sub-lattice as a 5-D tensor
             TPX_CHECK(a.out0 != nullptr && p.M % 64 == 0 && p.epi == EPI_STORE, TPX_ERR_ARG, "gemm: transposed-conv store needs EPI_STORE and M = P * 64");
@@ -236,16 +260,18 @@ static int make_output_maps(const GemmProblem& p, GemmArgs& a, const CUtensorMap
 template <int BN, int BK, int AMODE, int EPI>
 static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& td, const CUtensorMap& te, const GemmArgs& a,
                       cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, BK>;
+    using Cfg = GemmCfg<BN, BK, AMODE>;
+    GemmArgs ka = a;
+    ka.tiles_n = (a.N + BN - 1) / BN;
+    ka.num_tiles = ((a.M + 127) / 128) * ka.tiles_n;
     auto kern = gemm_tc_kernel<BN, BK, AMODE, EPI>;
     static bool attr_set = false;
     if (!attr_set) {
         TPX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         attr_set = true;
     }
-    const int tiles = ((a.M + 127) / 128) * ((a.N + BN - 1) / BN);
-    const int grid = tiles < gemm_num_sms() ? tiles : gemm_num_sms();
-    TPX_CUDA(launch_pdl(kern, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, ta, tb, tc, td, te, a));
+    const int grid = ka.num_tiles < gemm_num_sms() ? ka.num_tiles : gemm_num_sms();
+    TPX_CUDA(launch_pdl(kern, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, ta, tb, tc, td, te, ka));
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }
@@ -277,16 +303,18 @@ int launch_gemm(const GemmProblem& p, cudaStream_t stream) {
     CUtensorMap tc, td, te;
     rc = make_output_maps(p, a, ta, tc, td, te);
     if (rc != TPX_OK) return rc;
-    TPX_CHECK(p.BN != 144 || a.heads_tma != 0, TPX_ERR_SHAPE, "gemm: the 144-wide tile exists for the bulk-store head split only");
 
 #define TPX_CASE(BN_, BK_, AM_, EP_) \
     if (p.BN == BN_ && bk == BK_ && p.a_mode == AM_ && p.epi == EP_) return launch_one<BN_, BK_, AM_, EP_>(ta, tb, tc, td, te, a, stream);
-    // DiT (every tile width x every DiT epilogue, so any hidden size that is a multiple of 128 works)
+    // DiT (every tile width x every DiT epilogue, so any hidden size that is a multiple of 128 works); 128 / 144: ping-pong schedule
     TPX_CASE(128, 64, AMODE_LINEAR, EPI_STORE)
     TPX_CASE(128, 64, AMODE_LINEAR, EPI_GELU)
     TPX_CASE(128, 64, AMODE_LINEAR, EPI_HEADS)
     TPX_CASE(128, 64, AMODE_LINEAR, EPI_GATED)
-    TPX_CASE(144, 64, AMODE_LINEAR, EPI_HEADS)      // two 72-wide heads per tile: the N = 1152 head projections in one wave
+    TPX_CASE(144, 64, AMODE_LINEAR, EPI_STORE)
+    TPX_CASE(144, 64, AMODE_LINEAR, EPI_GELU)
+    TPX_CASE(144, 64, AMODE_LINEAR, EPI_HEADS)
+    TPX_CASE(144, 64, AMODE_LINEAR, EPI_GATED)
     TPX_CASE(192, 64, AMODE_LINEAR, EPI_STORE)
     TPX_CASE(192, 64, AMODE_LINEAR, EPI_GELU)
     TPX_CASE(192, 64, AMODE_LINEAR, EPI_HEADS)

@@ -2,13 +2,19 @@
 //
 //   warp 0          : TMA producer  (cp.async.bulk.tensor -> 128B/64B-swizzled smem ring, mbarrier complete_tx); warps 1-3 of its
 //                     warpgroup only give their registers away (setmaxnreg)
-//   warpgroups 1, 2 : consumers.  A CTA tile is 128 x BN; consumer c owns ALL 128 rows of columns [c BN/2, (c+1) BN/2) as two
-//                     wgmma m64 accumulators in registers (tiles narrower than 64 columns run on one consumer).  The two A
+//   warpgroups 1, 2 : consumers, in one of two schedules (gemm_pingpong):
+//                     ping-pong (linear GEMMs at BN 128 / 144): consumer c owns WHOLE 128 x BN tiles, the CTA's tiles j = c, c + 2, ...
+//                     The mainloops take turns through an ordered hand-off (named barriers), so one consumer's epilogue runs while
+//                     the other issues wgmma; the producer loads in tile order into the one ring and each consumer steps past the
+//                     other's k-blocks.
+//                     cooperative (every other width, and the conv GEMMs): both consumers work on every 128 x BN tile, consumer c
+//                     on columns [c BN/2, (c+1) BN/2) (tiles narrower than 64 columns run on one consumer).
+//                     Either way a consumer holds ALL 128 rows of its columns as two wgmma m64 accumulators in registers.  The two A
 //                     descriptors interleave the 8-row groups of the tile (stride 2 groups, starting at group 0 / 1), so warp q
 //                     of a consumer ends up with rows 32 q .. 32 q + 31 of the tile: the fused epilogues (bias / GELU / gated
 //                     residual / head split / conv scatter; bulk tensor stores) work on 32-row slabs, one row per thread, and
 //                     get them through a warp-private shared-memory exchange (acc_rows) with no block-wide synchronisation.
-//   The producer runs ahead into the next tile's k-blocks while the consumers are in their epilogue.
+//   The producer runs ahead into the next tile's k-blocks while a consumer is in its epilogue.
 //
 // A-operand modes: AMODE_LINEAR (2-D tensor map over a row-major [M,K] fp16 matrix) and AMODE_CONV3 (5-D tensor
 // map over a channels-last [P,S,S,S,C] fp16 volume: the 27 taps of a 3x3x3 / pad 1 convolution are 27 shifted
@@ -31,6 +37,7 @@ enum GemmAMode : int { AMODE_LINEAR = 0, AMODE_CONV3 = 1 };
 
 struct GemmArgs {
     int M, N, num_kb;
+    int tiles_n, num_tiles;   // 128 x BN tiles: per row of tiles, in all (kernel parameters, so they cost the consumers no registers)
     int conv_S, chunks_per_tap;
     const __half* bias;
     float post_scale;
@@ -53,21 +60,24 @@ struct GemmArgs {
     int heads_tma;    // EPI_HEADS: 1 = outputs leave as 24-column bulk tensor stores (launcher checked the geometry, padding is pre-zeroed)
 };
 
-constexpr int gemm_wn(int bn) { return bn >= 64 ? bn / 2 : bn; }   // columns of one consumer warpgroup
+constexpr bool gemm_pingpong(int bn, int amode) { return amode == AMODE_LINEAR && (bn == 128 || bn == 144); }
+constexpr int gemm_wn(int bn, int amode) { return gemm_pingpong(bn, amode) ? bn : (bn >= 64 ? bn / 2 : bn); }   // columns of one consumer warpgroup
+constexpr int GEMM_MAX_WN = 144;
 
-template <int BN, int BK>
+template <int BN, int BK, int AMODE>
 struct GemmCfg {
     static constexpr int BM = 128;
     static constexpr int SW = BK * 2;
+    static constexpr bool PP = gemm_pingpong(BN, AMODE);
     static constexpr int NWG = BN >= 64 ? 2 : 1;                 // consumer warpgroups
-    static constexpr int WN = gemm_wn(BN);
+    static constexpr int WN = gemm_wn(BN, AMODE);
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     // per consumer warp: one 32-row x 128-B staging buffer for the bulk stores (1024-B aligned: 128-B swizzle) and one exchange buffer
     static constexpr int STAGING_BYTES = BN >= 64 ? 8 * 4096 : 0;
     static constexpr int XCHG_BYTES = NWG * 4 * XCHG_FLOATS * 4;
-    static constexpr int TAIL_BYTES = 256 /*barriers*/ + 2048 /*bias + gate tile, fp32*/;
+    static constexpr int TAIL_BYTES = 256 /*barriers*/ + 4 * GEMM_MAX_WN * 4 /*bias + gate columns of both consumers, fp32*/;
     // dynamic shared memory is declared __align__(1024) (the kernel traps if the base is not), so no alignment slack is budgeted
     static constexpr int STAGES_RAW = (227 * 1024 - STAGING_BYTES - XCHG_BYTES - TAIL_BYTES) / STAGE_BYTES;
     static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
@@ -75,7 +85,7 @@ struct GemmCfg {
     static constexpr int THREADS = 384;
     static_assert(STAGES >= 2 && SMEM_BYTES <= 227 * 1024, "shared memory budget");
     static_assert(B_BYTES % 1024 == 0 && A_BYTES % 1024 == 0, "stage operands must stay 1024-B aligned");
-    static_assert(WN % 8 == 0 && WN <= 128 && (WN * SW) % 1024 == 0, "consumer tile: wgmma N, accumulator registers, swizzle alignment");
+    static_assert(WN % 8 == 0 && WN <= GEMM_MAX_WN && (WN * SW) % 1024 == 0, "consumer tile: wgmma N, accumulator registers, swizzle alignment");
 };
 
 union Pack8 {
@@ -264,10 +274,11 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, const float* __rest
 // group:
 //   fp16 outputs: 64 columns per store (cp.async.bulk.tensor, full 128-B lines instead of 16-B pieces per thread);
 //   gated residual: 32 fp32 columns per cp.reduce.async.bulk.tensor .add — the L2 performs  x += h(gate * h(acc + b)),  so the
-//   epilogue never loads the residual (one add per element per launch: deterministic; the L2 adder flushes subnormals).
+//   epilogue never loads the residual (one add per element per launch: deterministic; the L2 adder flushes subnormals).  A width
+//   of 32 k + 16 (144) ends with one 16-column reduce through its own 64-B-swizzled map.
 // Rows >= M and columns >= N are clipped by the tensor map.  wn = columns of one consumer warpgroup.
 constexpr bool gemm_tma_epilogue(int epi, int wn) {
-    return ((epi == EPI_STORE || epi == EPI_GELU) && wn % 64 == 0) || (epi == EPI_GATED && wn % 32 == 0);
+    return ((epi == EPI_STORE || epi == EPI_GELU) && wn % 64 == 0) || (epi == EPI_GATED && wn % 16 == 0 && wn >= 64);
 }
 
 __device__ __forceinline__ void staging_acquire(int lane) {
@@ -275,53 +286,68 @@ __device__ __forceinline__ void staging_acquire(int lane) {
     __syncwarp();
 }
 
-template <int EPI, int NCH, int NA>
-__device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMap* tmC, const float* __restrict__ sb, const float* __restrict__ sg,
-                                             bool gate_in_smem, const float (&accv)[2][NA], float* xb, uint32_t stg, int row0, int n0, int lane) {
-    const uint32_t dst = stg + lane * 128;
-    const int sw = lane & 7;
+// One CW-column (32 or 16) chunk of the gated residual: staged as 32 rows x CW fp32 in the tensor map's swizzle (128 B / 64 B rows:
+// conflict-free 16-B stores), then one bulk reduce-add.
+template <int CW, int NA>
+__device__ __forceinline__ void epilogue_gated_chunk(const GemmArgs& g, const CUtensorMap* tm, const float* __restrict__ sb, const float* __restrict__ sg,
+                                                     bool gate_in_smem, const float (&accv)[2][NA], float* xb, uint32_t stg, int row0, int n0, int c0,
+                                                     int lane) {
+    static_assert(CW == 32 || CW == 16, "gated chunk width");
+    const uint32_t dst = stg + lane * (CW * 4);
+    const int sw = ((lane * CW * 4) >> 7) & (CW / 4 - 1);     // the 16-B unit index bits the 128-B / 64-B swizzle XORs in
+    uint32_t acc[CW];
+    acc_rows<CW, 8, 16>(accv[0], accv[1], c0, xb, lane, acc);
+    staging_acquire(lane);
+    // a per-row gate stays packed fp16 until use (8 registers per 32 columns, not 32: the 144-wide accumulator leaves little room)
+    Pack8 gh[CW / 8];
+    if (!gate_in_smem) {
+        const int b = ((row0 + lane) / g.rows_per_batch) % g.gate_batches;
+        const __half* gp = g.gate + static_cast<size_t>(b) * g.gate_bstride + n0 + c0;
 #pragma unroll
-    for (int k = 0; k < NCH; ++k) {
-        uint32_t acc[32];
-        acc_rows<32, 8, 16>(accv[0], accv[1], k * 32, xb, lane, acc);
-        const int c0 = k * 32;
-        if constexpr (EPI == EPI_GATED) {
-            staging_acquire(lane);
-            float gt[32];
-            if (gate_in_smem) {
+        for (int j = 0; j < CW / 8; ++j) gh[j].u = (n0 + c0 + j * 8 < g.N) ? *reinterpret_cast<const uint4*>(gp + j * 8) : make_uint4(0, 0, 0, 0);
+    }
 #pragma unroll
-                for (int i = 0; i < 32; i += 4) {
-                    const float4 g4 = *reinterpret_cast<const float4*>(sg + c0 + i);
-                    gt[i] = g4.x; gt[i + 1] = g4.y; gt[i + 2] = g4.z; gt[i + 3] = g4.w;
-                }
-            } else {
-                const int b = ((row0 + lane) / g.rows_per_batch) % g.gate_batches;
-                const __half* gp = g.gate + static_cast<size_t>(b) * g.gate_bstride + n0 + c0;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    Pack8 t;
-                    t.u = (n0 + c0 + j * 8 < g.N) ? *reinterpret_cast<const uint4*>(gp + j * 8) : make_uint4(0, 0, 0, 0);
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) gt[j * 8 + i] = __half2float(t.h[i]);
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float4 b4 = *reinterpret_cast<const float4*>(sb + c0 + j * 4);
-                const float2 v01 = round_h2(__uint_as_float(acc[j * 4 + 0]) + b4.x, __uint_as_float(acc[j * 4 + 1]) + b4.y);
-                const float2 v23 = round_h2(__uint_as_float(acc[j * 4 + 2]) + b4.z, __uint_as_float(acc[j * 4 + 3]) + b4.w);
-                const float2 o01 = round_h2(gt[j * 4 + 0] * v01.x, gt[j * 4 + 1] * v01.y);
-                const float2 o23 = round_h2(gt[j * 4 + 2] * v23.x, gt[j * 4 + 3] * v23.y);
-                const float o[4] = {o01.x, o01.y, o23.x, o23.y};
-                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst + ((j ^ sw) << 4)), "f"(o[0]), "f"(o[1]), "f"(o[2]), "f"(o[3]) : "memory");
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-                tma_reduce_add_2d(tmC, stg, n0 + c0, row0);
-                bulk_commit();
-            }
+    for (int j = 0; j < CW / 4; ++j) {
+        float4 g4;
+        if (gate_in_smem) {
+            g4 = *reinterpret_cast<const float4*>(sg + c0 + j * 4);
         } else {
+            const float2 lo = __half22float2(gh[j >> 1].h2[(j & 1) * 2]), hi = __half22float2(gh[j >> 1].h2[(j & 1) * 2 + 1]);
+            g4 = make_float4(lo.x, lo.y, hi.x, hi.y);
+        }
+        const float4 b4 = *reinterpret_cast<const float4*>(sb + c0 + j * 4);
+        const float2 v01 = round_h2(__uint_as_float(acc[j * 4 + 0]) + b4.x, __uint_as_float(acc[j * 4 + 1]) + b4.y);
+        const float2 v23 = round_h2(__uint_as_float(acc[j * 4 + 2]) + b4.z, __uint_as_float(acc[j * 4 + 3]) + b4.w);
+        const float2 o01 = round_h2(g4.x * v01.x, g4.y * v01.y);
+        const float2 o23 = round_h2(g4.z * v23.x, g4.w * v23.y);
+        const float o[4] = {o01.x, o01.y, o23.x, o23.y};
+        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst + ((j ^ sw) << 4)), "f"(o[0]), "f"(o[1]), "f"(o[2]), "f"(o[3]) : "memory");
+    }
+    fence_proxy_async();
+    __syncwarp();
+    if (lane == 0) {
+        tma_reduce_add_2d(tm, stg, n0 + c0, row0);
+        bulk_commit();
+    }
+}
+
+// tmC: the fp16 output map, or the 32-column residual map; tmD: the 16-column residual map (gated widths 32 k + 16)
+template <int EPI, int WN, int NA>
+__device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMap* tmC, const CUtensorMap* tmD, const float* __restrict__ sb,
+                                             const float* __restrict__ sg, bool gate_in_smem, const float (&accv)[2][NA], float* xb, uint32_t stg,
+                                             int row0, int n0, int lane) {
+    if constexpr (EPI == EPI_GATED) {
+#pragma unroll
+        for (int k = 0; k < WN / 32; ++k) epilogue_gated_chunk<32>(g, tmC, sb, sg, gate_in_smem, accv, xb, stg, row0, n0, k * 32, lane);
+        if constexpr (WN % 32 != 0) epilogue_gated_chunk<16>(g, tmD, sb, sg, gate_in_smem, accv, xb, stg, row0, n0, WN - 16, lane);
+    } else {
+        const uint32_t dst = stg + lane * 128;
+        const int sw = lane & 7;
+#pragma unroll
+        for (int k = 0; k < WN / 32; ++k) {
+            uint32_t acc[32];
+            acc_rows<32, 8, 16>(accv[0], accv[1], k * 32, xb, lane, acc);
+            const int c0 = k * 32;
             if ((k & 1) == 0) staging_acquire(lane);
             uint32_t pk[16];
 #pragma unroll
@@ -427,19 +453,24 @@ __device__ __forceinline__ void epilogue_heads_tma(const GemmArgs& g, const CUte
 
 // named barrier of one consumer warpgroup (ids 1, 2; id 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar_sync(int cw) { asm volatile("bar.sync %0, 128;" ::"r"(cw + 1) : "memory"); }
+// ping-pong hand-off of the tensor cores (ids 3, 4): consumer cw waits on 3 + cw until the other one has issued its mainloop; every
+// arrive is matched by exactly one wait (an arrive is made only when the other consumer has a next tile)
+__device__ __forceinline__ void pp_turn_wait(int cw) { asm volatile("bar.sync %0, 256;" ::"r"(cw + 3) : "memory"); }
+__device__ __forceinline__ void pp_turn_pass(int cw) { asm volatile("bar.arrive %0, 256;" ::"r"((cw ^ 1) + 3) : "memory"); }
 
 template <int BN, int BK, int AMODE, int EPI>
 __global__ void __launch_bounds__(384, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
                const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmE, const GemmArgs g) {
-    using Cfg = GemmCfg<BN, BK>;
+    using Cfg = GemmCfg<BN, BK, AMODE>;
     constexpr int STAGES = Cfg::STAGES, WN = Cfg::WN, NWG = Cfg::NWG, SW = Cfg::SW;
+    constexpr bool kPP = Cfg::PP;
     constexpr bool kTmaEpi = gemm_tma_epilogue(EPI, WN);
     constexpr bool kHeadsTma = EPI == EPI_HEADS && WN % HG == 0 && Cfg::STAGING_BYTES > 0;   // taken when g.heads_tma is set
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw;
     if ((smem_u32(smem_raw) & 1023u) != 0) __trap();   // the swizzled operand / staging tiles need a 1024-B aligned base
-    // layout: [operand ring][epilogue staging][accumulator exchange][barriers 256 B][bias + gate tile 2 KB]
+    // layout: [operand ring][epilogue staging][accumulator exchange][barriers 256 B][bias + gate columns, 2 x 2 x GEMM_MAX_WN fp32]
     constexpr int OFF_STG = STAGES * Cfg::STAGE_BYTES;
     constexpr int OFF_XCHG = OFF_STG + Cfg::STAGING_BYTES;
     constexpr int OFF_BAR = OFF_XCHG + Cfg::XCHG_BYTES;
@@ -453,11 +484,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         if constexpr (kTmaEpi) tma_prefetch_desc(&tmC);
+        if constexpr (kTmaEpi && EPI == EPI_GATED && WN % 32 != 0) tma_prefetch_desc(&tmD);
     }
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], NWG * 4);   // one lane of every consumer warp
+            mbar_init(&empty_bar[s], kPP ? 4 : NWG * 4);   // one lane of every warp of the consumer(s) reading the stage
         }
         fence_barrier_init();
         fence_proxy_async();
@@ -466,9 +498,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     pdl_launch_dependents();   // the next kernel of the stream may start its own prologue
     pdl_wait();                // ... and ours ends here: the operands written by the previous kernel are now visible
 
-    const int tiles_n = (g.N + BN - 1) / BN;
-    const int tiles_m = (g.M + 127) / 128;
-    const int num_tiles = tiles_m * tiles_n;
+    const int tiles_n = g.tiles_n;
+    const int num_tiles = g.num_tiles;
     const int num_kb = g.num_kb;
 
     if (warp < 4) {
@@ -508,18 +539,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (cw < NWG) {
             const int quad = warp & 3;           // rows 32 quad .. 32 quad + 31 of the tile
             const int et = threadIdx.x - 128 * (cw + 1);
-            float* s_bias = reinterpret_cast<float*>(smem + OFF_BAR + 256) + cw * 128;
-            float* s_gate = s_bias + 256;
+            float* s_bias = reinterpret_cast<float*>(smem + OFF_BAR + 256) + cw * GEMM_MAX_WN;
+            float* s_gate = s_bias + 2 * GEMM_MAX_WN;
             float* xb = reinterpret_cast<float*>(smem + OFF_XCHG) + (cw * 4 + quad) * XCHG_FLOATS;
             const uint32_t stg = smem_u32(smem) + OFF_STG + (cw * 4 + quad) * 4096;
             const uint32_t smem_u = smem_u32(smem);
             const bool gate_in_smem = (EPI == EPI_GATED) && (g.rows_per_batch % 128 == 0);
             float acc[2][WN / 2];
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            // the CTA's tiles are j = 0, 1, ... (tile blockIdx.x + j gridDim.x); ping-pong: this consumer takes every other one
+            for (int j = kPP ? cw : 0;; j += kPP ? 2 : 1) {
+                const int tile = blockIdx.x + j * gridDim.x;
+                if (tile >= num_tiles) break;
                 const int m_blk = tile / tiles_n, n_blk = tile - m_blk * tiles_n;
-                const int n0 = n_blk * BN + cw * WN;
+                const int n0 = n_blk * BN + (kPP ? 0 : cw * WN);
+                // the producer fills the ring in tile order: tile j's k-blocks are ring slots j num_kb, j num_kb + 1, ...
+                const uint32_t slot0 = static_cast<uint32_t>(j) * static_cast<uint32_t>(num_kb);
+                int stage = static_cast<int>(slot0 % STAGES);
+                uint32_t phase = (slot0 / STAGES) & 1u;
                 // stage this warpgroup's bias (and gate) columns; they are read after the main loop
                 wg_bar_sync(cw);
                 for (int c = et; c < WN; c += 128) {
@@ -532,12 +568,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         }
                     }
                 }
+                if constexpr (kPP) {
+                    if (j > 0) pp_turn_wait(cw);   // tile j - 1 (the other consumer's) has all its wgmma issued
+                }
                 int prev = -1;
                 for (int kb = 0; kb < num_kb; ++kb) {
                     mbar_wait(&full_bar[stage], phase);
                     const uint32_t a_addr = smem_u + stage * Cfg::STAGE_BYTES;
                     const uint64_t da0 = wgmma_desc_kmajor<SW>(a_addr, 2 * SW * 8), da1 = wgmma_desc_kmajor<SW>(a_addr + SW * 8, 2 * SW * 8);
-                    const uint64_t db = wgmma_desc_kmajor<SW>(a_addr + Cfg::A_BYTES + cw * WN * SW);
+                    const uint64_t db = wgmma_desc_kmajor<SW>(a_addr + Cfg::A_BYTES + (kPP ? 0 : cw * WN * SW));
                     wgmma_fence();
 #pragma unroll
                     for (int k = 0; k < BK / 16; ++k) {
@@ -551,6 +590,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     }
                     prev = stage;
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
+                if constexpr (kPP) {
+                    if (tile + static_cast<int>(gridDim.x) < num_tiles) pp_turn_pass(cw);   // the other consumer's tile j + 1 may start
                 }
                 wgmma_wait<0>();
                 if (lane == 0) mbar_arrive(&empty_bar[prev]);
@@ -567,9 +609,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     }
                 }
                 if constexpr (kTmaEpi) {
-                    epilogue_tma<EPI, WN / 32>(g, &tmC, s_bias, s_gate, gate_in_smem, acc, xb, stg, row0, n0, lane);
+                    epilogue_tma<EPI, WN>(g, &tmC, &tmD, s_bias, s_gate, gate_in_smem, acc, xb, stg, row0, n0, lane);
                 } else if (!done) {
-                    constexpr int CH = WN >= 32 ? 32 : 16;
+                    constexpr int CH = WN % 32 == 0 ? 32 : 16;
                     if constexpr (WN % CH == 0) {
                         const int row = row0 + lane;
                         const bool row_ok = row < g.M;
@@ -610,11 +652,12 @@ struct GemmProblem {
     // W operand [N, K] row-major fp16 (K-major)
     const __half* W;
     int M, N, K;
-    int BN;             // tile N (128/144/192/256/32/16); BK chosen from K (64, or 32 when conv_C == 32)
+    int BN;             // tile N (128/144/192/256/32/16; linear 128 / 144 run the ping-pong schedule); BK chosen from K (64, or 32 when conv_C == 32)
     int epi;
-    GemmArgs args;      // epilogue fields (M,N,num_kb filled by the launcher)
+    GemmArgs args;      // epilogue fields (M, N, num_kb and the tile counts filled by the launcher)
 };
 int launch_gemm(const GemmProblem& p, cudaStream_t stream);
+int gemm_pick_bn(const GemmProblem& p);
 int gemm_num_sms();
 
 }  // namespace tpx

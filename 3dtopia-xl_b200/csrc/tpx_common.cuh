@@ -187,7 +187,7 @@ __device__ __forceinline__ uint64_t wgmma_desc_kmajor(uint32_t smem_addr, uint32
     return d;
 }
 
-// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T.  d: this thread's N/2 accumulator registers (row lane/4 (+8) of the warp's 16 rows,
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T  (N in {8, 16, 32, 64, 128, 144} for _ss).  d: this thread's N/2 accumulator registers (row lane/4 (+8) of the warp's 16 rows,
 // columns 8 j + 2 (lane%4) (+1) for d[4 j .. 4 j + 3]); scale_d = 0 overwrites D.  _ss: A and B from shared memory;
 // _rs: A from registers (the m64k16 fragment: a[0], a[2] row lane/4, a[1], a[3] row lane/4 + 8; k = 2 (lane%4) (+8)).
 template <int N>
@@ -235,6 +235,14 @@ __device__ __forceinline__ void wgmma_ss<128>(float* d, uint64_t da, uint64_t db
         : "l"(da), "l"(db), "r"(scale_d));
 }
 template <>
+__device__ __forceinline__ void wgmma_ss<144>(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n144k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, %72, %73, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+template <>
 __device__ __forceinline__ void wgmma_rs<16>(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
@@ -251,12 +259,12 @@ __device__ __forceinline__ void wgmma_rs<64>(float* d, const uint32_t* a, uint64
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
 }
 
-// A 64 x N product for any N that is a multiple of 8, as the widest instructions that tile it; the B descriptor advances by
-// n rows of b_row_bytes (n stays a multiple of 8, so every piece starts on an 8-row group).
+// A 64 x N product for any N that is a multiple of 8, as the widest instructions that tile it (144 is one instruction); the B
+// descriptor advances by n rows of b_row_bytes (n stays a multiple of 8, so every piece starts on an 8-row group).
 template <int N>
 __device__ __forceinline__ void wgmma_ss_n(float* d, uint64_t da, uint64_t db, uint32_t scale_d, uint32_t b_row_bytes) {
     static_assert(N % 8 == 0 && N > 0 && N <= 256, "wgmma N");
-    constexpr int W = N >= 128 ? 128 : N >= 64 ? 64 : N >= 32 ? 32 : N >= 16 ? 16 : 8;
+    constexpr int W = N == 144 ? 144 : N >= 128 ? 128 : N >= 64 ? 64 : N >= 32 ? 32 : N >= 16 ? 16 : 8;
     wgmma_ss<W>(d, da, db, scale_d);
     if constexpr (N > W) wgmma_ss_n<N - W>(d + W / 2, da, db + ((W * b_row_bytes) >> 4), scale_d, b_row_bytes);
 }
