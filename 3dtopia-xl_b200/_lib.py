@@ -78,6 +78,12 @@ SIGNATURES = {
     "tpx_mc_workspace_bytes": (_sz, [_i64, _i64, _i64]),
     "tpx_mc_count": (_i, [_vp, _i64, _i64, _i64, _f, _vp, _sz, _vp, _vp]),
     "tpx_mc_emit": (_i, [_vp, _i64, _i64, _i64, _f, _f, _f, _f, _f, _f, _f, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_mesh_components_workspace_bytes": (_sz, [_i64, _i64]),
+    "tpx_mesh_components_count": (_i, [_vp, _i64, _vp, _i64, _i64, C.c_double, _vp, _sz, _vp, _vp]),
+    "tpx_mesh_components_emit": (_i, [_vp, _i64, _i64, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_decimate_workspace_bytes": (_sz, [_i64, _i64]),
+    "tpx_decimate": (_i, [_vp, _i64, _vp, _i64, _i64, _vp, _sz, _vp, _vp, _i64, _vp]),
+    "tpx_decimate_emit": (_i, [_i64, _i64, _vp, _sz, _vp, _vp, _vp]),
     "tpx_uv_rasterize": (_i, [_vp, _i64, _vp, _i64, _i, _i, _vp, _vp, _vp]),
     "tpx_rast_interpolate": (_i, [_vp, _i64, _i, _vp, _i64, _vp, _i, _i, _vp, _vp]),
     "tpx_primsdf_bake": (_i, [_vp, _i, _i, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _sz, _i, _i, _i, _vp, _vp, _vp]),

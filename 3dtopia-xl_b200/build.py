@@ -17,10 +17,12 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libtpx_b200.so")
-SOURCES = ["gemm_tc.cu", "elementwise.cu", "attention.cu", "attention_tc.cu", "vae_kernels.cu", "conv_halo.cu", "primsdf.cu", "marching_cubes.cu", "texture_bake.cu", "raymarch.cu", "conditioner.cu", "dit.cu", "vae.cu"]
+SOURCES = ["gemm_tc.cu", "elementwise.cu", "attention.cu", "attention_tc.cu", "vae_kernels.cu", "conv_halo.cu", "primsdf.cu", "marching_cubes.cu", "texture_bake.cu", "mesh_simplify.cu", "raymarch.cu", "conditioner.cu", "dit.cu", "vae.cu"]
 HEADERS = ["tpx_common.cuh", "gemm_tc.cuh", "kernels.cuh", "mc_tables.cuh", "bake_interp.cuh", os.path.join("..", "..", "include", "tpx.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr"]
+# per-file extras: the decimation's fp64 arithmetic must equal its numpy oracle operation for operation, so no contraction into FMA
+FILE_FLAGS = {"mesh_simplify.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:
@@ -48,7 +50,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     def compile_one(job):
         s, o = job
-        cmd = [nvcc, *NVCC_FLAGS, "-c", s, "-o", o]
+        cmd = [nvcc, *NVCC_FLAGS, *FILE_FLAGS.get(os.path.basename(s), []), "-c", s, "-o", o]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed for {s}:\n{r.stdout}\n{r.stderr}")

@@ -1,0 +1,902 @@
+// Mesh clean-up and decimation (DESIGN.md §1 f-7): the GPU stand-in for the pymeshlab calls extract_texmesh makes between marching
+// cubes and the unwrap (inference.py:126-129, utils/meshutils.py:63-193):
+//   * remove_small_components — clean_mesh's remove_connected_component_by_face_number(min_f) / ..._by_diameter(min_d):
+//     (a) faces -> int32, index checks; half-edge keys (min << 32 | max, face) sorted; (b) union-find over faces that share a key,
+//     always hooking the larger root under the smaller, so each root is its component's smallest face id whatever the schedule;
+//     (c) per-root face count and box (atomicMin / atomicMax on order-preserving ints), whole-mesh box; (d) keep flags, scans.
+//   * decimate — quadric edge collapse in rounds of independent collapses; every round: corner keys (vertex << 32 | face) and
+//     half-edge keys sorted, vertex CSR, frozen flags and degrees, edge list (unique keys), per-edge cost / placement / validity,
+//     two minimum passes, accept, (last round) trim to the smallest keys, collapse, remap, stable face compaction.  The host reads
+//     the accepted count back once per round.
+// Every output position comes from a sort or a prefix sum, and every atomic is a min, max or count, so results are identical across
+// calls and streams.  This file is compiled with -fmad=false (build.py) and spells its fp64 arithmetic with explicit _rn intrinsics: it
+// is the numpy test oracle's (decimate.py) operation for operation, and a contracted product would change its last bits.
+#include <cub/cub.cuh>
+
+#include "kernels.cuh"
+
+namespace tpx {
+
+namespace {
+typedef unsigned long long u64;
+constexpr int MS_THREADS = 256;
+constexpr long long MS_INDEX_LIMIT = 1LL << 31;
+constexpr u64 KEY_NONE = ~0ull;
+constexpr double SINGULAR_REL = 1e-10;
+
+size_t align256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
+
+// bump allocator over the caller's workspace; with base == nullptr it only counts bytes (the *_workspace_bytes queries)
+struct Carve {
+    uint8_t* base;
+    size_t off = 0;
+    template <class T>
+    T* take(long long n) {
+        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+        off += align256(static_cast<size_t>(n) * sizeof(T));
+        return p;
+    }
+};
+
+// CUB scratch: the onesweep radix sort needs a lookback table of a few bytes per key; the launch checks the real need against this
+size_t cub_reserve(long long n3) { return align256(static_cast<size_t>(n3) * 8 + (16u << 20)); }
+
+unsigned blocks(long long n) { return static_cast<unsigned>((n + MS_THREADS - 1) / MS_THREADS); }
+int key_bits(long long V) {
+    int b = 1;
+    while ((1LL << b) < V) ++b;
+    return 32 + b;
+}
+
+// ------------------------------------------------------------------------------------------------------------ shared kernels
+// int64 faces -> int32; bad counts faces with an index outside [0, V) or a repeated index
+__global__ void __launch_bounds__(MS_THREADS) faces_in_kernel(const long long* __restrict__ fin, long long F, long long V, int* __restrict__ T, int* bad) {
+    const long long f = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (f >= F) return;
+    const long long a = fin[3 * f], b = fin[3 * f + 1], c = fin[3 * f + 2];
+    if (a < 0 || b < 0 || c < 0 || a >= V || b >= V || c >= V || a == b || b == c || c == a) {
+        atomicAdd(bad, 1);
+        T[3 * f] = T[3 * f + 1] = T[3 * f + 2] = 0;
+        return;
+    }
+    T[3 * f] = static_cast<int>(a);
+    T[3 * f + 1] = static_cast<int>(b);
+    T[3 * f + 2] = static_cast<int>(c);
+}
+
+// half-edge keys (min << 32 | max) and, when val != nullptr, the face id of each
+__global__ void __launch_bounds__(MS_THREADS) edge_keys_kernel(const int* __restrict__ T, long long F, u64* __restrict__ key, int* __restrict__ val) {
+    const long long h = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (h >= 3 * F) return;
+    const long long f = h / 3;
+    const int k = static_cast<int>(h - 3 * f);
+    const unsigned u = static_cast<unsigned>(T[3 * f + k]), v = static_cast<unsigned>(T[3 * f + (k + 1) % 3]);
+    key[h] = (static_cast<u64>(min(u, v)) << 32) | max(u, v);
+    if (val) val[h] = static_cast<int>(f);
+}
+
+// the vertices the first F faces use (flag memset to 0 before)
+__global__ void __launch_bounds__(MS_THREADS) ref_kernel(const int* __restrict__ T, const int* __restrict__ fkeep, long long F, int* __restrict__ vref) {
+    const long long h = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (h >= 3 * F) return;
+    if (fkeep == nullptr || fkeep[h / 3]) vref[T[h]] = 1;
+}
+
+// counts[0..1] = V_out, F_out from exclusive scans and their last flags (-1, -1 when the input was malformed)
+__global__ void counts_kernel(const int* vref, const int* vpos, long long V, const int* fkeep, const int* fpos, long long F, long long F_fixed, const int* bad,
+                              long long* counts) {
+    const bool malformed = bad != nullptr && *bad != 0;
+    counts[0] = malformed ? -1 : (V ? static_cast<long long>(vpos[V - 1]) + vref[V - 1] : 0);
+    counts[1] = malformed ? -1 : (fkeep == nullptr ? F_fixed : (F ? static_cast<long long>(fpos[F - 1]) + fkeep[F - 1] : 0));
+}
+
+__global__ void __launch_bounds__(MS_THREADS) emit_verts_kernel(const float* __restrict__ P, const int* __restrict__ vref, const int* __restrict__ vpos, long long V,
+                                                                float* __restrict__ out) {
+    const long long v = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (v >= V || !vref[v]) return;
+    const long long o = vpos[v];
+    out[3 * o] = P[3 * v];
+    out[3 * o + 1] = P[3 * v + 1];
+    out[3 * o + 2] = P[3 * v + 2];
+}
+
+__global__ void __launch_bounds__(MS_THREADS) emit_faces_kernel(const int* __restrict__ T, const int* __restrict__ fkeep, const int* __restrict__ fpos,
+                                                                const long long* __restrict__ nF, long long F, const int* __restrict__ vpos, long long* __restrict__ out) {
+    const long long f = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (f >= (nF ? *nF : F)) return;
+    if (fkeep && !fkeep[f]) return;
+    const long long o = fpos ? fpos[f] : f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) out[3 * o + k] = vpos[T[3 * f + k]];
+}
+
+// ------------------------------------------------------------------------------------------------------------ component filter
+__device__ __forceinline__ int ord_f32(float x) {
+    const int b = __float_as_int(x);
+    return b >= 0 ? b : b ^ 0x7fffffff;
+}
+__device__ __forceinline__ float unord_f32(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
+
+// root of x; parent[y] <= y always, path halving on the way (races only ever store an ancestor)
+__device__ __forceinline__ int find_root(volatile int* parent, int x) {
+    int cur = parent[x];
+    if (cur != x) {
+        int next, prev = x;
+        while (cur > (next = parent[cur])) {
+            parent[prev] = next;
+            prev = cur;
+            cur = next;
+        }
+    }
+    return cur;
+}
+
+__global__ void __launch_bounds__(MS_THREADS) cc_init_kernel(long long F, int* __restrict__ parent, int* __restrict__ cnt, int* __restrict__ bmin,
+                                                             int* __restrict__ bmax) {
+    const long long f = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (f >= F) return;
+    parent[f] = static_cast<int>(f);
+    cnt[f] = 0;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) { bmin[3 * f + d] = INT_MAX; bmax[3 * f + d] = INT_MIN; }
+}
+
+// union of the faces of consecutive equal sorted keys: hook the larger root under the smaller with a CAS, retry on a lost race
+__global__ void __launch_bounds__(MS_THREADS) cc_union_kernel(const u64* __restrict__ key, const int* __restrict__ val, long long n, int* parent) {
+    const long long i = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (i + 1 >= n || key[i] != key[i + 1]) return;
+    volatile int* p = parent;
+    int ra = find_root(p, val[i]), rb = find_root(p, val[i + 1]);
+    while (ra != rb) {
+        if (ra > rb) { const int t = ra; ra = rb; rb = t; }
+        const int old = atomicCAS(parent + rb, rb, ra);
+        if (old == rb) break;
+        ra = find_root(p, ra);
+        rb = find_root(p, old);
+    }
+}
+
+// every face's root, its component's face count and box, and the box of all referenced vertices (warp-reduced first)
+__global__ void __launch_bounds__(MS_THREADS) cc_stats_kernel(const int* __restrict__ T, const float* __restrict__ P, long long F, int* parent, int* __restrict__ cnt,
+                                                              int* __restrict__ bmin, int* __restrict__ bmax, int* __restrict__ gbox) {
+    const long long f = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
+    if (f < F) {
+        volatile int* p = parent;
+        int r = static_cast<int>(f);
+        while (p[r] != r) r = p[r];
+        p[f] = r;
+        atomicAdd(cnt + r, 1);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const float* v = P + 3 * static_cast<long long>(T[3 * f + k]);
+#pragma unroll
+            for (int d = 0; d < 3; ++d) {
+                const int o = ord_f32(v[d]);
+                lo[d] = min(lo[d], o);
+                hi[d] = max(hi[d], o);
+            }
+        }
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            atomicMin(bmin + 3 * r + d, lo[d]);
+            atomicMax(bmax + 3 * r + d, hi[d]);
+        }
+    }
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            lo[d] = min(lo[d], __shfl_xor_sync(0xffffffffu, lo[d], o));
+            hi[d] = max(hi[d], __shfl_xor_sync(0xffffffffu, hi[d], o));
+        }
+    }
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            atomicMin(gbox + d, lo[d]);
+            atomicMax(gbox + 3 + d, hi[d]);
+        }
+    }
+}
+
+__device__ __forceinline__ double box_diag(const int* lo, const int* hi) {
+    const double dx = __dsub_rn(static_cast<double>(unord_f32(hi[0])), static_cast<double>(unord_f32(lo[0])));
+    const double dy = __dsub_rn(static_cast<double>(unord_f32(hi[1])), static_cast<double>(unord_f32(lo[1])));
+    const double dz = __dsub_rn(static_cast<double>(unord_f32(hi[2])), static_cast<double>(unord_f32(lo[2])));
+    return sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
+}
+
+__global__ void __launch_bounds__(MS_THREADS) cc_keep_kernel(const int* __restrict__ parent, const int* __restrict__ cnt, const int* __restrict__ bmin,
+                                                             const int* __restrict__ bmax, const int* __restrict__ gbox, long long F, long long min_faces,
+                                                             double min_diameter, int* __restrict__ fkeep) {
+    const long long f = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (f >= F) return;
+    const int r = parent[f];
+    const double lim = __dmul_rn(min_diameter, box_diag(gbox, gbox + 3));
+    fkeep[f] = cnt[r] >= min_faces && !(box_diag(bmin + 3 * r, bmax + 3 * r) < lim);
+}
+
+// ------------------------------------------------------------------------------------------------------------ decimation
+struct DecHdr {
+    long long F;          // live faces (in T[buf])
+    long long E;          // edges of the round (DeviceSelect::Unique)
+    long long n_sel;      // accepted keys selected for trimming
+    u64 thr;              // largest key collapsed this round
+    int buf;              // which face buffer is live
+    int n_acc;            // accepted edges this round
+    int bad;              // malformed input faces
+};
+
+__device__ __forceinline__ void cross3(const double* p0, const double* p1, const double* p2, double* n) {
+    const double e1x = __dsub_rn(p1[0], p0[0]), e1y = __dsub_rn(p1[1], p0[1]), e1z = __dsub_rn(p1[2], p0[2]);
+    const double e2x = __dsub_rn(p2[0], p0[0]), e2y = __dsub_rn(p2[1], p0[1]), e2z = __dsub_rn(p2[2], p0[2]);
+    n[0] = __dsub_rn(__dmul_rn(e1y, e2z), __dmul_rn(e1z, e2y));
+    n[1] = __dsub_rn(__dmul_rn(e1z, e2x), __dmul_rn(e1x, e2z));
+    n[2] = __dsub_rn(__dmul_rn(e1x, e2y), __dmul_rn(e1y, e2x));
+}
+
+__device__ __forceinline__ void load3(const float* P, int v, double* p) {
+    p[0] = P[3 * v];
+    p[1] = P[3 * v + 1];
+    p[2] = P[3 * v + 2];
+}
+
+// x^T Q x at (x, y, z, 1), clamped below at 0
+__device__ __forceinline__ double quadric_cost(const double* q, double x, double y, double z) {
+    const double r0 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(q[0], x), __dmul_rn(q[1], y)), __dmul_rn(q[2], z)), q[3]);
+    const double r1 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(q[1], x), __dmul_rn(q[4], y)), __dmul_rn(q[5], z)), q[6]);
+    const double r2 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(q[2], x), __dmul_rn(q[5], y)), __dmul_rn(q[7], z)), q[8]);
+    const double r3 = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(q[3], x), __dmul_rn(q[6], y)), __dmul_rn(q[8], z)), q[9]);
+    const double c = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r0, x), __dmul_rn(r1, y)), __dmul_rn(r2, z)), r3);
+    return c > 0.0 ? c : 0.0;
+}
+
+__device__ __forceinline__ double cost_at(const double* q, const float* x) { return quadric_cost(q, x[0], x[1], x[2]); }
+
+// placement x̄ (fp32) of the summed quadric q and its cost
+__device__ __forceinline__ double placement(const double* q, const float* pa, const float* pb, float* x) {
+    const double c00 = __dsub_rn(__dmul_rn(q[4], q[7]), __dmul_rn(q[5], q[5]));
+    const double c01 = __dsub_rn(__dmul_rn(q[2], q[5]), __dmul_rn(q[1], q[7]));
+    const double c02 = __dsub_rn(__dmul_rn(q[1], q[5]), __dmul_rn(q[2], q[4]));
+    const double det = __dadd_rn(__dadd_rn(__dmul_rn(q[0], c00), __dmul_rn(q[1], c01)), __dmul_rn(q[2], c02));
+    const double tr = __dadd_rn(__dadd_rn(q[0], q[4]), q[7]);
+    bool solved = fabs(det) > __dmul_rn(SINGULAR_REL, __dmul_rn(__dmul_rn(tr, tr), tr));
+    if (solved) {
+        const double c11 = __dsub_rn(__dmul_rn(q[0], q[7]), __dmul_rn(q[2], q[2]));
+        const double c12 = __dsub_rn(__dmul_rn(q[1], q[2]), __dmul_rn(q[0], q[5]));
+        const double c22 = __dsub_rn(__dmul_rn(q[0], q[4]), __dmul_rn(q[1], q[1]));
+        const double b0 = -q[3], b1 = -q[6], b2 = -q[8];
+        x[0] = __double2float_rn(__ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(c00, b0), __dmul_rn(c01, b1)), __dmul_rn(c02, b2)), det));
+        x[1] = __double2float_rn(__ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(c01, b0), __dmul_rn(c11, b1)), __dmul_rn(c12, b2)), det));
+        x[2] = __double2float_rn(__ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(c02, b0), __dmul_rn(c12, b1)), __dmul_rn(c22, b2)), det));
+        solved = isfinite(x[0]) && isfinite(x[1]) && isfinite(x[2]);
+    }
+    if (solved) return cost_at(q, x);
+#pragma unroll
+    for (int d = 0; d < 3; ++d) x[d] = __double2float_rn(__dmul_rn(__dadd_rn(static_cast<double>(pa[d]), static_cast<double>(pb[d])), 0.5));
+    double best = cost_at(q, x);
+    const double ca = cost_at(q, pa);
+    if (ca < best) { best = ca; x[0] = pa[0]; x[1] = pa[1]; x[2] = pa[2]; }
+    const double cb = cost_at(q, pb);
+    if (cb < best) { best = cb; x[0] = pb[0]; x[1] = pb[1]; x[2] = pb[2]; }
+    return best;
+}
+
+// corner i of vertex v: the face id (low half of the sorted corner key) and the next (out) / previous (in) vertex of that face
+__device__ __forceinline__ int corner(const u64* ck, const int* T, int v, int i, int* out, int* in) {
+    const int f = static_cast<int>(static_cast<unsigned>(ck[i]));
+    const int* t = T + 3 * static_cast<long long>(f);
+    const int k = t[0] == v ? 0 : (t[1] == v ? 1 : 2);
+    *out = t[k == 2 ? 0 : k + 1];
+    *in = t[k == 0 ? 2 : k - 1];
+    return f;
+}
+
+__global__ void __launch_bounds__(MS_THREADS) corner_keys_kernel(const int* __restrict__ T, long long F, u64* __restrict__ ck) {
+    const long long h = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (h >= 3 * F) return;
+    ck[h] = (static_cast<u64>(static_cast<unsigned>(T[h])) << 32) | static_cast<u64>(h / 3);
+}
+
+// vertex CSR over the sorted corner keys: [vstart[v], vend[v]) (both memset to 0 first)
+__global__ void __launch_bounds__(MS_THREADS) csr_kernel(const u64* __restrict__ ck, long long n, int* __restrict__ vstart, int* __restrict__ vend) {
+    const long long i = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (i >= n) return;
+    const unsigned v = static_cast<unsigned>(ck[i] >> 32);
+    if (i == 0 || static_cast<unsigned>(ck[i - 1] >> 32) != v) vstart[v] = static_cast<int>(i);
+    if (i == n - 1 || static_cast<unsigned>(ck[i + 1] >> 32) != v) vend[v] = static_cast<int>(i + 1);
+}
+
+// Q_v = sum over v's faces in ascending face index (the corner list order) of the area-weighted plane quadric
+__global__ void __launch_bounds__(MS_THREADS) quadric_kernel(const float* __restrict__ P, const int* __restrict__ T, const u64* __restrict__ ck,
+                                                             const int* __restrict__ vstart, const int* __restrict__ vend, long long V, double* __restrict__ Q) {
+    const long long v = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (v >= V) return;
+    double acc[10];
+#pragma unroll
+    for (int k = 0; k < 10; ++k) acc[k] = 0.0;
+    for (int i = vstart[v]; i < vend[v]; ++i) {
+        const int* t = T + 3 * static_cast<long long>(static_cast<unsigned>(ck[i]));
+        double p0[3], p1[3], p2[3], c[3];
+        load3(P, t[0], p0);
+        load3(P, t[1], p1);
+        load3(P, t[2], p2);
+        cross3(p0, p1, p2, c);
+        const double ln = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(c[0], c[0]), __dmul_rn(c[1], c[1])), __dmul_rn(c[2], c[2])));
+        if (ln == 0.0) continue;
+        const double area = __dmul_rn(0.5, ln);
+        double u[4];
+        u[0] = __ddiv_rn(c[0], ln);
+        u[1] = __ddiv_rn(c[1], ln);
+        u[2] = __ddiv_rn(c[2], ln);
+        u[3] = -__dadd_rn(__dadd_rn(__dmul_rn(u[0], p0[0]), __dmul_rn(u[1], p0[1])), __dmul_rn(u[2], p0[2]));
+        int k = 0;
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int b = a; b < 4; ++b) acc[k] = __dadd_rn(acc[k], __dmul_rn(area, __dmul_rn(u[a], u[b]))), ++k;
+    }
+#pragma unroll
+    for (int k = 0; k < 10; ++k) Q[10 * v + k] = acc[k];
+}
+
+// frozen flag and degree (distinct neighbours) of every vertex
+__global__ void __launch_bounds__(MS_THREADS) vertex_state_kernel(const int* __restrict__ T, const u64* __restrict__ ck, const int* __restrict__ vstart,
+                                                                  const int* __restrict__ vend, long long V, uint8_t* __restrict__ frozen, int* __restrict__ deg) {
+    const long long vv = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (vv >= V) return;
+    const int v = static_cast<int>(vv), s = vstart[v], n = vend[v] - s;
+    bool ok = n > 0;
+    int distinct = 0;
+    for (int i = 0; i < n; ++i) {
+        int oi, ii;
+        corner(ck, T, v, s + i, &oi, &ii);
+        int c_oo = 0, c_oi = 0;
+        bool new_o = true, new_i = true;
+        for (int j = 0; j < n; ++j) {
+            int oj, ij;
+            corner(ck, T, v, s + j, &oj, &ij);
+            c_oo += oj == oi;
+            c_oi += ij == oi;
+            if (j < i && (oj == oi || ij == oi)) new_o = false;       // out_i seen among earlier outs or ins
+            if (j <= i && oj == ii) new_i = false;                    // in_i seen among outs up to i
+            if (j < i && ij == ii) new_i = false;                     // ... or among earlier ins
+        }
+        distinct += new_o;
+        distinct += new_i && ii != oi;
+        ok = ok && c_oo == 1 && c_oi == 1;
+    }
+    if (ok) {                                                         // one fan: the walk out -> in returns to corner 0 after n steps
+        int o0, cur;
+        corner(ck, T, v, s, &o0, &cur);
+        int steps = 1;
+        while (cur != o0 && steps <= n) {
+            int j = 0, oj, ij;
+            for (; j < n; ++j) {
+                corner(ck, T, v, s + j, &oj, &ij);
+                if (oj == cur) break;
+            }
+            cur = ij;
+            ++steps;
+        }
+        ok = steps == n;
+    }
+    frozen[v] = !ok;
+    deg[v] = distinct;
+}
+
+// no face of v's star but those containing `other` turns by 90 degrees or more when v moves to x (faces with a zero normal exempt)
+__device__ __forceinline__ bool star_ok(const float* P, const int* T, const u64* ck, int s, int n, int v, int other, const float* x) {
+    for (int i = 0; i < n; ++i) {
+        const int* t = T + 3 * static_cast<long long>(static_cast<unsigned>(ck[s + i]));
+        if (t[0] == other || t[1] == other || t[2] == other) continue;
+        double p[3][3], m[3][3], no[3], nn[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            load3(P, t[k], p[k]);
+#pragma unroll
+            for (int d = 0; d < 3; ++d) m[k][d] = t[k] == v ? static_cast<double>(x[d]) : p[k][d];
+        }
+        cross3(p[0], p[1], p[2], no);
+        if (no[0] == 0.0 && no[1] == 0.0 && no[2] == 0.0) continue;
+        cross3(m[0], m[1], m[2], nn);
+        if (!(__dadd_rn(__dadd_rn(__dmul_rn(no[0], nn[0]), __dmul_rn(no[1], nn[1])), __dmul_rn(no[2], nn[2])) > 0.0)) return false;
+    }
+    return true;
+}
+
+// one edge per thread; min-blocks 1 lets ptxas keep the fp64 solve and flip test in registers (it spills under the default bound)
+__global__ void __launch_bounds__(MS_THREADS, 1) edge_cost_kernel(const u64* __restrict__ edges, const DecHdr* __restrict__ hdr, const float* __restrict__ P,
+                                                               const double* __restrict__ Q, const int* __restrict__ T, const u64* __restrict__ ck,
+                                                               const int* __restrict__ vstart, const int* __restrict__ vend, const uint8_t* __restrict__ frozen,
+                                                               const int* __restrict__ deg, u64* __restrict__ ekey, float* __restrict__ xbar, u64* m1) {
+    const long long e = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (e >= hdr->E) return;
+    const u64 ed = edges[e];
+    const int a = static_cast<int>(ed >> 32), b = static_cast<int>(static_cast<unsigned>(ed));
+    u64 key = KEY_NONE;
+    if (!frozen[a] && !frozen[b]) {
+        const int sa = vstart[a], na = vend[a] - sa, sb = vstart[b], nb = vend[b] - sb;
+        int c = -1, d = -1, link = 0;
+        for (int i = 0; i < na; ++i) {
+            int oa, ia;
+            corner(ck, T, a, sa + i, &oa, &ia);
+            if (oa == b) c = ia;
+            if (ia == b) d = oa;
+            for (int j = 0; j < nb; ++j) {
+                int ob, ib;
+                corner(ck, T, b, sb + j, &ob, &ib);
+                link += oa == ob;
+            }
+        }
+        bool ok = link == 2 && c >= 0 && d >= 0 && c != d && deg[a] + deg[b] >= 7 && deg[c] >= 4 && deg[d] >= 4;
+        if (ok) {
+            double q[10];
+#pragma unroll
+            for (int k = 0; k < 10; ++k) q[k] = __dadd_rn(Q[10LL * a + k], Q[10LL * b + k]);
+            const float pa[3] = {P[3LL * a], P[3LL * a + 1], P[3LL * a + 2]}, pb[3] = {P[3LL * b], P[3LL * b + 1], P[3LL * b + 2]};
+            float x[3];
+            const double cost = placement(q, pa, pb, x);
+            ok = star_ok(P, T, ck, sa, na, a, b, x) && star_ok(P, T, ck, sb, nb, b, a, x);
+            if (ok) {
+                key = (static_cast<u64>(__float_as_uint(__double2float_rn(cost))) << 32) | static_cast<u64>(e);
+                xbar[3 * e] = x[0];
+                xbar[3 * e + 1] = x[1];
+                xbar[3 * e + 2] = x[2];
+                atomicMin(m1 + a, key);
+                atomicMin(m1 + b, key);
+            }
+        }
+    }
+    ekey[e] = key;
+}
+
+// m2 = m1 (copied before); m2[v] = min over v's neighbours of m1 too
+__global__ void __launch_bounds__(MS_THREADS) edge_min2_kernel(const u64* __restrict__ edges, const DecHdr* __restrict__ hdr, const u64* __restrict__ m1, u64* m2) {
+    const long long e = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (e >= hdr->E) return;
+    const u64 ed = edges[e];
+    const int a = static_cast<int>(ed >> 32), b = static_cast<int>(static_cast<unsigned>(ed));
+    if (m1[b] != KEY_NONE) atomicMin(m2 + a, m1[b]);
+    if (m1[a] != KEY_NONE) atomicMin(m2 + b, m1[a]);
+}
+
+__global__ void __launch_bounds__(MS_THREADS) edge_accept_kernel(const u64* __restrict__ edges, DecHdr* hdr, const u64* __restrict__ ekey, const u64* __restrict__ m2,
+                                                                 int* __restrict__ aflag) {
+    __shared__ int s_warp[MS_THREADS / 32];
+    const long long e = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    int acc = 0;
+    if (e < hdr->E) {
+        const u64 ed = edges[e], key = ekey[e];
+        const int a = static_cast<int>(ed >> 32), b = static_cast<int>(static_cast<unsigned>(ed));
+        acc = key != KEY_NONE && m2[a] == key && m2[b] == key;
+        aflag[e] = acc;
+    }
+    const int w = __popc(__ballot_sync(0xffffffffu, acc));
+    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = w;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int i = 0; i < MS_THREADS / 32; ++i) t += s_warp[i];
+        if (t) atomicAdd(&hdr->n_acc, t);
+    }
+}
+
+// the largest key collapsed this round: the k-th smallest accepted key when trimming (sorted != nullptr), else every accepted key
+__global__ void set_thr_kernel(DecHdr* hdr, const u64* sorted, long long k) { hdr->thr = sorted ? sorted[k - 1] : KEY_NONE - 1; }
+
+__global__ void __launch_bounds__(MS_THREADS) collapse_kernel(const u64* __restrict__ edges, const DecHdr* __restrict__ hdr, const u64* __restrict__ ekey,
+                                                              const int* __restrict__ aflag, const float* __restrict__ xbar, float* __restrict__ P, double* __restrict__ Q,
+                                                              int* __restrict__ rep) {
+    const long long e = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (e >= hdr->E || !aflag[e] || ekey[e] > hdr->thr) return;
+    const u64 ed = edges[e];
+    const long long a = static_cast<long long>(ed >> 32), b = static_cast<long long>(static_cast<unsigned>(ed));
+    P[3 * a] = xbar[3 * e];
+    P[3 * a + 1] = xbar[3 * e + 1];
+    P[3 * a + 2] = xbar[3 * e + 2];
+#pragma unroll
+    for (int k = 0; k < 10; ++k) Q[10 * a + k] = __dadd_rn(Q[10 * a + k], Q[10 * b + k]);
+    rep[b] = static_cast<int>(a);
+}
+
+__global__ void __launch_bounds__(MS_THREADS) remap_kernel(int* __restrict__ T, long long F, const int* __restrict__ rep, int* __restrict__ fkeep) {
+    const long long f = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (f >= F) return;
+    const int a = rep[T[3 * f]], b = rep[T[3 * f + 1]], c = rep[T[3 * f + 2]];
+    T[3 * f] = a;
+    T[3 * f + 1] = b;
+    T[3 * f + 2] = c;
+    fkeep[f] = a != b && b != c && c != a;
+}
+
+__global__ void __launch_bounds__(MS_THREADS) compact_faces_kernel(const int* __restrict__ T, long long F, const int* __restrict__ fkeep, const int* __restrict__ fpos,
+                                                                   int* __restrict__ Tout, DecHdr* hdr, int buf) {
+    const long long f = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (f == 0) {
+        hdr->F = F ? static_cast<long long>(fpos[F - 1]) + fkeep[F - 1] : 0;
+        hdr->buf = buf;
+    }
+    if (f >= F || !fkeep[f]) return;
+    const long long o = fpos[f];
+    Tout[3 * o] = T[3 * f];
+    Tout[3 * o + 1] = T[3 * f + 1];
+    Tout[3 * o + 2] = T[3 * f + 2];
+}
+
+__global__ void __launch_bounds__(MS_THREADS) iota_copy_kernel(const float* __restrict__ verts, long long V, float* __restrict__ P, int* __restrict__ rep) {
+    const long long v = blockIdx.x * static_cast<long long>(MS_THREADS) + threadIdx.x;
+    if (v >= V) return;
+    P[3 * v] = verts[3 * v];
+    P[3 * v + 1] = verts[3 * v + 1];
+    P[3 * v + 2] = verts[3 * v + 2];
+    rep[v] = static_cast<int>(v);
+}
+
+// ------------------------------------------------------------------------------------------------------------ workspaces
+struct CcWs {
+    int* bad;
+    int* gbox;
+    int* T;
+    u64* key[2];
+    int* val[2];
+    int *parent, *cnt, *bmin, *bmax, *fkeep, *fpos, *vref, *vpos;
+    void* cub;
+    size_t cub_bytes, total;
+};
+
+CcWs cc_layout(void* ws, long long V, long long F) {
+    Carve c{static_cast<uint8_t*>(ws)};
+    CcWs w;
+    w.bad = c.take<int>(1);
+    w.gbox = c.take<int>(6);
+    w.T = c.take<int>(3 * F);
+    w.key[0] = c.take<u64>(3 * F);
+    w.key[1] = c.take<u64>(3 * F);
+    w.val[0] = c.take<int>(3 * F);
+    w.val[1] = c.take<int>(3 * F);
+    w.parent = c.take<int>(F);
+    w.cnt = c.take<int>(F);
+    w.bmin = c.take<int>(3 * F);
+    w.bmax = c.take<int>(3 * F);
+    w.fkeep = c.take<int>(F);
+    w.fpos = c.take<int>(F);
+    w.vref = c.take<int>(V);
+    w.vpos = c.take<int>(V);
+    w.cub_bytes = cub_reserve(3 * F);
+    w.cub = c.take<uint8_t>(static_cast<long long>(w.cub_bytes));
+    w.total = c.off;
+    return w;
+}
+
+struct DecWs {
+    DecHdr* hdr;
+    float* P;
+    double* Q;
+    int *rep, *vstart, *vend, *deg;
+    uint8_t* frozen;
+    u64 *m1, *m2;
+    int* T[2];
+    u64* ck[2];
+    u64* hk[2];
+    u64* ekey;
+    float* xbar;
+    int *aflag, *fkeep, *fpos, *vref, *vpos;
+    void* cub;
+    size_t cub_bytes, total;
+};
+
+DecWs dec_layout(void* ws, long long V, long long F) {
+    Carve c{static_cast<uint8_t*>(ws)};
+    DecWs w;
+    w.hdr = c.take<DecHdr>(1);
+    w.P = c.take<float>(3 * V);
+    w.Q = c.take<double>(10 * V);
+    w.rep = c.take<int>(V);
+    w.vstart = c.take<int>(V);
+    w.vend = c.take<int>(V);
+    w.deg = c.take<int>(V);
+    w.frozen = c.take<uint8_t>(V);
+    w.m1 = c.take<u64>(V);
+    w.m2 = c.take<u64>(V);
+    w.vref = c.take<int>(V);
+    w.vpos = c.take<int>(V);
+    w.T[0] = c.take<int>(3 * F);
+    w.T[1] = c.take<int>(3 * F);
+    w.ck[0] = c.take<u64>(3 * F);
+    w.ck[1] = c.take<u64>(3 * F);
+    w.hk[0] = c.take<u64>(3 * F);
+    w.hk[1] = c.take<u64>(3 * F);
+    w.ekey = c.take<u64>(3 * F);
+    w.xbar = c.take<float>(9 * F);
+    w.aflag = c.take<int>(3 * F);
+    w.fkeep = c.take<int>(F);
+    w.fpos = c.take<int>(F);
+    w.cub_bytes = cub_reserve(3 * F);
+    w.cub = c.take<uint8_t>(static_cast<long long>(w.cub_bytes));
+    w.total = c.off;
+    return w;
+}
+
+// the largest CUB scratch either operation asks for at these sizes (host-side queries, no launch)
+int cub_need(long long V, long long F, size_t* need) {
+    size_t b = 0, m = 0;
+    const long long n3 = 3 * F;
+    cub::DoubleBuffer<u64> dk(nullptr, nullptr);
+    cub::DoubleBuffer<int> dv(nullptr, nullptr);
+    TPX_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, b, dk, dv, n3, 0, 64));
+    m = b > m ? b : m;
+    TPX_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, b, dk, n3, 0, 64));
+    m = b > m ? b : m;
+    TPX_CUDA(cub::DeviceSelect::Unique(nullptr, b, static_cast<const u64*>(nullptr), static_cast<u64*>(nullptr), static_cast<long long*>(nullptr), n3));
+    m = b > m ? b : m;
+    TPX_CUDA(cub::DeviceSelect::Flagged(nullptr, b, static_cast<const u64*>(nullptr), static_cast<const int*>(nullptr), static_cast<u64*>(nullptr),
+                                        static_cast<long long*>(nullptr), n3));
+    m = b > m ? b : m;
+    TPX_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b, static_cast<const int*>(nullptr), static_cast<int*>(nullptr), F > V ? F : V));
+    m = b > m ? b : m;
+    *need = m;
+    return TPX_OK;
+}
+
+int mesh_check(const char* what, const float* verts, long long V, const long long* faces, long long F, void* ws, size_t ws_bytes, size_t need, long long Vf,
+               long long Ff) {
+    TPX_CHECK(V >= 0 && F >= 0 && V < MS_INDEX_LIMIT && F < MS_INDEX_LIMIT, TPX_ERR_SHAPE, "%s: %lld vertices / %lld faces: each must be below 2^31", what, V, F);
+    TPX_CHECK((verts != nullptr || V == 0) && (faces != nullptr || F == 0) && ws != nullptr, TPX_ERR_ARG, "%s: null mesh or workspace", what);
+    TPX_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "%s: workspace must be 256-B aligned", what);
+    TPX_CHECK(V > 0 || F == 0, TPX_ERR_ARG, "%s: %lld faces index an empty vertex array", what, F);
+    TPX_CHECK(ws_bytes >= need, TPX_ERR_ARG, "%s: workspace of %zu bytes, %zu needed", what, ws_bytes, need);
+    size_t cub_bytes;
+    const int rc = cub_need(Vf, Ff, &cub_bytes);
+    if (rc != TPX_OK) return rc;
+    TPX_CHECK(cub_bytes <= cub_reserve(3 * Ff), TPX_ERR_STATE, "%s: sort scratch of %zu bytes exceeds the %zu reserved", what, cub_bytes, cub_reserve(3 * Ff));
+    return TPX_OK;
+}
+
+// scan of n int flags into pos (exclusive)
+int scan(const int* flags, int* pos, long long n, void* cub, size_t cub_bytes, cudaStream_t st) {
+    if (n == 0) return TPX_OK;
+    size_t b = cub_bytes;
+    TPX_CUDA(cub::DeviceScan::ExclusiveSum(cub, b, flags, pos, n, st));
+    return TPX_OK;
+}
+}  // namespace
+
+// ------------------------------------------------------------------------------------------------------------ component filter
+size_t cc_workspace_bytes(long long V, long long F) {
+    if (V < 0 || F < 0 || V >= MS_INDEX_LIMIT || F >= MS_INDEX_LIMIT) return 0;
+    return cc_layout(nullptr, V, F).total;
+}
+
+int launch_cc_count(const float* verts, long long V, const long long* faces, long long F, long long min_faces, double min_diameter, void* ws, size_t ws_bytes,
+                    long long* counts, cudaStream_t st) {
+    const int rc = mesh_check("remove_small_components", verts, V, faces, F, ws, ws_bytes, cc_workspace_bytes(V, F), V, F);
+    if (rc != TPX_OK) return rc;
+    TPX_CHECK(counts != nullptr, TPX_ERR_ARG, "remove_small_components: null counts");
+    const CcWs w = cc_layout(ws, V, F);
+    ProfScope prof(PROF_VAE_MISC, st);
+    TPX_CUDA(cudaMemsetAsync(w.bad, 0, sizeof(int), st));
+    static const int gbox0[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
+    TPX_CUDA(cudaMemcpyAsync(w.gbox, gbox0, sizeof(gbox0), cudaMemcpyHostToDevice, st));
+    if (V) TPX_CUDA(cudaMemsetAsync(w.vref, 0, V * sizeof(int), st));
+    if (F) {
+        faces_in_kernel<<<blocks(F), MS_THREADS, 0, st>>>(faces, F, V, w.T, w.bad);
+        TPX_LAUNCH_CHECK();
+        edge_keys_kernel<<<blocks(3 * F), MS_THREADS, 0, st>>>(w.T, F, w.key[0], w.val[0]);
+        TPX_LAUNCH_CHECK();
+        cub::DoubleBuffer<u64> dk(w.key[0], w.key[1]);
+        cub::DoubleBuffer<int> dv(w.val[0], w.val[1]);
+        size_t b = w.cub_bytes;
+        TPX_CUDA(cub::DeviceRadixSort::SortPairs(w.cub, b, dk, dv, 3 * F, 0, key_bits(V), st));
+        cc_init_kernel<<<blocks(F), MS_THREADS, 0, st>>>(F, w.parent, w.cnt, w.bmin, w.bmax);
+        TPX_LAUNCH_CHECK();
+        cc_union_kernel<<<blocks(3 * F), MS_THREADS, 0, st>>>(dk.Current(), dv.Current(), 3 * F, w.parent);
+        TPX_LAUNCH_CHECK();
+        cc_stats_kernel<<<blocks(F), MS_THREADS, 0, st>>>(w.T, verts, F, w.parent, w.cnt, w.bmin, w.bmax, w.gbox);
+        TPX_LAUNCH_CHECK();
+        cc_keep_kernel<<<blocks(F), MS_THREADS, 0, st>>>(w.parent, w.cnt, w.bmin, w.bmax, w.gbox, F, min_faces, min_diameter, w.fkeep);
+        TPX_LAUNCH_CHECK();
+        ref_kernel<<<blocks(3 * F), MS_THREADS, 0, st>>>(w.T, w.fkeep, F, w.vref);
+        TPX_LAUNCH_CHECK();
+    }
+    int r = scan(w.fkeep, w.fpos, F, w.cub, w.cub_bytes, st);
+    if (r == TPX_OK) r = scan(w.vref, w.vpos, V, w.cub, w.cub_bytes, st);
+    if (r != TPX_OK) return r;
+    counts_kernel<<<1, 1, 0, st>>>(w.vref, w.vpos, V, w.fkeep, w.fpos, F, 0, w.bad, counts);
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+int launch_cc_emit(const float* verts, long long V, long long F, const void* ws, size_t ws_bytes, float* verts_out, long long* faces_out, cudaStream_t st) {
+    TPX_CHECK(ws_bytes >= cc_workspace_bytes(V, F) && ws != nullptr && (V == 0 || verts != nullptr), TPX_ERR_ARG, "remove_small_components: bad emit arguments");
+    const CcWs w = cc_layout(const_cast<void*>(ws), V, F);
+    ProfScope prof(PROF_VAE_MISC, st);
+    if (V) {
+        emit_verts_kernel<<<blocks(V), MS_THREADS, 0, st>>>(verts, w.vref, w.vpos, V, verts_out);
+        TPX_LAUNCH_CHECK();
+    }
+    if (F) {
+        emit_faces_kernel<<<blocks(F), MS_THREADS, 0, st>>>(w.T, w.fkeep, w.fpos, nullptr, F, w.vpos, faces_out);
+        TPX_LAUNCH_CHECK();
+    }
+    return TPX_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------ decimation
+size_t dec_workspace_bytes(long long V, long long F) {
+    if (V < 0 || F < 0 || V >= MS_INDEX_LIMIT || F >= MS_INDEX_LIMIT) return 0;
+    return dec_layout(nullptr, V, F).total;
+}
+
+int launch_decimate(const float* verts, long long V, const long long* faces, long long F, long long target, void* ws, size_t ws_bytes, long long* counts,
+                    long long* trace, long long trace_cap, cudaStream_t st) {
+    const int rc = mesh_check("decimate", verts, V, faces, F, ws, ws_bytes, dec_workspace_bytes(V, F), V, F);
+    if (rc != TPX_OK) return rc;
+    TPX_CHECK(counts != nullptr && target >= 0, TPX_ERR_ARG, "decimate: null counts or negative target");
+    const DecWs w = dec_layout(ws, V, F);
+    ProfScope prof(PROF_VAE_MISC, st);
+    TPX_CUDA(cudaMemsetAsync(w.hdr, 0, sizeof(DecHdr), st));
+    if (V) {
+        iota_copy_kernel<<<blocks(V), MS_THREADS, 0, st>>>(verts, V, w.P, w.rep);
+        TPX_LAUNCH_CHECK();
+    }
+    if (F) {
+        faces_in_kernel<<<blocks(F), MS_THREADS, 0, st>>>(faces, F, V, w.T[0], &w.hdr->bad);
+        TPX_LAUNCH_CHECK();
+    }
+    const int bits = key_bits(V);
+    long long Fc = F, rounds = 0;
+    int buf = 0;
+    DecHdr h;
+    while (Fc > target) {
+        const long long n3 = 3 * Fc;
+        int* T = w.T[buf];
+        corner_keys_kernel<<<blocks(n3), MS_THREADS, 0, st>>>(T, Fc, w.ck[0]);
+        TPX_LAUNCH_CHECK();
+        cub::DoubleBuffer<u64> dc(w.ck[0], w.ck[1]);
+        size_t b = w.cub_bytes;
+        TPX_CUDA(cub::DeviceRadixSort::SortKeys(w.cub, b, dc, n3, 0, bits, st));
+        const u64* ck = dc.Current();
+        TPX_CUDA(cudaMemsetAsync(w.vstart, 0, V * sizeof(int), st));
+        TPX_CUDA(cudaMemsetAsync(w.vend, 0, V * sizeof(int), st));
+        csr_kernel<<<blocks(n3), MS_THREADS, 0, st>>>(ck, n3, w.vstart, w.vend);
+        TPX_LAUNCH_CHECK();
+        if (rounds == 0) {
+            quadric_kernel<<<blocks(V), MS_THREADS, 0, st>>>(w.P, T, ck, w.vstart, w.vend, V, w.Q);
+            TPX_LAUNCH_CHECK();
+        }
+        vertex_state_kernel<<<blocks(V), MS_THREADS, 0, st>>>(T, ck, w.vstart, w.vend, V, w.frozen, w.deg);
+        TPX_LAUNCH_CHECK();
+        // edges: sorted unique half-edge keys, into the buffer the sort did not end in
+        edge_keys_kernel<<<blocks(n3), MS_THREADS, 0, st>>>(T, Fc, w.hk[0], nullptr);
+        TPX_LAUNCH_CHECK();
+        cub::DoubleBuffer<u64> dh(w.hk[0], w.hk[1]);
+        b = w.cub_bytes;
+        TPX_CUDA(cub::DeviceRadixSort::SortKeys(w.cub, b, dh, n3, 0, bits, st));
+        const u64* edges = dh.Alternate();
+        b = w.cub_bytes;
+        TPX_CUDA(cub::DeviceSelect::Unique(w.cub, b, dh.Current(), dh.Alternate(), &w.hdr->E, n3, st));
+        TPX_CUDA(cudaMemsetAsync(w.m1, 0xff, V * sizeof(u64), st));
+        TPX_CUDA(cudaMemsetAsync(&w.hdr->n_acc, 0, sizeof(int), st));
+        edge_cost_kernel<<<blocks(n3), MS_THREADS, 0, st>>>(edges, w.hdr, w.P, w.Q, T, ck, w.vstart, w.vend, w.frozen, w.deg, w.ekey, w.xbar, w.m1);
+        TPX_LAUNCH_CHECK();
+        TPX_CUDA(cudaMemcpyAsync(w.m2, w.m1, V * sizeof(u64), cudaMemcpyDeviceToDevice, st));
+        edge_min2_kernel<<<blocks(n3), MS_THREADS, 0, st>>>(edges, w.hdr, w.m1, w.m2);
+        TPX_LAUNCH_CHECK();
+        edge_accept_kernel<<<blocks(n3), MS_THREADS, 0, st>>>(edges, w.hdr, w.ekey, w.m2, w.aflag);
+        TPX_LAUNCH_CHECK();
+        TPX_CUDA(cudaMemcpyAsync(&h, w.hdr, sizeof(DecHdr), cudaMemcpyDeviceToHost, st));
+        TPX_CUDA(cudaStreamSynchronize(st));                              // the one readback of the round
+        TPX_CHECK(h.bad == 0, TPX_ERR_ARG, "decimate: %d faces have an index outside [0, %lld) or a repeated index", h.bad, V);
+        TPX_CHECK(h.E < (1LL << 32), TPX_ERR_SHAPE, "decimate: %lld edges: edge ids must fit in 32 bits", h.E);
+        if (h.n_acc == 0) break;
+        long long k = h.n_acc;
+        if (Fc - 2 * k < target) {                                        // last round: the smallest keys only
+            k = (Fc - target + 1) / 2;
+            u64* sel = w.ck[dc.selector ^ 1];                             // the corner keys' spare buffer and the half-edges' sorted buffer
+            b = w.cub_bytes;
+            TPX_CUDA(cub::DeviceSelect::Flagged(w.cub, b, w.ekey, w.aflag, sel, &w.hdr->n_sel, h.E, st));
+            cub::DoubleBuffer<u64> ds(sel, dh.Current());
+            b = w.cub_bytes;
+            TPX_CUDA(cub::DeviceRadixSort::SortKeys(w.cub, b, ds, static_cast<long long>(h.n_acc), 0, 64, st));
+            set_thr_kernel<<<1, 1, 0, st>>>(w.hdr, ds.Current(), k);
+        } else {
+            set_thr_kernel<<<1, 1, 0, st>>>(w.hdr, nullptr, 0);
+        }
+        TPX_LAUNCH_CHECK();
+        collapse_kernel<<<blocks(n3), MS_THREADS, 0, st>>>(edges, w.hdr, w.ekey, w.aflag, w.xbar, w.P, w.Q, w.rep);
+        TPX_LAUNCH_CHECK();
+        remap_kernel<<<blocks(Fc), MS_THREADS, 0, st>>>(T, Fc, w.rep, w.fkeep);
+        TPX_LAUNCH_CHECK();
+        const int r = scan(w.fkeep, w.fpos, Fc, w.cub, w.cub_bytes, st);
+        if (r != TPX_OK) return r;
+        compact_faces_kernel<<<blocks(Fc), MS_THREADS, 0, st>>>(T, Fc, w.fkeep, w.fpos, w.T[buf ^ 1], w.hdr, buf ^ 1);
+        TPX_LAUNCH_CHECK();
+        buf ^= 1;
+        Fc -= 2 * k;
+        if (trace && rounds < trace_cap) trace[rounds] = Fc;
+        ++rounds;
+    }
+    if (rounds == 0 && F > 0) {                                           // no round ran: the input faces still need their check
+        TPX_CUDA(cudaMemcpyAsync(&h, w.hdr, sizeof(DecHdr), cudaMemcpyDeviceToHost, st));
+        TPX_CUDA(cudaStreamSynchronize(st));
+        TPX_CHECK(h.bad == 0, TPX_ERR_ARG, "decimate: %d faces have an index outside [0, %lld) or a repeated index", h.bad, V);
+    }
+    if (rounds == 0) {
+        static const int zero = 0;
+        TPX_CUDA(cudaMemcpyAsync(&w.hdr->buf, &zero, sizeof(int), cudaMemcpyHostToDevice, st));
+        TPX_CUDA(cudaMemcpyAsync(&w.hdr->F, &F, sizeof(long long), cudaMemcpyHostToDevice, st));
+        TPX_CUDA(cudaStreamSynchronize(st));                              // the host values above live on this stack frame
+    }
+    if (V) TPX_CUDA(cudaMemsetAsync(w.vref, 0, V * sizeof(int), st));
+    if (Fc) {
+        ref_kernel<<<blocks(3 * Fc), MS_THREADS, 0, st>>>(w.T[buf], nullptr, Fc, w.vref);
+        TPX_LAUNCH_CHECK();
+    }
+    const int r = scan(w.vref, w.vpos, V, w.cub, w.cub_bytes, st);
+    if (r != TPX_OK) return r;
+    counts_kernel<<<1, 1, 0, st>>>(w.vref, w.vpos, V, nullptr, nullptr, 0, Fc, nullptr, counts);
+    TPX_LAUNCH_CHECK();
+    TPX_CUDA(cudaMemcpyAsync(counts + 2, &rounds, sizeof(long long), cudaMemcpyHostToDevice, st));
+    TPX_CUDA(cudaStreamSynchronize(st));
+    return TPX_OK;
+}
+
+int launch_decimate_emit(long long V, long long F, const void* ws, size_t ws_bytes, float* verts_out, long long* faces_out, cudaStream_t st) {
+    TPX_CHECK(ws_bytes >= dec_workspace_bytes(V, F) && ws != nullptr, TPX_ERR_ARG, "decimate: bad emit arguments");
+    const DecWs w = dec_layout(const_cast<void*>(ws), V, F);
+    DecHdr h;
+    TPX_CUDA(cudaMemcpyAsync(&h, w.hdr, sizeof(DecHdr), cudaMemcpyDeviceToHost, st));
+    TPX_CUDA(cudaStreamSynchronize(st));
+    ProfScope prof(PROF_VAE_MISC, st);
+    if (V) {
+        emit_verts_kernel<<<blocks(V), MS_THREADS, 0, st>>>(w.P, w.vref, w.vpos, V, verts_out);
+        TPX_LAUNCH_CHECK();
+    }
+    if (h.F) {
+        emit_faces_kernel<<<blocks(h.F), MS_THREADS, 0, st>>>(w.T[h.buf], nullptr, nullptr, nullptr, h.F, w.vpos, faces_out);
+        TPX_LAUNCH_CHECK();
+    }
+    return TPX_OK;
+}
+
+}  // namespace tpx
+
+using namespace tpx;
+
+extern "C" {
+
+size_t tpx_mesh_components_workspace_bytes(int64_t V, int64_t F) { return cc_workspace_bytes(V, F); }
+
+int tpx_mesh_components_count(const float* verts, int64_t V, const int64_t* faces, int64_t F, int64_t min_faces, double min_diameter, void* ws, size_t ws_bytes,
+                              int64_t* counts, void* stream) {
+    const int rc = tpx_device_check();
+    if (rc != TPX_OK) return rc;
+    return launch_cc_count(verts, V, reinterpret_cast<const long long*>(faces), F, min_faces, min_diameter, ws, ws_bytes, reinterpret_cast<long long*>(counts),
+                           static_cast<cudaStream_t>(stream));
+}
+
+int tpx_mesh_components_emit(const float* verts, int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out, int64_t* faces_out, void* stream) {
+    const int rc = tpx_device_check();
+    if (rc != TPX_OK) return rc;
+    return launch_cc_emit(verts, V, F, ws, ws_bytes, verts_out, reinterpret_cast<long long*>(faces_out), static_cast<cudaStream_t>(stream));
+}
+
+size_t tpx_decimate_workspace_bytes(int64_t V, int64_t F) { return dec_workspace_bytes(V, F); }
+
+int tpx_decimate(const float* verts, int64_t V, const int64_t* faces, int64_t F, int64_t target, void* ws, size_t ws_bytes, int64_t* counts, int64_t* trace,
+                 int64_t trace_cap, void* stream) {
+    const int rc = tpx_device_check();
+    if (rc != TPX_OK) return rc;
+    return launch_decimate(verts, V, reinterpret_cast<const long long*>(faces), F, target, ws, ws_bytes, reinterpret_cast<long long*>(counts),
+                           reinterpret_cast<long long*>(trace), trace_cap, static_cast<cudaStream_t>(stream));
+}
+
+int tpx_decimate_emit(int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out, int64_t* faces_out, void* stream) {
+    const int rc = tpx_device_check();
+    if (rc != TPX_OK) return rc;
+    return launch_decimate_emit(V, F, ws, ws_bytes, verts_out, reinterpret_cast<long long*>(faces_out), static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

@@ -5,9 +5,13 @@
 in index units, component d along array axis d, shared between triangles; faces are int64 and wound so that the normal
 (v1 - v0) x (v2 - v0) points toward increasing value (outward for an SDF that is negative inside).  See INTEGRATION.md for how
 this differs from PyMCubes.
+
+``remove_small_components`` and ``decimate`` (csrc/mesh_simplify.cu) are the clean_mesh / decimate_mesh calls extract_texmesh makes
+next (inference.py:126-129, pymeshlab there); see INTEGRATION.md for how they differ from pymeshlab.
 """
 from __future__ import annotations
 
+import ctypes as C
 import types
 
 import numpy as np
@@ -67,6 +71,114 @@ def marching_cubes(volume, isovalue: float = 0.0):
     vol = torch.from_numpy(np.ascontiguousarray(arr, dtype=np.float32)).to(torch.device("cuda", torch.cuda.current_device()))
     verts, faces = _mesh(vol, isovalue)
     return verts.cpu().numpy().astype(np.float64), faces.cpu().numpy()
+
+
+def _check_mesh(verts: torch.Tensor, faces: torch.Tensor):
+    """ValueError unless verts is fp32 [V,3] and faces int64 [F,3] with every index in [0, V) and three distinct indices per face."""
+    if verts.dim() != 2 or verts.shape[1] != 3 or verts.dtype != torch.float32:
+        raise ValueError(f"verts must be float32 [V,3], got {verts.dtype} {tuple(verts.shape)}")
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype != torch.int64:
+        raise ValueError(f"faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
+    V, F = verts.shape[0], faces.shape[0]
+    if V >= _INDEX_LIMIT or F >= _INDEX_LIMIT:
+        raise ValueError(f"{V} vertices / {F} faces: each must be below 2^31")
+    if F:
+        if int(faces.min()) < 0 or int(faces.max()) >= V:
+            raise ValueError(f"a face index is outside [0, {V})")
+        if bool(((faces[:, 0] == faces[:, 1]) | (faces[:, 1] == faces[:, 2]) | (faces[:, 2] == faces[:, 0])).any()):
+            raise ValueError("a face repeats a vertex index")
+
+
+def _remove_small(verts: torch.Tensor, faces: torch.Tensor, min_faces: int, min_diameter: float):
+    """CUDA verts fp32 [V,3] / faces int64 [F,3] (checked) -> the kept mesh on their device.  Reads the two counts back once."""
+    dev = verts.device
+    V, F = verts.shape[0], faces.shape[0]
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        nbytes = int(lib.tpx_mesh_components_workspace_bytes(V, F))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        counts = torch.empty(2, dtype=torch.int64, device=dev)
+        st = _lib.stream_ptr()
+        _lib.check(lib.tpx_mesh_components_count(verts.data_ptr(), V, faces.data_ptr(), F, int(min_faces), float(min_diameter), ws.data_ptr(), nbytes,
+                                                 counts.data_ptr(), st), "tpx_mesh_components_count")
+        Vo, Fo = counts.tolist()
+        if Vo < 0:
+            raise ValueError("a face index is outside [0, V) or a face repeats an index")
+        vo = torch.empty(Vo, 3, dtype=torch.float32, device=dev)
+        fo = torch.empty(Fo, 3, dtype=torch.int64, device=dev)
+        _lib.check(lib.tpx_mesh_components_emit(verts.data_ptr(), V, F, ws.data_ptr(), nbytes, vo.data_ptr(), fo.data_ptr(), st), "tpx_mesh_components_emit")
+    return vo, fo
+
+
+def _decimate(verts: torch.Tensor, faces: torch.Tensor, target: int, trace: list | None = None):
+    """CUDA verts / faces (checked) -> the decimated mesh on their device; ``trace`` (a list) receives the face count after each round."""
+    dev = verts.device
+    V, F = verts.shape[0], faces.shape[0]
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        nbytes = int(lib.tpx_decimate_workspace_bytes(V, F))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        counts = torch.empty(3, dtype=torch.int64, device=dev)
+        st = _lib.stream_ptr()
+        cap = 4096 if trace is not None else 0
+        buf = (C.c_int64 * max(cap, 1))()
+        _lib.check(lib.tpx_decimate(verts.data_ptr(), V, faces.data_ptr(), F, int(target), ws.data_ptr(), nbytes, counts.data_ptr(),
+                                    buf if cap else None, cap, st), "tpx_decimate")
+        Vo, Fo, rounds = counts.tolist()
+        if trace is not None:
+            trace.extend(int(buf[i]) for i in range(min(rounds, cap)))
+        vo = torch.empty(Vo, 3, dtype=torch.float32, device=dev)
+        fo = torch.empty(Fo, 3, dtype=torch.int64, device=dev)
+        _lib.check(lib.tpx_decimate_emit(V, F, ws.data_ptr(), nbytes, vo.data_ptr(), fo.data_ptr(), st), "tpx_decimate_emit")
+    return vo, fo
+
+
+def _mesh_call(fn, verts, faces, *args):
+    """The marching_cubes convention: CUDA tensors in, CUDA tensors out; numpy in, numpy float64 / int64 out from the current device."""
+    if isinstance(verts, torch.Tensor) or isinstance(faces, torch.Tensor):
+        if not (isinstance(verts, torch.Tensor) and isinstance(faces, torch.Tensor)):
+            raise ValueError("pass verts and faces both as tensors or both as numpy arrays")
+        if not verts.is_cuda or not faces.is_cuda:
+            raise _lib.TpxError("mesh clean-up runs on CUDA only (no CPU path): pass CUDA tensors or numpy arrays")
+        if verts.device != faces.device:
+            raise ValueError(f"verts on {verts.device}, faces on {faces.device}")
+        verts, faces = verts.contiguous(), faces.contiguous()
+        _check_mesh(verts, faces)
+        return fn(verts, faces, *args)
+    v, f = np.asarray(verts), np.asarray(faces)
+    if v.ndim != 2 or v.shape[1] != 3 or f.ndim != 2 or f.shape[1] != 3 or not np.issubdtype(f.dtype, np.integer):
+        raise ValueError(f"verts must be [V,3] and faces integer [F,3], got {v.shape} and {f.dtype} {f.shape}")
+    _lib.lib()                                 # raises TpxError without a GPU
+    dev = torch.device("cuda", torch.cuda.current_device())
+    vt = torch.from_numpy(np.ascontiguousarray(v, dtype=np.float32)).to(dev)
+    ft = torch.from_numpy(np.ascontiguousarray(f, dtype=np.int64)).to(dev)
+    _check_mesh(vt, ft)
+    vo, fo = fn(vt, ft, *args)
+    return vo.cpu().numpy().astype(np.float64), fo.cpu().numpy()
+
+
+def remove_small_components(verts, faces, min_faces: int = 8, min_diameter: float = 0.05):
+    """Drop the small connected components of a triangle mesh: clean_mesh's remove_connected_component_by_face_number(min_f) and
+    ..._by_diameter(PercentageValue(min_d)) (utils/meshutils.py:63-193, inference.py:126 with min_f = 8, min_d = 5).
+
+    Faces are connected iff they share an undirected edge; a component is removed iff it has fewer than ``min_faces`` faces or its
+    bounding-box diagonal is below ``min_diameter`` (a fraction, 0.05 for min_d = 5) times that of all referenced vertices.  Returns the
+    vertices the kept faces use (ascending original id) and the kept faces (original order, remapped, winding unchanged).
+    CUDA fp32 [V,3] / int64 [F,3] tensors give CUDA tensors; numpy arrays give float64 / int64 numpy arrays computed on the current
+    device; a CPU tensor or a call without a GPU raises TpxError; malformed input (shapes, dtypes, an index outside [0, V), a face
+    repeating an index) raises ValueError."""
+    return _mesh_call(_remove_small, verts, faces, int(min_faces), float(min_diameter))
+
+
+def decimate(verts, faces, target_faces: int):
+    """Quadric-error edge-collapse decimation to ``target_faces`` faces: the GPU stand-in for decimate_mesh(v, t, target)
+    (utils/meshutils.py:63-193, inference.py:129 with 100000).  Deterministic rounds of independent collapses (DESIGN.md §1 f-7);
+    boundary and non-manifold vertices never move.  A reachable target ends at ``target_faces - 1`` or ``target_faces`` faces; if a
+    round finds no valid collapse (e.g. a mesh of only boundary or tetrahedron-like pieces) the mesh is returned ABOVE the target.
+    ``target_faces >= F`` returns the input (minus unreferenced vertices).  Inputs and outputs as ``remove_small_components``."""
+    if int(target_faces) < 0:
+        raise ValueError(f"target_faces must be >= 0, got {target_faces}")
+    return _mesh_call(_decimate, verts, faces, int(target_faces))
 
 
 def mcubes_module() -> types.ModuleType:

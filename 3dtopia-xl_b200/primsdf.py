@@ -88,16 +88,28 @@ class PrimSDF(nn.Module):
                        "tpx_primsdf_sdf_grid")
         return grid
 
-    def extract_mesh(self, resolution: int = 256, isovalue: float = 0.0, bound: float = 1.0):
+    def extract_mesh(self, resolution: int = 256, isovalue: float = 0.0, bound: float = 1.0, *, min_faces: int = 0, min_diameter: float = 0.0,
+                     target_faces: int | None = None):
         """Surface of the sdf field on the GPU: ``sdf_grid`` + marching cubes, in world coordinates (origin -bound, spacing
         2 bound / (R - 1)), i.e. inference.py:107-124 without the host copy.  Returns (verts fp32 [V,3], faces int64 [F,3]) on the
-        module's device.  The primitive noise filter of extract_texmesh (:90-103) stays with the caller."""
+        module's device.  Then, in the order of inference.py:126-129: when ``min_faces`` > 0 or ``min_diameter`` > 0,
+        ``mesh.remove_small_components`` with those thresholds; when ``target_faces`` is set, ``mesh.decimate`` to it (see its note on
+        unreachable targets).  ``extract_mesh(256, min_faces=8, min_diameter=0.05, target_faces=100000)`` is the geometry of
+        extract_texmesh up to the parts of clean_mesh this package does not implement (DESIGN.md §8).  The defaults run marching cubes
+        only.  The primitive noise filter of extract_texmesh (:90-103) stays with the caller."""
         R = int(resolution)
         if R < 2:
             raise ValueError(f"resolution must be >= 2, got {resolution}")
+        if target_faces is not None and int(target_faces) < 0:
+            raise ValueError(f"target_faces must be >= 0, got {target_faces}")
         grid = self.sdf_grid(R, bound)
         step = 2.0 * bound / (R - 1)
-        return mesh._mesh(grid, isovalue, origin=(-bound,) * 3, spacing=(step,) * 3)
+        v, f = mesh._mesh(grid, isovalue, origin=(-bound,) * 3, spacing=(step,) * 3)
+        if min_faces > 0 or min_diameter > 0:
+            v, f = mesh._remove_small(v, f, int(min_faces), float(min_diameter))
+        if target_faces is not None:
+            v, f = mesh._decimate(v, f, int(target_faces))
+        return v, f
 
     def bake_texture(self, v, f, vt, ft, resolution=1024, pad: int = 32):
         """Texture atlas of the colour / material channels over a UV-unwrapped mesh, on the GPU: inference.py:163-211 in one call

@@ -254,7 +254,38 @@ int tpx_mc_emit(const float* vol_dev, int64_t X, int64_t Y, int64_t Z, float iso
                 size_t ws_bytes, float* verts_dev, int64_t* faces_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Texture bake — the back half of extract_texmesh (inference.py:163-211), device-resident.  All tensors contiguous, row-major;
+ * Mesh clean-up and decimation — the host stage extract_texmesh runs between marching cubes and the unwrap (inference.py:126-129:
+ * clean_mesh(v, t, min_f=8, min_d=5, ...) then decimate_mesh(v, t, 100000), both pymeshlab, utils/meshutils.py:63-193).
+ * Input: verts device fp32 [V,3], faces device int64 [F,3] (as tpx_mc_emit writes them), V and F below 2^31.  An index outside [0, V)
+ * or a face that repeats an index is an error; zero-area faces with distinct indices are allowed.  Output: the vertices some kept face
+ * uses, in ascending original id, and the kept faces in their original order, remapped, each with its own cyclic vertex order.
+ * Deterministic: repeated calls, on any stream, give identical bytes.  Workspaces: 256-B aligned device memory of *_workspace_bytes(V, F)
+ * bytes (0 = too large); the emit call takes the same workspace, V and F, on the same stream.  The full contract, with the arithmetic
+ * spelled out, is in DESIGN.md §1 f-7.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* clean_mesh's remove_connected_component_by_face_number(min_f) and ..._by_diameter(PercentageValue(min_d)) (utils/meshutils.py:63-193,
+ * called at inference.py:126-127): faces are adjacent iff they share an undirected edge; a component is removed iff it has fewer than
+ * min_faces faces or its box diagonal is below min_diameter (a fraction: min_d = 5 is 0.05) times the box diagonal of all referenced
+ * vertices.  _count writes counts_dev[0] = V_out, [1] = F_out (device int64; both -1 for malformed faces, which _emit must then not be
+ * called for); neither call synchronises.  About 150 bytes of workspace per face. */
+size_t tpx_mesh_components_workspace_bytes(int64_t V, int64_t F);
+int tpx_mesh_components_count(const float* verts_dev, int64_t V, const int64_t* faces_dev, int64_t F, int64_t min_faces, double min_diameter, void* ws,
+                              size_t ws_bytes, int64_t* counts_dev, void* stream);
+int tpx_mesh_components_emit(const float* verts_dev, int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out_dev, int64_t* faces_out_dev,
+                             void* stream);
+/* decimate_mesh(v, t, target) (utils/meshutils.py:63-193, called at inference.py:129 with 100000): quadric-error edge collapse in rounds of
+ * independent collapses (DESIGN.md §1 f-7); boundary and non-manifold vertices stay fixed.  Stops when F <= target (a reachable target
+ * ends at F in {target - 1, target}) or when a round accepts nothing (the mesh is then left above target).  tpx_decimate SYNCHRONISES
+ * the stream once per round (it reads the accepted count back) and on return; it writes counts_dev[0] = V_out, [1] = F_out,
+ * [2] = rounds, and, when trace_host is not NULL, the face count after each of the first trace_cap rounds into that host array.
+ * Malformed faces return TPX_ERR_ARG.  About 290 bytes of workspace per face.  tpx_decimate_emit writes the result (it reads the live counts back, so it synchronises too). */
+size_t tpx_decimate_workspace_bytes(int64_t V, int64_t F);
+int tpx_decimate(const float* verts_dev, int64_t V, const int64_t* faces_dev, int64_t F, int64_t target, void* ws, size_t ws_bytes, int64_t* counts_dev,
+                 int64_t* trace_host, int64_t trace_cap, void* stream);
+int tpx_decimate_emit(int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out_dev, int64_t* faces_out_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Texture bake —the back half of extract_texmesh (inference.py:163-211), device-resident.  All tensors contiguous, row-major;
  * atlas H, W in 1..8192; index tensors int32.
  *
  * tpx_uv_rasterize stands behind dr.rasterize as called at inference.py:163-172 (positions (2 uv - 1, 0, 1), i.e. a UV-space
