@@ -31,7 +31,7 @@ class SamplerCoefs(C.Structure):
                                          "coef1", "coef2", "min_log", "max_log")] + [("clip", C.c_int32)]
 
 
-# name -> (restype, argtypes); mirrors include/tpx.h one to one (tests/test_abi.py checks the header against this table)
+# name -> (restype, argtypes); mirrors include/tpx.h one to one and in its order (tests/test_abi.py checks every type)
 SIGNATURES = {
     "tpx_version": (_i, []),
     "tpx_last_error": (C.c_char_p, []),
@@ -68,13 +68,14 @@ SIGNATURES = {
     "tpx_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "tpx_attention_tc": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "tpx_cfg_combine": (_i, [_vp, _i64, _f, _vp, _vp]),
-    "tpx_gelu_erf": (_i, [_vp, _i64, _vp]),
+    "tpx_groupnorm_silu": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp, _vp]),
+    "tpx_conv3d_k3": (_i, [_vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _i, _vp]),
     "tpx_primsdf_query": (_i, [_vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp, _vp]),
-    "tpx_raymarch_preview": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _f, _vp, _vp]),
     "tpx_primsdf_grid_bytes": (_sz, [_i64]),
     "tpx_primsdf_grid_build": (_i, [_vp, _i, _vp, _sz, _vp]),
     "tpx_primsdf_query_grid": (_i, [_vp, _vp, _vp, _vp, _sz, _i64, _i, _i, _i, _i, _vp, _vp]),
     "tpx_primsdf_sdf_grid": (_i, [_vp, _i, _vp, _vp, _vp, _sz, _i, _i, _i, _i, _vp, _vp]),
+    "tpx_raymarch_preview": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _f, _vp, _vp]),
     "tpx_mc_workspace_bytes": (_sz, [_i64, _i64, _i64]),
     "tpx_mc_count": (_i, [_vp, _i64, _i64, _i64, _f, _vp, _sz, _vp, _vp]),
     "tpx_mc_emit": (_i, [_vp, _i64, _i64, _i64, _f, _f, _f, _f, _f, _f, _f, _vp, _sz, _vp, _vp, _vp]),
@@ -89,8 +90,7 @@ SIGNATURES = {
     "tpx_primsdf_bake": (_i, [_vp, _i, _i, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _sz, _i, _i, _i, _vp, _vp, _vp]),
     "tpx_texture_inpaint_bytes": (_sz, [_i, _i]),
     "tpx_texture_inpaint": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp, _vp]),
-    "tpx_groupnorm_silu": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp, _vp]),
-    "tpx_conv3d_k3": (_i, [_vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _i, _vp]),
+    "tpx_gelu_erf": (_i, [_vp, _i64, _vp]),
 }
 
 

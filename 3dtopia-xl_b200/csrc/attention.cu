@@ -253,3 +253,13 @@ int launch_attention(const __half* q, const __half* k, const __half* v, __half* 
 }
 
 }  // namespace tpx
+
+using namespace tpx;
+
+extern "C" int tpx_attention(const void* q, const void* k, const void* v, void* out, int B, int H, int Nq, int Nk, int Dh, int DhP, float scale,
+                             void* stream) {
+    TPX_CHECK(q != nullptr && k != nullptr && v != nullptr && out != nullptr, TPX_ERR_ARG, "attention: null argument");
+    TPX_DEVICE_GUARD();
+    return launch_attention(static_cast<const __half*>(q), static_cast<const __half*>(k), static_cast<const __half*>(v), static_cast<__half*>(out), B, H,
+                            Nq, Nk, Dh, DhP, scale, static_cast<cudaStream_t>(stream));
+}

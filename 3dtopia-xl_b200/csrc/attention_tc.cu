@@ -229,3 +229,13 @@ int launch_attention_tc(const __half* q, const __half* k, const __half* vT, __ha
 }
 
 }  // namespace tpx
+
+using namespace tpx;
+
+extern "C" int tpx_attention_tc(const void* q, const void* k, const void* vT, void* out, int B, int H, int Nq, int Nk, int NkPad, int Dh, float scale,
+                                void* stream) {
+    TPX_CHECK(q != nullptr && k != nullptr && vT != nullptr && out != nullptr, TPX_ERR_ARG, "attention_tc: null argument");
+    TPX_DEVICE_GUARD();
+    return launch_attention_tc(static_cast<const __half*>(q), static_cast<const __half*>(k), static_cast<const __half*>(vT), static_cast<__half*>(out), B, H,
+                               Nq, Nk, NkPad, Dh, scale, static_cast<cudaStream_t>(stream));
+}

@@ -30,6 +30,7 @@ extern "C" int tpx_gelu_erf(void* x_f16, int64_t n, void* stream) {
     TPX_CHECK(n >= 0 && n % 8 == 0 && (reinterpret_cast<uintptr_t>(x_f16) & 15) == 0, TPX_ERR_SHAPE, "gelu_erf: %lld elements (need a multiple of 8, 16-B aligned)",
               static_cast<long long>(n));
     if (n == 0) return TPX_OK;
+    TPX_DEVICE_GUARD();
     const long long n8 = n / 8;
     const long long want = (n8 + 255) / 256;
     const unsigned blocks = static_cast<unsigned>(want < gemm_num_sms() * 8LL ? want : gemm_num_sms() * 8LL);

@@ -17,8 +17,6 @@
 // Roles: warp 0 TMA producer, warps 4-7 one consumer warpgroup (wgmma + the per-thread epilogue shared with the GEMM: bias /
 // residual-scale / NCDHW output; warp q holds rows 16 q .. 16 q + 15 of both planes and hands them to one-row-per-thread form
 // through its exchange buffer).
-#include <cstdlib>
-
 #include "kernels.cuh"
 
 namespace tpx {
@@ -183,8 +181,7 @@ int launch_halo(const CUtensorMap& ta, const CUtensorMap& tb, const HaloArgs& ha
 }  // namespace
 
 bool conv3_halo_supported(int S, int C, int Cout, int epi) {
-    static const bool off = getenv("TPX_CONV_HALO") != nullptr && getenv("TPX_CONV_HALO")[0] == '0';    // 0: use the per-tap implicit GEMM everywhere
-    if (off || S != 8 || C % CH_KC != 0) return false;
+    if (S != 8 || C % CH_KC != 0) return false;
     if (Cout == 32) return epi == EPI_STORE || epi == EPI_RESID_SCALE;
     if (Cout == 16) return epi == EPI_NCDHW;
     return false;

@@ -2,7 +2,6 @@
 // conditioning hoist, and the per-step forward schedule (one stream, ~12 launches per block, no host sync).
 //   reference: models/dit_crossattn.py:111-213, models/attention.py, models/utils.py
 #include <cstdlib>
-#include <cstring>
 #include <string>
 #include <vector>
 
@@ -194,44 +193,9 @@ TsWs carve_ts(const tpx_dit* h, int K, uint8_t* base) {
     return w;
 }
 
-// tile_n: 0 = automatic; > 0 = that tile width
-int gemm_linear(const __half* A, int lda, const __half* W, int M, int N, int K, int epi, const GemmArgs& args, int tile_n, cudaStream_t st) {
-    GemmProblem p{};
-    p.A = A; p.a_mode = AMODE_LINEAR; p.lda = lda; p.W = W; p.M = M; p.N = N; p.K = K;
-    p.epi = epi; p.args = args;
-    TPX_CHECK(tile_n >= 0, TPX_ERR_ARG, "gemm: tile width %d (0 = automatic, or one of the instantiated widths)", tile_n);
-    p.BN = tile_n > 0 ? tile_n : gemm_pick_bn(p);
-    return launch_gemm(p, st);
-}
 }  // namespace
 
 extern "C" {
-
-int tpx_version(void) { return TPX_VERSION; }
-const char* tpx_last_error(void) { return tpx::last_error(); }
-
-int64_t tpx_launch_count(void) { return tpx::launch_count(); }
-int tpx_profile_begin(void) { tpx::prof_begin(); return TPX_OK; }
-int tpx_profile_end(float* ms_by_class, int64_t* launches_by_class) {
-    TPX_CHECK(ms_by_class != nullptr && launches_by_class != nullptr, TPX_ERR_ARG, "profile_end: null argument");
-    long long n[PROF_NCLASS];
-    int rc = tpx::prof_end(ms_by_class, n);
-    for (int i = 0; i < PROF_NCLASS; ++i) launches_by_class[i] = n[i];
-    return rc;
-}
-
-int tpx_device_check(void) {
-    static int checked[64] = {0};   // per device ordinal: 0 unknown, 1 ok (attribute queries are cheap, but this sits on per-kernel entry points)
-    int dev = 0;
-    TPX_CUDA(cudaGetDevice(&dev));
-    if (dev >= 0 && dev < 64 && checked[dev] == 1) return TPX_OK;
-    int major = 0, minor = 0;
-    TPX_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    TPX_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-    TPX_CHECK(major == 9, TPX_ERR_CUDA, "libtpx_b200 is built for sm_90a only; device %d is sm_%d%d (no fallback path exists)", dev, major, minor);
-    if (dev >= 0 && dev < 64) checked[dev] = 1;
-    return TPX_OK;
-}
 
 int tpx_dit_create(const tpx_dit_config* c, tpx_dit** out) {
     TPX_CHECK(c != nullptr && out != nullptr, TPX_ERR_ARG, "dit_create: null argument");
@@ -243,8 +207,7 @@ int tpx_dit_create(const tpx_dit_config* c, tpx_dit** out) {
               "dit_create: condition/mlp/out channels must be multiples of 8 (%d/%d/%d)", c->condition_channels, c->mlp_hidden, c->out_channels);
     TPX_CHECK(c->depth > 0 && c->seq_length > 0 && c->in_channels > 0, TPX_ERR_SHAPE, "dit_create: non-positive size");
     TPX_CHECK(c->in_channels % 4 == 0, TPX_ERR_SHAPE, "dit_create: in_channels %d must be a multiple of 4", c->in_channels);
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
+    TPX_DEVICE_GUARD();
     tpx_dit* h = new tpx_dit();
     h->N = c->seq_length; h->Cin = c->in_channels; h->Cout = c->out_channels; h->Dc = c->condition_channels;
     h->D = c->hidden_size; h->L = c->depth; h->H = c->num_heads; h->Dm = c->mlp_hidden; h->Dh = Dh;
@@ -538,110 +501,6 @@ int tpx_dit_debug_residual(const tpx_dit* h, const void* ws, int n_seq, float* o
     const DitWs w = carve_ws(h, n_seq, static_cast<uint8_t*>(const_cast<void*>(ws)));
     TPX_CUDA(cudaMemcpyAsync(out, w.xres, static_cast<size_t>(n_seq) * h->N * h->D * 4, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
     return TPX_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// sampler + per-kernel entry points
-// ---------------------------------------------------------------------------------------------------------
-int tpx_sampler_step(int ddim, const float* x, const void* mo, int mo_dtype, const float* noise, int64_t n, int C, const tpx_sampler_coefs* k,
-                     float* x_prev, float* x0, void* stream) {
-    TPX_CHECK(x != nullptr && mo != nullptr && k != nullptr && x_prev != nullptr && x0 != nullptr, TPX_ERR_ARG, "sampler_step: null argument");
-    TPX_CHECK(C > 0 && n % C == 0, TPX_ERR_SHAPE, "sampler_step: n %lld not a multiple of C %d", (long long)n, C);
-    SamplerCoefs c;
-    static_assert(sizeof(SamplerCoefs) == sizeof(tpx_sampler_coefs), "coef struct mirror");
-    memcpy(&c, k, sizeof(c));
-    return launch_sampler_step(ddim, x, mo, mo_dtype == TPX_DTYPE_F16, noise, n, C, c, x_prev, x0, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_latent_split(const float* sample, const float* mean, const float* stdv, float inv_nf, int64_t T, int C, float* srt, float* z, void* stream) {
-    TPX_CHECK(sample != nullptr && srt != nullptr && z != nullptr, TPX_ERR_ARG, "latent_split: null argument");
-    TPX_CHECK((mean == nullptr) == (stdv == nullptr), TPX_ERR_ARG, "latent_split: latent_mean and latent_std go together");
-    TPX_CHECK(T >= 0 && C > 4, TPX_ERR_SHAPE, "latent_split: need more than 4 channels (got %d)", C);
-    return launch_latent_split(sample, mean, stdv, inv_nf, T, C, srt, z, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_primvolume_pack(const float* srt, const void* decoded, int decoded_dtype, int64_t T, int F, int vox, int srt_fix, float* out, void* stream) {
-    TPX_CHECK(srt != nullptr && decoded != nullptr && out != nullptr, TPX_ERR_ARG, "primvolume_pack: null argument");
-    TPX_CHECK(decoded_dtype == TPX_DTYPE_F32 || decoded_dtype == TPX_DTYPE_F16, TPX_ERR_ARG, "primvolume_pack: dtype %d", decoded_dtype);
-    return launch_primvolume_pack(srt, decoded, decoded_dtype == TPX_DTYPE_F16, T, F, vox, srt_fix, out, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_linear(const void* A, int lda, const void* W, const void* bias, void* out, int ldo, int M, int N, int K, int act, float post_scale, int tile_n,
-               void* stream) {
-    TPX_CHECK(A != nullptr && W != nullptr && out != nullptr, TPX_ERR_ARG, "linear: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    GemmArgs a{};
-    a.bias = static_cast<const __half*>(bias); a.post_scale = post_scale; a.out0 = static_cast<__half*>(out); a.ldo = ldo;
-    return gemm_linear(static_cast<const __half*>(A), lda, static_cast<const __half*>(W), M, N, K, act ? EPI_GELU : EPI_STORE, a, tile_n,
-                       static_cast<cudaStream_t>(stream));
-}
-
-int tpx_linear_gated(const void* A, int lda, const void* W, const void* bias, const void* gate, int gate_bstride, int gate_batches, int rows_per_batch,
-                     float* xres, int ldx, int M, int N, int K, int tile_n, void* stream) {
-    TPX_CHECK(A != nullptr && W != nullptr && gate != nullptr && xres != nullptr, TPX_ERR_ARG, "linear_gated: null argument");
-    TPX_CHECK(gate_batches > 0 && rows_per_batch > 0, TPX_ERR_ARG, "linear_gated: bad gate batching");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    GemmArgs a{};
-    a.bias = static_cast<const __half*>(bias); a.post_scale = 1.0f; a.xres = xres; a.ldx = ldx;
-    a.gate = static_cast<const __half*>(gate); a.gate_bstride = gate_bstride; a.rows_per_batch = rows_per_batch; a.gate_batches = gate_batches;
-    return gemm_linear(static_cast<const __half*>(A), lda, static_cast<const __half*>(W), M, N, K, EPI_GATED, a, tile_n, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_linear_heads(const void* A, int lda, const void* W, const void* bias, void* out0, void* out1, void* out2, int M, int N, int K, int split_cols,
-                     int H, int Dh, int DhP, int n_seq_tokens, float post_scale, int tile_n, int transposed_which, int transposed_ld, void* stream) {
-    TPX_CHECK(A != nullptr && W != nullptr && out0 != nullptr, TPX_ERR_ARG, "linear_heads: null argument");
-    TPX_CHECK(Dh % 8 == 0 && DhP % 8 == 0 && DhP >= Dh && split_cols == H * Dh && N % split_cols == 0, TPX_ERR_SHAPE, "linear_heads: bad head geometry");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    GemmArgs a{};
-    a.bias = static_cast<const __half*>(bias); a.post_scale = post_scale;
-    a.out0 = static_cast<__half*>(out0); a.out1 = static_cast<__half*>(out1); a.out2 = static_cast<__half*>(out2);
-    a.split_cols = split_cols; a.Dh = Dh; a.DhP = DhP; a.H = H; a.Nseq = n_seq_tokens;
-    a.vt_which_plus1 = transposed_which >= 0 ? transposed_which + 1 : 0;
-    a.vt_ld = transposed_ld;
-    if (Dh % 24 == 0 && n_seq_tokens % 32 == 0 && n_seq_tokens > 0 && M % n_seq_tokens == 0) {
-        // bulk-store epilogue: it writes the Dh real columns only, so the padding is cleared here (the DiT forward clears its
-        // workspace once per call instead)
-        void* outs[3] = {out0, out1, out2};
-        const size_t per = static_cast<size_t>(M / n_seq_tokens) * H * n_seq_tokens * DhP * 2;
-        for (int w = 0; w < N / split_cols && w < 3; ++w) {
-            TPX_CHECK(outs[w] != nullptr, TPX_ERR_ARG, "linear_heads: output %d is null", w);
-            const size_t bytes = w == transposed_which ? static_cast<size_t>(M / n_seq_tokens) * H * DhP * transposed_ld * 2 : per;
-            TPX_CUDA(cudaMemsetAsync(outs[w], 0, bytes, static_cast<cudaStream_t>(stream)));
-        }
-        a.heads_tma = 1;
-    }
-    return gemm_linear(static_cast<const __half*>(A), lda, static_cast<const __half*>(W), M, N, K, EPI_HEADS, a, tile_n, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_ln_modulate(float* x, int rows, int D, float eps, const void* shift, const void* scale, int mod_bstride, int rows_per_batch, int mod_batches,
-                    void* out, const void* pre_gate, const void* pre_const, int pre_row0, void* stream) {
-    TPX_CHECK(x != nullptr && shift != nullptr && scale != nullptr && out != nullptr, TPX_ERR_ARG, "ln_modulate: null argument");
-    TPX_CHECK(rows_per_batch > 0 && mod_batches > 0, TPX_ERR_ARG, "ln_modulate: bad batching");
-    return launch_ln_modulate(x, rows, D, eps, static_cast<const __half*>(shift), static_cast<const __half*>(scale), mod_bstride, rows_per_batch,
-                              mod_batches, static_cast<__half*>(out), static_cast<const __half*>(pre_gate), static_cast<const __half*>(pre_const),
-                              pre_row0, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_attention(const void* q, const void* k, const void* v, void* out, int B, int H, int Nq, int Nk, int Dh, int DhP, float scale, void* stream) {
-    TPX_CHECK(q != nullptr && k != nullptr && v != nullptr && out != nullptr, TPX_ERR_ARG, "attention: null argument");
-    return launch_attention(static_cast<const __half*>(q), static_cast<const __half*>(k), static_cast<const __half*>(v), static_cast<__half*>(out), B, H,
-                            Nq, Nk, Dh, DhP, scale, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_attention_tc(const void* q, const void* k, const void* vT, void* out, int B, int H, int Nq, int Nk, int NkPad, int Dh, float scale, void* stream) {
-    TPX_CHECK(q != nullptr && k != nullptr && vT != nullptr && out != nullptr, TPX_ERR_ARG, "attention_tc: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_attention_tc(static_cast<const __half*>(q), static_cast<const __half*>(k), static_cast<const __half*>(vT), static_cast<__half*>(out), B, H,
-                               Nq, Nk, NkPad, Dh, scale, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_cfg_combine(const void* both, int64_t n_half, float s, void* out, void* stream) {
-    TPX_CHECK(both != nullptr && out != nullptr, TPX_ERR_ARG, "cfg_combine: null argument");
-    return launch_cfg_combine(static_cast<const __half*>(both), n_half, s, static_cast<__half*>(out), static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -317,7 +317,7 @@ __device__ __forceinline__ float mo_load<float>(const float* p, size_t i) { retu
 
 template <typename MO>
 __global__ void ddim_step_kernel(const float* __restrict__ x, const MO* __restrict__ mo, const float* __restrict__ noise, long long n, int C,
-                                 SamplerCoefs k, float* __restrict__ x_prev, float* __restrict__ x0_out) {
+                                 tpx_sampler_coefs k, float* __restrict__ x_prev, float* __restrict__ x0_out) {
     const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const long long tok = i / C;
@@ -335,7 +335,7 @@ __global__ void ddim_step_kernel(const float* __restrict__ x, const MO* __restri
 
 template <typename MO>
 __global__ void ddpm_step_kernel(const float* __restrict__ x, const MO* __restrict__ mo, const float* __restrict__ noise, long long n, int C,
-                                 SamplerCoefs k, float* __restrict__ x_prev, float* __restrict__ x0_out) {
+                                 tpx_sampler_coefs k, float* __restrict__ x_prev, float* __restrict__ x0_out) {
     const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const long long tok = i / C;
@@ -361,21 +361,6 @@ __global__ void ddpm_step_kernel(const float* __restrict__ x, const MO* __restri
     x0_out[i] = x0;
 }
 
-int launch_sampler_step(int ddim, const float* x, const void* mo, int mo_is_half, const float* noise, long long n, int C, const SamplerCoefs& k,
-                        float* x_prev, float* x0_out, cudaStream_t st) {
-    if (n <= 0) return TPX_OK;
-    const unsigned grid = static_cast<unsigned>((n + 255) / 256);
-    ProfScope prof(PROF_ELEMWISE, st);
-    if (ddim) {
-        if (mo_is_half) ddim_step_kernel<__half><<<grid, 256, 0, st>>>(x, static_cast<const __half*>(mo), noise, n, C, k, x_prev, x0_out);
-        else ddim_step_kernel<float><<<grid, 256, 0, st>>>(x, static_cast<const float*>(mo), noise, n, C, k, x_prev, x0_out);
-    } else {
-        if (mo_is_half) ddpm_step_kernel<__half><<<grid, 256, 0, st>>>(x, static_cast<const __half*>(mo), noise, n, C, k, x_prev, x0_out);
-        else ddpm_step_kernel<float><<<grid, 256, 0, st>>>(x, static_cast<const float*>(mo), noise, n, C, k, x_prev, x0_out);
-    }
-    TPX_LAUNCH_CHECK();
-    return TPX_OK;
-}
 
 // =====================================================================================================
 // dtype conversion (weight ingestion: fp32/fp16 checkpoint tensor -> packed fp16 slot; y -> fp16)
@@ -457,14 +442,6 @@ __global__ void latent_split_kernel(const float* __restrict__ x, const float* __
     else z[tok * (C - 4) + (c - 4)] = v;
 }
 
-int launch_latent_split(const float* x, const float* mean, const float* stdv, float inv_nf, long long T, int C, float* srt, float* z, cudaStream_t st) {
-    const long long n = T * C;
-    if (n <= 0) return TPX_OK;
-    ProfScope prof(PROF_ELEMWISE, st);
-    latent_split_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(x, mean, stdv, inv_nf, T, C, srt, z);
-    TPX_LAUNCH_CHECK();
-    return TPX_OK;
-}
 
 template <typename T_IN>
 __global__ void primvolume_pack_kernel(const float* __restrict__ srt, const T_IN* __restrict__ dec, long long T, int F, int vox, int srt_fix,
@@ -500,16 +477,77 @@ __global__ void primvolume_pack_kernel(const float* __restrict__ srt, const T_IN
     *reinterpret_cast<float4*>(out + tok * (4 + F) + g * 4) = o;
 }
 
-int launch_primvolume_pack(const float* srt, const void* dec, int dec_is_half, long long T, int F, int vox, int srt_fix, float* out, cudaStream_t st) {
+
+}  // namespace tpx
+
+using namespace tpx;
+
+extern "C" {
+
+int tpx_ln_modulate(float* x, int rows, int D, float eps, const void* shift, const void* scale, int mod_bstride, int rows_per_batch, int mod_batches,
+                    void* out, const void* pre_gate, const void* pre_const, int pre_row0, void* stream) {
+    TPX_CHECK(x != nullptr && shift != nullptr && scale != nullptr && out != nullptr, TPX_ERR_ARG, "ln_modulate: null argument");
+    TPX_CHECK(rows_per_batch > 0 && mod_batches > 0, TPX_ERR_ARG, "ln_modulate: bad batching");
+    TPX_DEVICE_GUARD();
+    return launch_ln_modulate(x, rows, D, eps, static_cast<const __half*>(shift), static_cast<const __half*>(scale), mod_bstride, rows_per_batch,
+                              mod_batches, static_cast<__half*>(out), static_cast<const __half*>(pre_gate), static_cast<const __half*>(pre_const),
+                              pre_row0, static_cast<cudaStream_t>(stream));
+}
+
+int tpx_cfg_combine(const void* both, int64_t n_half, float s, void* out, void* stream) {
+    TPX_CHECK(both != nullptr && out != nullptr, TPX_ERR_ARG, "cfg_combine: null argument");
+    TPX_DEVICE_GUARD();
+    return launch_cfg_combine(static_cast<const __half*>(both), n_half, s, static_cast<__half*>(out), static_cast<cudaStream_t>(stream));
+}
+
+int tpx_sampler_step(int ddim, const float* x, const void* mo, int mo_dtype, const float* noise, int64_t n, int C, const tpx_sampler_coefs* k,
+                     float* x_prev, float* x0, void* stream) {
+    TPX_CHECK(x != nullptr && mo != nullptr && k != nullptr && x_prev != nullptr && x0 != nullptr, TPX_ERR_ARG, "sampler_step: null argument");
+    TPX_CHECK(C > 0 && n % C == 0, TPX_ERR_SHAPE, "sampler_step: n %lld not a multiple of C %d", (long long)n, C);
+    if (n <= 0) return TPX_OK;
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const unsigned grid = static_cast<unsigned>((n + 255) / 256);
+    ProfScope prof(PROF_ELEMWISE, st);
+    if (ddim) {
+        if (mo_dtype == TPX_DTYPE_F16) ddim_step_kernel<__half><<<grid, 256, 0, st>>>(x, static_cast<const __half*>(mo), noise, n, C, *k, x_prev, x0);
+        else ddim_step_kernel<float><<<grid, 256, 0, st>>>(x, static_cast<const float*>(mo), noise, n, C, *k, x_prev, x0);
+    } else {
+        if (mo_dtype == TPX_DTYPE_F16) ddpm_step_kernel<__half><<<grid, 256, 0, st>>>(x, static_cast<const __half*>(mo), noise, n, C, *k, x_prev, x0);
+        else ddpm_step_kernel<float><<<grid, 256, 0, st>>>(x, static_cast<const float*>(mo), noise, n, C, *k, x_prev, x0);
+    }
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+int tpx_latent_split(const float* sample, const float* mean, const float* stdv, float inv_nf, int64_t T, int C, float* srt, float* z, void* stream) {
+    TPX_CHECK(sample != nullptr && srt != nullptr && z != nullptr, TPX_ERR_ARG, "latent_split: null argument");
+    TPX_CHECK((mean == nullptr) == (stdv == nullptr), TPX_ERR_ARG, "latent_split: latent_mean and latent_std go together");
+    TPX_CHECK(T >= 0 && C > 4, TPX_ERR_SHAPE, "latent_split: need more than 4 channels (got %d)", C);
+    const long long n = T * C;
+    if (n <= 0) return TPX_OK;
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ProfScope prof(PROF_ELEMWISE, st);
+    latent_split_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(sample, mean, stdv, inv_nf, T, C, srt, z);
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+int tpx_primvolume_pack(const float* srt, const void* dec, int dec_dtype, int64_t T, int F, int vox, int srt_fix, float* out, void* stream) {
+    TPX_CHECK(srt != nullptr && dec != nullptr && out != nullptr, TPX_ERR_ARG, "primvolume_pack: null argument");
+    TPX_CHECK(dec_dtype == TPX_DTYPE_F32 || dec_dtype == TPX_DTYPE_F16, TPX_ERR_ARG, "primvolume_pack: dtype %d", dec_dtype);
     TPX_CHECK(F % 4 == 0 && vox % 4 == 0 && vox <= F, TPX_ERR_SHAPE, "primvolume_pack: feature length %d / voxel count %d must be multiples of 4", F, vox);
     const long long n = T * (1 + F / 4);
     if (n <= 0) return TPX_OK;
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     ProfScope prof(PROF_ELEMWISE, st);
     const unsigned grid = static_cast<unsigned>((n + 255) / 256);
-    if (dec_is_half) primvolume_pack_kernel<__half><<<grid, 256, 0, st>>>(srt, static_cast<const __half*>(dec), T, F, vox, srt_fix, out);
+    if (dec_dtype == TPX_DTYPE_F16) primvolume_pack_kernel<__half><<<grid, 256, 0, st>>>(srt, static_cast<const __half*>(dec), T, F, vox, srt_fix, out);
     else primvolume_pack_kernel<float><<<grid, 256, 0, st>>>(srt, static_cast<const float*>(dec), T, F, vox, srt_fix, out);
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }
 
-}  // namespace tpx
+}  // extern "C"

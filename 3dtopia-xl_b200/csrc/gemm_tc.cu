@@ -1,85 +1,11 @@
-// Host launcher for the wgmma GEMM: tensor-map construction (cached), tile-shape dispatch.
+// Host launcher for the wgmma GEMM: tensor-map construction (cached), tile-shape dispatch, and the linear-GEMM entry points.
 #include "gemm_tc.cuh"
 
-#include <atomic>
-#include <cstdarg>
-#include <cstdio>
-#include <cstring>
 #include <map>
 #include <mutex>
 #include <tuple>
-#include <vector>
 
 namespace tpx {
-
-// ---- error plumbing -------------------------------------------------------------------------------------
-static thread_local char g_err[512] = "";
-void set_error(const char* fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-}
-const char* last_error() { return g_err; }
-int cuda_fail(cudaError_t e, const char* what) {
-    set_error("CUDA error %d (%s) at %s", static_cast<int>(e), cudaGetErrorString(e), what);
-    return TPX_ERR_CUDA;
-}
-
-// ---- launch counter + optional event profiling ------------------------------------------------------------------
-static std::atomic<long long> g_launches{0};
-void note_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
-long long launch_count() { return g_launches.load(); }
-
-struct ProfRec { int cls; cudaEvent_t a, b; };
-static bool g_prof_on = false;
-static std::vector<ProfRec> g_prof_recs;
-static std::vector<cudaEvent_t> g_prof_pool;
-static cudaEvent_t prof_event() {
-    if (!g_prof_pool.empty()) { cudaEvent_t e = g_prof_pool.back(); g_prof_pool.pop_back(); return e; }
-    cudaEvent_t e = nullptr;
-    cudaEventCreate(&e);
-    return e;
-}
-ProfScope::ProfScope(int cls, cudaStream_t s) : idx(-1), st(s) {
-    if (!g_prof_on) return;
-    ProfRec r{cls, prof_event(), prof_event()};
-    cudaEventRecord(r.a, st);
-    idx = static_cast<int>(g_prof_recs.size());
-    g_prof_recs.push_back(r);
-}
-ProfScope::~ProfScope() {
-    if (idx >= 0) cudaEventRecord(g_prof_recs[idx].b, st);
-}
-void prof_begin() {
-    for (auto& r : g_prof_recs) { g_prof_pool.push_back(r.a); g_prof_pool.push_back(r.b); }
-    g_prof_recs.clear();
-    g_prof_on = true;
-}
-int prof_end(float* ms_by_class, long long* n_by_class) {
-    g_prof_on = false;
-    TPX_CUDA(cudaDeviceSynchronize());
-    for (int i = 0; i < PROF_NCLASS; ++i) { ms_by_class[i] = 0.f; n_by_class[i] = 0; }
-    for (auto& r : g_prof_recs) {
-        float ms = 0.f;
-        if (cudaEventElapsedTime(&ms, r.a, r.b) == cudaSuccess) { ms_by_class[r.cls] += ms; n_by_class[r.cls] += 1; }
-        g_prof_pool.push_back(r.a);
-        g_prof_pool.push_back(r.b);
-    }
-    g_prof_recs.clear();
-    return TPX_OK;
-}
-
-int gemm_num_sms() {
-    static int n = 0;
-    if (n == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 132;
-    }
-    return n;
-}
 
 // ---- tensor maps ------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -327,7 +253,6 @@ int launch_gemm(const GemmProblem& p, cudaStream_t stream) {
     TPX_CASE(256, 64, AMODE_CONV3, EPI_STORE)
     TPX_CASE(256, 64, AMODE_CONV3, EPI_RESID_SCALE)
     TPX_CASE(256, 64, AMODE_LINEAR, EPI_RESID_SCALE)
-    TPX_CASE(256, 64, AMODE_LINEAR, EPI_CONVT2)
     TPX_CASE(32, 64, AMODE_CONV3, EPI_STORE)
     TPX_CASE(32, 64, AMODE_LINEAR, EPI_STORE)
     TPX_CASE(32, 32, AMODE_CONV3, EPI_STORE)
@@ -338,4 +263,66 @@ int launch_gemm(const GemmProblem& p, cudaStream_t stream) {
     return TPX_ERR_SHAPE;
 }
 
+int gemm_linear(const __half* A, int lda, const __half* W, int M, int N, int K, int epi, const GemmArgs& args, int tile_n, cudaStream_t st) {
+    GemmProblem p{};
+    p.A = A; p.a_mode = AMODE_LINEAR; p.lda = lda; p.W = W; p.M = M; p.N = N; p.K = K;
+    p.epi = epi; p.args = args;
+    TPX_CHECK(tile_n >= 0, TPX_ERR_ARG, "gemm: tile width %d (0 = automatic, or one of the instantiated widths)", tile_n);
+    p.BN = tile_n > 0 ? tile_n : gemm_pick_bn(p);
+    return launch_gemm(p, st);
+}
+
 }  // namespace tpx
+
+using namespace tpx;
+
+extern "C" {
+
+int tpx_linear(const void* A, int lda, const void* W, const void* bias, void* out, int ldo, int M, int N, int K, int act, float post_scale, int tile_n,
+               void* stream) {
+    TPX_CHECK(A != nullptr && W != nullptr && out != nullptr, TPX_ERR_ARG, "linear: null argument");
+    TPX_DEVICE_GUARD();
+    GemmArgs a{};
+    a.bias = static_cast<const __half*>(bias); a.post_scale = post_scale; a.out0 = static_cast<__half*>(out); a.ldo = ldo;
+    return gemm_linear(static_cast<const __half*>(A), lda, static_cast<const __half*>(W), M, N, K, act ? EPI_GELU : EPI_STORE, a, tile_n,
+                       static_cast<cudaStream_t>(stream));
+}
+
+int tpx_linear_gated(const void* A, int lda, const void* W, const void* bias, const void* gate, int gate_bstride, int gate_batches, int rows_per_batch,
+                     float* xres, int ldx, int M, int N, int K, int tile_n, void* stream) {
+    TPX_CHECK(A != nullptr && W != nullptr && gate != nullptr && xres != nullptr, TPX_ERR_ARG, "linear_gated: null argument");
+    TPX_CHECK(gate_batches > 0 && rows_per_batch > 0, TPX_ERR_ARG, "linear_gated: bad gate batching");
+    TPX_DEVICE_GUARD();
+    GemmArgs a{};
+    a.bias = static_cast<const __half*>(bias); a.post_scale = 1.0f; a.xres = xres; a.ldx = ldx;
+    a.gate = static_cast<const __half*>(gate); a.gate_bstride = gate_bstride; a.rows_per_batch = rows_per_batch; a.gate_batches = gate_batches;
+    return gemm_linear(static_cast<const __half*>(A), lda, static_cast<const __half*>(W), M, N, K, EPI_GATED, a, tile_n, static_cast<cudaStream_t>(stream));
+}
+
+int tpx_linear_heads(const void* A, int lda, const void* W, const void* bias, void* out0, void* out1, void* out2, int M, int N, int K, int split_cols,
+                     int H, int Dh, int DhP, int n_seq_tokens, float post_scale, int tile_n, int transposed_which, int transposed_ld, void* stream) {
+    TPX_CHECK(A != nullptr && W != nullptr && out0 != nullptr, TPX_ERR_ARG, "linear_heads: null argument");
+    TPX_CHECK(Dh % 8 == 0 && DhP % 8 == 0 && DhP >= Dh && split_cols == H * Dh && N % split_cols == 0, TPX_ERR_SHAPE, "linear_heads: bad head geometry");
+    TPX_DEVICE_GUARD();
+    GemmArgs a{};
+    a.bias = static_cast<const __half*>(bias); a.post_scale = post_scale;
+    a.out0 = static_cast<__half*>(out0); a.out1 = static_cast<__half*>(out1); a.out2 = static_cast<__half*>(out2);
+    a.split_cols = split_cols; a.Dh = Dh; a.DhP = DhP; a.H = H; a.Nseq = n_seq_tokens;
+    a.vt_which_plus1 = transposed_which >= 0 ? transposed_which + 1 : 0;
+    a.vt_ld = transposed_ld;
+    if (Dh % 24 == 0 && n_seq_tokens % 32 == 0 && n_seq_tokens > 0 && M % n_seq_tokens == 0) {
+        // bulk-store epilogue: it writes the Dh real columns only, so the padding is cleared here (the DiT forward clears its
+        // workspace once per call instead)
+        void* outs[3] = {out0, out1, out2};
+        const size_t per = static_cast<size_t>(M / n_seq_tokens) * H * n_seq_tokens * DhP * 2;
+        for (int w = 0; w < N / split_cols && w < 3; ++w) {
+            TPX_CHECK(outs[w] != nullptr, TPX_ERR_ARG, "linear_heads: output %d is null", w);
+            const size_t bytes = w == transposed_which ? static_cast<size_t>(M / n_seq_tokens) * H * DhP * transposed_ld * 2 : per;
+            TPX_CUDA(cudaMemsetAsync(outs[w], 0, bytes, static_cast<cudaStream_t>(stream)));
+        }
+        a.heads_tma = 1;
+    }
+    return gemm_linear(static_cast<const __half*>(A), lda, static_cast<const __half*>(W), M, N, K, EPI_HEADS, a, tile_n, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

@@ -30,7 +30,6 @@ enum GemmEpiMode : int {
     EPI_HEADS = 2,       // split columns into (which, head, d) -> out{which}[b,head,n,DhP]  (zero pad written)
     EPI_GATED = 3,       // xres[row*ldx+col] += float( h( gate[b,col] * h(acc+bias) ) )
     EPI_RESID_SCALE = 4, // out0 = h( (acc + bias + resid[row*ldo+col]) * alpha )
-    EPI_CONVT2 = 5,      // k2s2 transposed conv scatter: col=(abc,co), row=(p,z,y,x)@4^3 -> channels-last 8^3
     EPI_NCDHW = 6,       // out[(p*Cout+co)*S3 + vox] = acc + bias   (fp32 or fp16 out, co < n_valid)
 };
 enum GemmAMode : int { AMODE_LINEAR = 0, AMODE_CONV3 = 1 };
@@ -238,20 +237,6 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, const float* __rest
 #pragma unroll
             for (int i = 0; i < 8; ++i) o.h[i] = __float2half_rn((v[j * 8 + i] + __half2float(rs[j].h[i])) * g.alpha);
             if (ok[j]) *reinterpret_cast<uint4*>(g.out0 + off + j * 8) = o.u;
-        }
-    } else if constexpr (EPI == EPI_CONVT2) {
-        const int p = row >> 6, vox = row & 63;
-        const int z = vox >> 4, y = (vox >> 2) & 3, x = vox & 3;
-#pragma unroll
-        for (int j = 0; j < NG; ++j) {
-            const int col = col0 + j * 8;
-            const int abc = col / g.split_cols;
-            const int co = col - abc * g.split_cols;
-            const int oz = 2 * z + (abc >> 2), oy = 2 * y + ((abc >> 1) & 1), ox = 2 * x + (abc & 1);
-            Pack8 o;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) o.h[i] = __float2half_rn(v[j * 8 + i]);
-            if (ok[j]) *reinterpret_cast<uint4*>(g.out0 + (static_cast<size_t>(p) * 512 + (oz * 8 + oy) * 8 + ox) * g.split_cols + co) = o.u;
         }
     } else if constexpr (EPI == EPI_NCDHW) {
         const int p = row / g.S3, vox = row - p * g.S3;
@@ -658,6 +643,7 @@ struct GemmProblem {
 };
 int launch_gemm(const GemmProblem& p, cudaStream_t stream);
 int gemm_pick_bn(const GemmProblem& p);
-int gemm_num_sms();
+// linear GEMM out = A[M,K] W[N,K]^T through `epi`; tile_n: 0 = automatic (gemm_pick_bn), > 0 = that tile width
+int gemm_linear(const __half* A, int lda, const __half* W, int M, int N, int K, int epi, const GemmArgs& args, int tile_n, cudaStream_t st);
 
 }  // namespace tpx

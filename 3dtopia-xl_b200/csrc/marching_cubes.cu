@@ -238,64 +238,52 @@ int mc_check(const float* vol, long long X, long long Y, long long Z, const void
 }
 }  // namespace
 
-size_t mc_workspace_bytes(long long X, long long Y, long long Z) {
-    if (X < 2 || Y < 2 || Z < 2 || X >= MC_INDEX_LIMIT || Y >= MC_INDEX_LIMIT || Z >= MC_INDEX_LIMIT || X * Y >= MC_INDEX_LIMIT || X * Y * Z >= MC_INDEX_LIMIT)
-        return 0;
-    const long long N = X * Y * Z;
-    return mc_bytes(N, (N + MC_THREADS - 1) / MC_THREADS);
-}
-
-int launch_mc_count(const float* vol, long long X, long long Y, long long Z, float iso, void* ws, size_t ws_bytes, long long* counts, cudaStream_t st) {
-    long long N, nb;
-    const int rc = mc_check(vol, X, Y, Z, ws, ws_bytes, &N, &nb);
-    if (rc != TPX_OK) return rc;
-    TPX_CHECK(counts != nullptr, TPX_ERR_ARG, "marching_cubes: null counts");
-    const McPtrs w = mc_carve(ws, N, nb);
-    ProfScope prof(PROF_VAE_MISC, st);
-    mc_count_kernel<<<static_cast<unsigned>(nb), MC_THREADS, 0, st>>>(vol, static_cast<int>(X), static_cast<int>(Y), static_cast<int>(Z), iso, w.code, w.blk_v,
-                                                                      w.blk_f);
-    TPX_LAUNCH_CHECK();
-    mc_scan_kernel<<<1, MC_SCAN_THREADS, 0, st>>>(w.blk_v, w.blk_f, static_cast<int>(nb), w.off_v, w.off_f, w.hdr, counts);
-    TPX_LAUNCH_CHECK();
-    return TPX_OK;
-}
-
-int launch_mc_emit(const float* vol, long long X, long long Y, long long Z, float iso, const float origin[3], const float spacing[3], void* ws, size_t ws_bytes,
-                   float* verts, long long* faces, cudaStream_t st) {
-    long long N, nb;
-    const int rc = mc_check(vol, X, Y, Z, ws, ws_bytes, &N, &nb);
-    if (rc != TPX_OK) return rc;
-    const McPtrs w = mc_carve(ws, N, nb);
-    ProfScope prof(PROF_VAE_MISC, st);
-    const int x = static_cast<int>(X), y = static_cast<int>(Y), z = static_cast<int>(Z);
-    mc_vertex_kernel<<<static_cast<unsigned>(nb), MC_THREADS, 0, st>>>(vol, x, y, z, iso, make_float3(origin[0], origin[1], origin[2]),
-                                                                       make_float3(spacing[0], spacing[1], spacing[2]), w.code, w.off_v, w.hdr, w.vbase, verts);
-    TPX_LAUNCH_CHECK();
-    mc_face_kernel<<<static_cast<unsigned>(nb), MC_THREADS, 0, st>>>(x, y, z, w.code, w.off_f, w.hdr, w.vbase, faces);
-    TPX_LAUNCH_CHECK();
-    return TPX_OK;
-}
-
 }  // namespace tpx
 
 using namespace tpx;
 
 extern "C" {
 
-size_t tpx_mc_workspace_bytes(int64_t X, int64_t Y, int64_t Z) { return mc_workspace_bytes(X, Y, Z); }
+size_t tpx_mc_workspace_bytes(int64_t X, int64_t Y, int64_t Z) {
+    if (X < 2 || Y < 2 || Z < 2 || X >= MC_INDEX_LIMIT || Y >= MC_INDEX_LIMIT || Z >= MC_INDEX_LIMIT || X * Y >= MC_INDEX_LIMIT || X * Y * Z >= MC_INDEX_LIMIT)
+        return 0;
+    const long long N = X * Y * Z;
+    return mc_bytes(N, (N + MC_THREADS - 1) / MC_THREADS);
+}
 
 int tpx_mc_count(const float* vol, int64_t X, int64_t Y, int64_t Z, float iso, void* ws, size_t ws_bytes, int64_t* counts, void* stream) {
-    const int rc = tpx_device_check();
+    long long N, nb;
+    const int rc = mc_check(vol, X, Y, Z, ws, ws_bytes, &N, &nb);
     if (rc != TPX_OK) return rc;
-    return launch_mc_count(vol, X, Y, Z, iso, ws, ws_bytes, reinterpret_cast<long long*>(counts), static_cast<cudaStream_t>(stream));
+    TPX_CHECK(counts != nullptr, TPX_ERR_ARG, "marching_cubes: null counts");
+    TPX_DEVICE_GUARD();
+    const McPtrs w = mc_carve(ws, N, nb);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ProfScope prof(PROF_VAE_MISC, st);
+    mc_count_kernel<<<static_cast<unsigned>(nb), MC_THREADS, 0, st>>>(vol, static_cast<int>(X), static_cast<int>(Y), static_cast<int>(Z), iso, w.code, w.blk_v,
+                                                                      w.blk_f);
+    TPX_LAUNCH_CHECK();
+    mc_scan_kernel<<<1, MC_SCAN_THREADS, 0, st>>>(w.blk_v, w.blk_f, static_cast<int>(nb), w.off_v, w.off_f, w.hdr, reinterpret_cast<long long*>(counts));
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
 }
 
 int tpx_mc_emit(const float* vol, int64_t X, int64_t Y, int64_t Z, float iso, float ox, float oy, float oz, float sx, float sy, float sz, void* ws, size_t ws_bytes,
                 float* verts, int64_t* faces, void* stream) {
-    const int rc = tpx_device_check();
+    long long N, nb;
+    const int rc = mc_check(vol, X, Y, Z, ws, ws_bytes, &N, &nb);
     if (rc != TPX_OK) return rc;
-    const float origin[3] = {ox, oy, oz}, spacing[3] = {sx, sy, sz};
-    return launch_mc_emit(vol, X, Y, Z, iso, origin, spacing, ws, ws_bytes, verts, reinterpret_cast<long long*>(faces), static_cast<cudaStream_t>(stream));
+    TPX_DEVICE_GUARD();
+    const McPtrs w = mc_carve(ws, N, nb);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ProfScope prof(PROF_VAE_MISC, st);
+    const int x = static_cast<int>(X), y = static_cast<int>(Y), z = static_cast<int>(Z);
+    mc_vertex_kernel<<<static_cast<unsigned>(nb), MC_THREADS, 0, st>>>(vol, x, y, z, iso, make_float3(ox, oy, oz), make_float3(sx, sy, sz), w.code, w.off_v, w.hdr,
+                                                                       w.vbase, verts);
+    TPX_LAUNCH_CHECK();
+    mc_face_kernel<<<static_cast<unsigned>(nb), MC_THREADS, 0, st>>>(x, y, z, w.code, w.off_f, w.hdr, w.vbase, reinterpret_cast<long long*>(faces));
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
 }
 
 }  // extern "C"

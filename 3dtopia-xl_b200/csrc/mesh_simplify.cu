@@ -663,15 +663,25 @@ int scan(const int* flags, int* pos, long long n, void* cub, size_t cub_bytes, c
 }
 }  // namespace
 
+}  // namespace tpx
+
+using namespace tpx;
+
+extern "C" {
+
 // ------------------------------------------------------------------------------------------------------------ component filter
-size_t cc_workspace_bytes(long long V, long long F) {
+size_t tpx_mesh_components_workspace_bytes(int64_t V, int64_t F) {
     if (V < 0 || F < 0 || V >= MS_INDEX_LIMIT || F >= MS_INDEX_LIMIT) return 0;
     return cc_layout(nullptr, V, F).total;
 }
 
-int launch_cc_count(const float* verts, long long V, const long long* faces, long long F, long long min_faces, double min_diameter, void* ws, size_t ws_bytes,
-                    long long* counts, cudaStream_t st) {
-    const int rc = mesh_check("remove_small_components", verts, V, faces, F, ws, ws_bytes, cc_workspace_bytes(V, F), V, F);
+int tpx_mesh_components_count(const float* verts, int64_t V, const int64_t* faces_dev, int64_t F, int64_t min_faces, double min_diameter, void* ws,
+                              size_t ws_bytes, int64_t* counts_dev, void* stream) {
+    TPX_DEVICE_GUARD();   // first: the argument check below sizes the CUB scratch, a CUDA query
+    const long long* faces = reinterpret_cast<const long long*>(faces_dev);
+    long long* counts = reinterpret_cast<long long*>(counts_dev);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int rc = mesh_check("remove_small_components", verts, V, faces, F, ws, ws_bytes, tpx_mesh_components_workspace_bytes(V, F), V, F);
     if (rc != TPX_OK) return rc;
     TPX_CHECK(counts != nullptr, TPX_ERR_ARG, "remove_small_components: null counts");
     const CcWs w = cc_layout(ws, V, F);
@@ -708,8 +718,11 @@ int launch_cc_count(const float* verts, long long V, const long long* faces, lon
     return TPX_OK;
 }
 
-int launch_cc_emit(const float* verts, long long V, long long F, const void* ws, size_t ws_bytes, float* verts_out, long long* faces_out, cudaStream_t st) {
-    TPX_CHECK(ws_bytes >= cc_workspace_bytes(V, F) && ws != nullptr && (V == 0 || verts != nullptr), TPX_ERR_ARG, "remove_small_components: bad emit arguments");
+int tpx_mesh_components_emit(const float* verts, int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out, int64_t* faces_out, void* stream) {
+    TPX_DEVICE_GUARD();
+    TPX_CHECK(ws_bytes >= tpx_mesh_components_workspace_bytes(V, F) && ws != nullptr && (V == 0 || verts != nullptr), TPX_ERR_ARG,
+              "remove_small_components: bad emit arguments");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     const CcWs w = cc_layout(const_cast<void*>(ws), V, F);
     ProfScope prof(PROF_VAE_MISC, st);
     if (V) {
@@ -717,21 +730,25 @@ int launch_cc_emit(const float* verts, long long V, long long F, const void* ws,
         TPX_LAUNCH_CHECK();
     }
     if (F) {
-        emit_faces_kernel<<<blocks(F), MS_THREADS, 0, st>>>(w.T, w.fkeep, w.fpos, nullptr, F, w.vpos, faces_out);
+        emit_faces_kernel<<<blocks(F), MS_THREADS, 0, st>>>(w.T, w.fkeep, w.fpos, nullptr, F, w.vpos, reinterpret_cast<long long*>(faces_out));
         TPX_LAUNCH_CHECK();
     }
     return TPX_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------------ decimation
-size_t dec_workspace_bytes(long long V, long long F) {
+size_t tpx_decimate_workspace_bytes(int64_t V, int64_t F) {
     if (V < 0 || F < 0 || V >= MS_INDEX_LIMIT || F >= MS_INDEX_LIMIT) return 0;
     return dec_layout(nullptr, V, F).total;
 }
 
-int launch_decimate(const float* verts, long long V, const long long* faces, long long F, long long target, void* ws, size_t ws_bytes, long long* counts,
-                    long long* trace, long long trace_cap, cudaStream_t st) {
-    const int rc = mesh_check("decimate", verts, V, faces, F, ws, ws_bytes, dec_workspace_bytes(V, F), V, F);
+int tpx_decimate(const float* verts, int64_t V, const int64_t* faces_dev, int64_t F, int64_t target, void* ws, size_t ws_bytes, int64_t* counts_dev,
+                 int64_t* trace, int64_t trace_cap, void* stream) {
+    TPX_DEVICE_GUARD();   // first: the argument check below sizes the CUB scratch, a CUDA query
+    const long long* faces = reinterpret_cast<const long long*>(faces_dev);
+    long long* counts = reinterpret_cast<long long*>(counts_dev);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int rc = mesh_check("decimate", verts, V, faces, F, ws, ws_bytes, tpx_decimate_workspace_bytes(V, F), V, F);
     if (rc != TPX_OK) return rc;
     TPX_CHECK(counts != nullptr && target >= 0, TPX_ERR_ARG, "decimate: null counts or negative target");
     const DecWs w = dec_layout(ws, V, F);
@@ -788,7 +805,7 @@ int launch_decimate(const float* verts, long long V, const long long* faces, lon
         TPX_LAUNCH_CHECK();
         TPX_CUDA(cudaMemcpyAsync(&h, w.hdr, sizeof(DecHdr), cudaMemcpyDeviceToHost, st));
         TPX_CUDA(cudaStreamSynchronize(st));                              // the one readback of the round
-        TPX_CHECK(h.bad == 0, TPX_ERR_ARG, "decimate: %d faces have an index outside [0, %lld) or a repeated index", h.bad, V);
+        TPX_CHECK(h.bad == 0, TPX_ERR_ARG, "decimate: %d faces have an index outside [0, %lld) or a repeated index", h.bad, (long long)V);
         TPX_CHECK(h.E < (1LL << 32), TPX_ERR_SHAPE, "decimate: %lld edges: edge ids must fit in 32 bits", h.E);
         if (h.n_acc == 0) break;
         long long k = h.n_acc;
@@ -821,7 +838,7 @@ int launch_decimate(const float* verts, long long V, const long long* faces, lon
     if (rounds == 0 && F > 0) {                                           // no round ran: the input faces still need their check
         TPX_CUDA(cudaMemcpyAsync(&h, w.hdr, sizeof(DecHdr), cudaMemcpyDeviceToHost, st));
         TPX_CUDA(cudaStreamSynchronize(st));
-        TPX_CHECK(h.bad == 0, TPX_ERR_ARG, "decimate: %d faces have an index outside [0, %lld) or a repeated index", h.bad, V);
+        TPX_CHECK(h.bad == 0, TPX_ERR_ARG, "decimate: %d faces have an index outside [0, %lld) or a repeated index", h.bad, (long long)V);
     }
     if (rounds == 0) {
         static const int zero = 0;
@@ -843,8 +860,10 @@ int launch_decimate(const float* verts, long long V, const long long* faces, lon
     return TPX_OK;
 }
 
-int launch_decimate_emit(long long V, long long F, const void* ws, size_t ws_bytes, float* verts_out, long long* faces_out, cudaStream_t st) {
-    TPX_CHECK(ws_bytes >= dec_workspace_bytes(V, F) && ws != nullptr, TPX_ERR_ARG, "decimate: bad emit arguments");
+int tpx_decimate_emit(int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out, int64_t* faces_out, void* stream) {
+    TPX_DEVICE_GUARD();
+    TPX_CHECK(ws_bytes >= tpx_decimate_workspace_bytes(V, F) && ws != nullptr, TPX_ERR_ARG, "decimate: bad emit arguments");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     const DecWs w = dec_layout(const_cast<void*>(ws), V, F);
     DecHdr h;
     TPX_CUDA(cudaMemcpyAsync(&h, w.hdr, sizeof(DecHdr), cudaMemcpyDeviceToHost, st));
@@ -855,48 +874,10 @@ int launch_decimate_emit(long long V, long long F, const void* ws, size_t ws_byt
         TPX_LAUNCH_CHECK();
     }
     if (h.F) {
-        emit_faces_kernel<<<blocks(h.F), MS_THREADS, 0, st>>>(w.T[h.buf], nullptr, nullptr, nullptr, h.F, w.vpos, faces_out);
+        emit_faces_kernel<<<blocks(h.F), MS_THREADS, 0, st>>>(w.T[h.buf], nullptr, nullptr, nullptr, h.F, w.vpos, reinterpret_cast<long long*>(faces_out));
         TPX_LAUNCH_CHECK();
     }
     return TPX_OK;
-}
-
-}  // namespace tpx
-
-using namespace tpx;
-
-extern "C" {
-
-size_t tpx_mesh_components_workspace_bytes(int64_t V, int64_t F) { return cc_workspace_bytes(V, F); }
-
-int tpx_mesh_components_count(const float* verts, int64_t V, const int64_t* faces, int64_t F, int64_t min_faces, double min_diameter, void* ws, size_t ws_bytes,
-                              int64_t* counts, void* stream) {
-    const int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_cc_count(verts, V, reinterpret_cast<const long long*>(faces), F, min_faces, min_diameter, ws, ws_bytes, reinterpret_cast<long long*>(counts),
-                           static_cast<cudaStream_t>(stream));
-}
-
-int tpx_mesh_components_emit(const float* verts, int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out, int64_t* faces_out, void* stream) {
-    const int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_cc_emit(verts, V, F, ws, ws_bytes, verts_out, reinterpret_cast<long long*>(faces_out), static_cast<cudaStream_t>(stream));
-}
-
-size_t tpx_decimate_workspace_bytes(int64_t V, int64_t F) { return dec_workspace_bytes(V, F); }
-
-int tpx_decimate(const float* verts, int64_t V, const int64_t* faces, int64_t F, int64_t target, void* ws, size_t ws_bytes, int64_t* counts, int64_t* trace,
-                 int64_t trace_cap, void* stream) {
-    const int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_decimate(verts, V, reinterpret_cast<const long long*>(faces), F, target, ws, ws_bytes, reinterpret_cast<long long*>(counts),
-                           reinterpret_cast<long long*>(trace), trace_cap, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_decimate_emit(int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out, int64_t* faces_out, void* stream) {
-    const int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_decimate_emit(V, F, ws, ws_bytes, verts_out, reinterpret_cast<long long*>(faces_out), static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -363,30 +363,11 @@ __global__ void __launch_bounds__(PS_THREADS) primsdf_bake_kernel(const float4* 
     out[4] = __fmul_rn(o[4], 255.f); out[5] = __fmul_rn(o[5], 255.f);
     mask[p] = covered;
 }
-}  // namespace
 
-int launch_primsdf_query(const float* x, const float* srt, const float* feat, long long n, int K, int S, int dim_feat, int inference, float* out,
-                         cudaStream_t st) {
-    TPX_CHECK(dim_feat == 6, TPX_ERR_SHAPE, "primsdf_query: dim_feat %d (kernel covers the released 6-channel layout)", dim_feat);
-    TPX_CHECK(S >= 2 && S <= 32 && K >= 0, TPX_ERR_SHAPE, "primsdf_query: bad primitive geometry (S %d, K %d)", S, K);
-    TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0, TPX_ERR_ARG, "primsdf_query: srt must be 16-B aligned");
-    if (n <= 0) return TPX_OK;
-    ProfScope prof(PROF_VAE_MISC, st);
-    const long long blocks = (n + PS_THREADS - 1) / PS_THREADS;
-    TPX_CHECK(blocks < (1LL << 31), TPX_ERR_SHAPE, "primsdf_query: too many points");
-    primsdf_query_kernel<6><<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(x, srt, feat, n, K, S, inference, out);
-    TPX_LAUNCH_CHECK();
-    return TPX_OK;
-}
-
-size_t primsdf_grid_bytes(long long cap_entries) {
-    return sizeof(GridHdr) + 256 + static_cast<size_t>(2 * PG_CELLS) * 4 + static_cast<size_t>(2 * PG_CELLS + 2) * 4 + static_cast<size_t>(cap_entries) * 4;
-}
-
-namespace {
 struct GridPtrs { GridHdr* hdr; int* counts; int* offsets; int* entries; long long cap; };
-GridPtrs grid_carve(void* ws, size_t bytes) {
-    uint8_t* b = static_cast<uint8_t*>(ws);
+GridPtrs grid_carve(const void* ws, size_t bytes) {
+    if (ws == nullptr) return GridPtrs{nullptr, nullptr, nullptr, nullptr, 0};
+    uint8_t* b = static_cast<uint8_t*>(const_cast<void*>(ws));
     GridPtrs g;
     g.hdr = reinterpret_cast<GridHdr*>(b);
     g.counts = reinterpret_cast<int*>(b + 256);
@@ -398,11 +379,41 @@ GridPtrs grid_carve(void* ws, size_t bytes) {
 }
 }  // namespace
 
-int launch_primsdf_grid_build(const float* srt, int K, void* ws, size_t ws_bytes, cudaStream_t st) {
+}  // namespace tpx
+
+using namespace tpx;
+
+extern "C" {
+
+int tpx_primsdf_query(const float* x, const float* srt, const float* feat, int64_t n, int K, int S, int dim_feat, int inference, float* out, void* stream) {
+    if (n == 0) return TPX_OK;
+    TPX_CHECK(n > 0 && x != nullptr && srt != nullptr && feat != nullptr && out != nullptr, TPX_ERR_ARG, "primsdf_query: null argument or negative n");
+    TPX_CHECK(dim_feat == 6, TPX_ERR_SHAPE, "primsdf_query: dim_feat %d (kernel covers the released 6-channel layout)", dim_feat);
+    TPX_CHECK(S >= 2 && S <= 32 && K >= 0, TPX_ERR_SHAPE, "primsdf_query: bad primitive geometry (S %d, K %d)", S, K);
+    TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0, TPX_ERR_ARG, "primsdf_query: srt must be 16-B aligned");
+    const long long blocks = (n + PS_THREADS - 1) / PS_THREADS;
+    TPX_CHECK(blocks < (1LL << 31), TPX_ERR_SHAPE, "primsdf_query: too many points");
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ProfScope prof(PROF_VAE_MISC, st);
+    primsdf_query_kernel<6><<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(x, srt, feat, n, K, S, inference, out);
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+size_t tpx_primsdf_grid_bytes(int64_t cap_entries) {
+    if (cap_entries <= 0) return 0;
+    return sizeof(GridHdr) + 256 + static_cast<size_t>(2 * PG_CELLS) * 4 + static_cast<size_t>(2 * PG_CELLS + 2) * 4 + static_cast<size_t>(cap_entries) * 4;
+}
+
+int tpx_primsdf_grid_build(const float* srt, int K, void* grid_ws, size_t grid_bytes, void* stream) {
+    TPX_CHECK(srt != nullptr && grid_ws != nullptr, TPX_ERR_ARG, "primsdf_grid_build: null argument");
     TPX_CHECK(K > 0 && K <= 4096, TPX_ERR_SHAPE, "primsdf_grid_build: K %d (1..4096 primitives fit the builder's shared memory)", K);
-    TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0 && (reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "primsdf_grid_build: alignment");
-    const GridPtrs g = grid_carve(ws, ws_bytes);
+    TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0 && (reinterpret_cast<uintptr_t>(grid_ws) & 255) == 0, TPX_ERR_ARG, "primsdf_grid_build: alignment");
+    const GridPtrs g = grid_carve(grid_ws, grid_bytes);
     TPX_CHECK(g.cap >= 1024, TPX_ERR_ARG, "primsdf_grid_build: workspace too small");
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     ProfScope prof(PROF_VAE_MISC, st);
     const int cap = g.cap > 0x7fffffffLL ? 0x7fffffff : static_cast<int>(g.cap);
     grid_bounds_kernel<<<1, 256, 0, st>>>(srt, K, g.hdr, cap);
@@ -423,43 +434,53 @@ int launch_primsdf_grid_build(const float* srt, int K, void* ws, size_t ws_bytes
     return TPX_OK;
 }
 
-int launch_primsdf_query_grid(const float* x, const float* srt, const float* feat, const void* ws, size_t ws_bytes, long long n, int K, int S, int dim_feat,
-                              int inference, float* out, cudaStream_t st) {
+int tpx_primsdf_query_grid(const float* x, const float* srt, const float* feat, const void* grid_ws, size_t grid_bytes, int64_t n, int K, int S, int dim_feat,
+                           int inference, float* out, void* stream) {
+    if (n == 0) return TPX_OK;
+    TPX_CHECK(n > 0 && x != nullptr && srt != nullptr && feat != nullptr && out != nullptr && grid_ws != nullptr, TPX_ERR_ARG,
+              "primsdf_query_grid: null argument or negative n");
     TPX_CHECK(dim_feat == 6, TPX_ERR_SHAPE, "primsdf_query: dim_feat %d (kernel covers the released 6-channel layout)", dim_feat);
     TPX_CHECK(S >= 2 && S <= 32 && K > 0, TPX_ERR_SHAPE, "primsdf_query: bad primitive geometry (S %d, K %d)", S, K);
-    if (n <= 0) return TPX_OK;
-    const GridPtrs g = grid_carve(const_cast<void*>(ws), ws_bytes);
-    ProfScope prof(PROF_VAE_MISC, st);
     const long long blocks = (n + PS_THREADS - 1) / PS_THREADS;
     TPX_CHECK(blocks < (1LL << 31), TPX_ERR_SHAPE, "primsdf_query: too many points");
+    TPX_DEVICE_GUARD();
+    const GridPtrs g = grid_carve(grid_ws, grid_bytes);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ProfScope prof(PROF_VAE_MISC, st);
     primsdf_query_grid_kernel<6><<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(x, srt, feat, g.hdr, g.offsets, g.entries, n, K, S, inference, out);
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }
 
-int launch_primsdf_sdf_grid(const float* coords, int R, const float* srt, const float* feat, const void* ws, size_t ws_bytes, int K, int S, int dim_feat,
-                            int inference, float* grid, cudaStream_t st) {
+int tpx_primsdf_sdf_grid(const float* coords, int R, const float* srt, const float* feat, const void* grid_ws, size_t grid_bytes, int K, int S, int dim_feat,
+                         int inference, float* grid_out, void* stream) {
+    TPX_CHECK(coords != nullptr && srt != nullptr && feat != nullptr && grid_out != nullptr, TPX_ERR_ARG, "primsdf_sdf_grid: null argument");
     TPX_CHECK(dim_feat == 6, TPX_ERR_SHAPE, "primsdf_sdf_grid: dim_feat %d (kernel covers the released 6-channel layout)", dim_feat);
-    TPX_CHECK(S >= 2 && S <= 32 && K >= 0 && (K > 0 || ws == nullptr), TPX_ERR_SHAPE, "primsdf_sdf_grid: bad primitive geometry (S %d, K %d)", S, K);
+    TPX_CHECK(S >= 2 && S <= 32 && K >= 0 && (K > 0 || grid_ws == nullptr), TPX_ERR_SHAPE, "primsdf_sdf_grid: bad primitive geometry (S %d, K %d)", S, K);
     TPX_CHECK(R >= 1 && R <= 2048, TPX_ERR_SHAPE, "primsdf_sdf_grid: resolution %d (1..2048)", R);
     TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0, TPX_ERR_ARG, "primsdf_sdf_grid: srt must be 16-B aligned");
-    GridPtrs g{nullptr, nullptr, nullptr, nullptr, 0};
-    if (ws != nullptr) g = grid_carve(const_cast<void*>(ws), ws_bytes);
+    TPX_DEVICE_GUARD();
+    const GridPtrs g = grid_carve(grid_ws, grid_bytes);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     ProfScope prof(PROF_VAE_MISC, st);
     const long long blocks = (static_cast<long long>(R) * R * R + PS_THREADS - 1) / PS_THREADS;
-    primsdf_sdf_grid_kernel<<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(coords, R, srt, feat, g.hdr, g.offsets, g.entries, K, S, inference, grid);
+    primsdf_sdf_grid_kernel<<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(coords, R, srt, feat, g.hdr, g.offsets, g.entries, K, S, inference, grid_out);
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }
 
-int launch_primsdf_bake(const float* rast, int H, int W, const float* v, long long Nv, const int* f, long long F, const float* srt, const float* feat, const void* ws,
-                        size_t ws_bytes, int K, int S, int dim_feat, float* feats, uint8_t* mask, cudaStream_t st) {
+int tpx_primsdf_bake(const float* rast, int H, int W, const float* v, int64_t Nv, const int32_t* f, int64_t F, const float* srt, const float* feat,
+                     const void* grid_ws, size_t grid_bytes, int K, int S, int dim_feat, float* feats, uint8_t* mask, void* stream) {
+    TPX_CHECK(rast != nullptr && feats != nullptr && mask != nullptr && srt != nullptr && feat != nullptr && (F == 0 || Nv == 0 || (v != nullptr && f != nullptr)),
+              TPX_ERR_ARG, "primsdf_bake: null argument");
     TPX_CHECK(dim_feat == 6, TPX_ERR_SHAPE, "primsdf_bake: dim_feat %d (kernel covers the released 6-channel layout)", dim_feat);
-    TPX_CHECK(S >= 2 && S <= 32 && K >= 0 && (K > 0 || ws == nullptr), TPX_ERR_SHAPE, "primsdf_bake: bad primitive geometry (S %d, K %d)", S, K);
-    TPX_CHECK(H >= 1 && W >= 1 && H <= 8192 && W <= 8192 && F >= 0 && Nv >= 0, TPX_ERR_SHAPE, "primsdf_bake: atlas %d x %d (1..8192 each), F %lld, Nv %lld", H, W, F, Nv);
+    TPX_CHECK(S >= 2 && S <= 32 && K >= 0 && (K > 0 || grid_ws == nullptr), TPX_ERR_SHAPE, "primsdf_bake: bad primitive geometry (S %d, K %d)", S, K);
+    TPX_CHECK(H >= 1 && W >= 1 && H <= 8192 && W <= 8192 && F >= 0 && Nv >= 0, TPX_ERR_SHAPE, "primsdf_bake: atlas %d x %d (1..8192 each), F %lld, Nv %lld", H, W,
+              (long long)F, (long long)Nv);
     TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0 && (reinterpret_cast<uintptr_t>(rast) & 15) == 0, TPX_ERR_ARG, "primsdf_bake: srt and rast must be 16-B aligned");
-    GridPtrs g{nullptr, nullptr, nullptr, nullptr, 0};
-    if (ws != nullptr) g = grid_carve(const_cast<void*>(ws), ws_bytes);
+    TPX_DEVICE_GUARD();
+    const GridPtrs g = grid_carve(grid_ws, grid_bytes);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     ProfScope prof(PROF_VAE_MISC, st);
     const long long n = static_cast<long long>(H) * W;
     primsdf_bake_kernel<<<static_cast<unsigned>((n + PS_THREADS - 1) / PS_THREADS), PS_THREADS, 0, st>>>(reinterpret_cast<const float4*>(rast), n, v, Nv, f, F, srt, feat, g.hdr,
@@ -468,4 +489,4 @@ int launch_primsdf_bake(const float* rast, int H, int W, const float* v, long lo
     return TPX_OK;
 }
 
-}  // namespace tpx
+}  // extern "C"

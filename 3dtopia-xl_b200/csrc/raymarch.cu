@@ -212,12 +212,21 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_preview_kernel(const R
 
 }  // namespace
 
-int launch_raymarch_preview(const float* tpl, const float* primpos, const float* primrot, const float* primscale, const float* campos, const float* camrot,
-                            const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius, float stepsize, float fadescale,
-                            float fadeexp, float* out, cudaStream_t st) {
+}  // namespace tpx
+
+using namespace tpx;
+
+extern "C" int tpx_raymarch_preview(const float* tpl, const float* primpos, const float* primrot, const float* primscale, const float* campos,
+                                    const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius,
+                                    float stepsize, float fadescale, float fadeexp, float* out, void* stream) {
+    TPX_CHECK(tpl != nullptr && primpos != nullptr && primrot != nullptr && primscale != nullptr && campos != nullptr && camrot != nullptr && focal != nullptr &&
+                  princpt != nullptr && out != nullptr,
+              TPX_ERR_ARG, "raymarch_preview: null argument");
     TPX_CHECK(N > 0 && K > 0 && S >= 2 && S <= 64 && H > 0 && W > 0 && N <= 65535, TPX_ERR_SHAPE, "raymarch: bad geometry (N %d K %d S %d %d x %d)", N, K, S, H, W);
     TPX_CHECK(stepsize > 0.f && volradius > 0.f, TPX_ERR_ARG, "raymarch: step size and volume radius must be positive");
     TPX_CHECK((reinterpret_cast<uintptr_t>(tpl) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, TPX_ERR_ARG, "raymarch: template / output must be 16-B aligned");
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     ProfScope prof(PROF_VAE_MISC, st);
     RayMarchArgs a{tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, out, N, K, S, H, W, volradius, stepsize, fadescale, fadeexp};
     const dim3 grid((W + RM_BX - 1) / RM_BX, (H + RM_BY - 1) / RM_BY, N), block(RM_BX, RM_BY);
@@ -225,5 +234,3 @@ int launch_raymarch_preview(const float* tpl, const float* primpos, const float*
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }
-
-}  // namespace tpx

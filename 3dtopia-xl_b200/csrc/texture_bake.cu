@@ -201,11 +201,21 @@ bool atlas_ok(int H, int W) { return H >= 1 && W >= 1 && H <= 8192 && W <= 8192;
 unsigned texel_blocks(int H, int W) { return static_cast<unsigned>((static_cast<long long>(H) * W + RB_THREADS - 1) / RB_THREADS); }
 }  // namespace
 
-int launch_uv_rasterize(const float* vt, long long Nt, const int* ft, long long F, int H, int W, float* rast, int* winner, cudaStream_t st) {
+}  // namespace tpx
+
+using namespace tpx;
+
+extern "C" {
+
+int tpx_uv_rasterize(const float* vt, int64_t Nt, const int32_t* ft, int64_t F, int H, int W, float* rast, int32_t* winner, void* stream) {
+    TPX_CHECK(rast != nullptr && winner != nullptr && (F == 0 || (vt != nullptr && ft != nullptr)), TPX_ERR_ARG, "uv_rasterize: null argument");
     TPX_CHECK(atlas_ok(H, W), TPX_ERR_SHAPE, "uv_rasterize: atlas %d x %d (1..8192 each)", H, W);
     // channel 3 of rast carries triangle id + 1 as a float, exact up to 2^24
-    TPX_CHECK(F >= 0 && F < (1LL << 24) && Nt >= 0 && Nt < (1LL << 31), TPX_ERR_SHAPE, "uv_rasterize: %lld triangles / %lld vertices (F < 2^24, Nt < 2^31)", F, Nt);
+    TPX_CHECK(F >= 0 && F < (1LL << 24) && Nt >= 0 && Nt < (1LL << 31), TPX_ERR_SHAPE, "uv_rasterize: %lld triangles / %lld vertices (F < 2^24, Nt < 2^31)",
+              (long long)F, (long long)Nt);
     TPX_CHECK((reinterpret_cast<uintptr_t>(rast) & 15) == 0, TPX_ERR_ARG, "uv_rasterize: rast must be 16-B aligned");
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     ProfScope prof(PROF_VAE_MISC, st);
     TPX_CUDA(cudaMemsetAsync(winner, 0xff, static_cast<size_t>(H) * W * sizeof(int), st));
     if (F > 0) {
@@ -218,67 +228,36 @@ int launch_uv_rasterize(const float* vt, long long Nt, const int* ft, long long 
     return TPX_OK;
 }
 
-int launch_rast_interpolate(const float* attr, long long Nv, int C, const int* tri, long long F, const float* rast, int H, int W, float* out, cudaStream_t st) {
+int tpx_rast_interpolate(const float* attr, int64_t Nv, int C, const int32_t* tri, int64_t F, const float* rast, int H, int W, float* out, void* stream) {
+    TPX_CHECK(rast != nullptr && out != nullptr && (F == 0 || Nv == 0 || (attr != nullptr && tri != nullptr)), TPX_ERR_ARG, "rast_interpolate: null argument");
     TPX_CHECK(atlas_ok(H, W), TPX_ERR_SHAPE, "rast_interpolate: atlas %d x %d (1..8192 each)", H, W);
-    TPX_CHECK(C >= 1 && C <= 4096 && F >= 0 && Nv >= 0, TPX_ERR_SHAPE, "rast_interpolate: bad sizes (C %d, F %lld, Nv %lld)", C, F, Nv);
+    TPX_CHECK(C >= 1 && C <= 4096 && F >= 0 && Nv >= 0, TPX_ERR_SHAPE, "rast_interpolate: bad sizes (C %d, F %lld, Nv %lld)", C, (long long)F, (long long)Nv);
     TPX_CHECK((reinterpret_cast<uintptr_t>(rast) & 15) == 0, TPX_ERR_ARG, "rast_interpolate: rast must be 16-B aligned");
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     ProfScope prof(PROF_VAE_MISC, st);
     rast_interpolate_kernel<<<texel_blocks(H, W), RB_THREADS, 0, st>>>(attr, Nv, C, tri, F, reinterpret_cast<const float4*>(rast), static_cast<long long>(H) * W, out);
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }
 
-size_t texture_inpaint_bytes(int H, int W) { return atlas_ok(H, W) ? ((static_cast<size_t>(H) * W * sizeof(short) + 255) & ~static_cast<size_t>(255)) : 0; }
-
-int launch_texture_inpaint(float* feats, const uint8_t* mask, int H, int W, int C, int P, void* ws, size_t ws_bytes, int* src, cudaStream_t st) {
-    TPX_CHECK(atlas_ok(H, W), TPX_ERR_SHAPE, "texture_inpaint: atlas %d x %d (1..8192 each)", H, W);
-    TPX_CHECK(C >= 1 && C <= 4096 && P >= 0 && P <= IP_MAX_PAD, TPX_ERR_SHAPE, "texture_inpaint: bad sizes (C %d, pad %d; pad 0..%d)", C, P, IP_MAX_PAD);
-    TPX_CHECK(ws_bytes >= texture_inpaint_bytes(H, W) && (reinterpret_cast<uintptr_t>(ws) & 1) == 0, TPX_ERR_ARG, "texture_inpaint: workspace too small or misaligned");
-    ProfScope prof(PROF_VAE_MISC, st);
-    short* rowd = static_cast<short*>(ws);
-    inpaint_rows_kernel<<<texel_blocks(H, W), RB_THREADS, 0, st>>>(mask, H, W, P, rowd);
-    TPX_LAUNCH_CHECK();
-    inpaint_cols_kernel<<<texel_blocks(H, W), RB_THREADS, 0, st>>>(mask, rowd, H, W, C, P, feats, src);
-    TPX_LAUNCH_CHECK();
-    return TPX_OK;
-}
-
-}  // namespace tpx
-
-using namespace tpx;
-
-extern "C" {
-
-int tpx_uv_rasterize(const float* vt, int64_t Nt, const int32_t* ft, int64_t F, int H, int W, float* rast, int32_t* winner, void* stream) {
-    TPX_CHECK(rast != nullptr && winner != nullptr && (F == 0 || (vt != nullptr && ft != nullptr)), TPX_ERR_ARG, "uv_rasterize: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_uv_rasterize(vt, Nt, ft, F, H, W, rast, winner, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_rast_interpolate(const float* attr, int64_t Nv, int C, const int32_t* tri, int64_t F, const float* rast, int H, int W, float* out, void* stream) {
-    TPX_CHECK(rast != nullptr && out != nullptr && (F == 0 || Nv == 0 || (attr != nullptr && tri != nullptr)), TPX_ERR_ARG, "rast_interpolate: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_rast_interpolate(attr, Nv, C, tri, F, rast, H, W, out, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_primsdf_bake(const float* rast, int H, int W, const float* v, int64_t Nv, const int32_t* f, int64_t F, const float* srt, const float* feat,
-                     const void* grid_ws, size_t grid_bytes, int K, int S, int dim_feat, float* feats, uint8_t* mask, void* stream) {
-    TPX_CHECK(rast != nullptr && feats != nullptr && mask != nullptr && srt != nullptr && feat != nullptr && (F == 0 || Nv == 0 || (v != nullptr && f != nullptr)),
-              TPX_ERR_ARG, "primsdf_bake: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_primsdf_bake(rast, H, W, v, Nv, f, F, srt, feat, grid_ws, grid_bytes, K, S, dim_feat, feats, mask, static_cast<cudaStream_t>(stream));
-}
-
-size_t tpx_texture_inpaint_bytes(int H, int W) { return texture_inpaint_bytes(H, W); }
+size_t tpx_texture_inpaint_bytes(int H, int W) { return atlas_ok(H, W) ? ((static_cast<size_t>(H) * W * sizeof(short) + 255) & ~static_cast<size_t>(255)) : 0; }
 
 int tpx_texture_inpaint(float* feats, const uint8_t* mask, int H, int W, int C, int pad, void* ws, size_t ws_bytes, int32_t* src, void* stream) {
     TPX_CHECK(feats != nullptr && mask != nullptr && ws != nullptr, TPX_ERR_ARG, "texture_inpaint: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_texture_inpaint(feats, mask, H, W, C, pad, ws, ws_bytes, src, static_cast<cudaStream_t>(stream));
+    TPX_CHECK(atlas_ok(H, W), TPX_ERR_SHAPE, "texture_inpaint: atlas %d x %d (1..8192 each)", H, W);
+    TPX_CHECK(C >= 1 && C <= 4096 && pad >= 0 && pad <= IP_MAX_PAD, TPX_ERR_SHAPE, "texture_inpaint: bad sizes (C %d, pad %d; pad 0..%d)", C, pad, IP_MAX_PAD);
+    TPX_CHECK(ws_bytes >= tpx_texture_inpaint_bytes(H, W) && (reinterpret_cast<uintptr_t>(ws) & 1) == 0, TPX_ERR_ARG,
+              "texture_inpaint: workspace too small or misaligned");
+    TPX_DEVICE_GUARD();
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ProfScope prof(PROF_VAE_MISC, st);
+    short* rowd = static_cast<short*>(ws);
+    inpaint_rows_kernel<<<texel_blocks(H, W), RB_THREADS, 0, st>>>(mask, H, W, pad, rowd);
+    TPX_LAUNCH_CHECK();
+    inpaint_cols_kernel<<<texel_blocks(H, W), RB_THREADS, 0, st>>>(mask, rowd, H, W, C, pad, feats, src);
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
 }
 
 }  // extern "C"

@@ -27,6 +27,13 @@ int cuda_fail(cudaError_t e, const char* what);
     do {                                                                 \
         if (!(cond)) { ::tpx::set_error(__VA_ARGS__); return (code); }   \
     } while (0)
+// Device guard of the stateless entry points: after the argument checks, before the first CUDA call, so that a device
+// other than sm_90 fails here with TPX_ERR_CUDA and a message naming the check rather than at some later launch.
+#define TPX_DEVICE_GUARD()                              \
+    do {                                                \
+        const int _rc = tpx_device_check();             \
+        if (_rc != TPX_OK) return _rc;                  \
+    } while (0)
 void note_launch();
 #define TPX_LAUNCH_CHECK()              \
     do {                                \
@@ -43,6 +50,9 @@ struct ProfScope {
     int idx;
     cudaStream_t st;
 };
+
+// SM count of the current device (cached on first use): the grid of the persistent kernels.
+int gemm_num_sms();
 
 #ifdef __CUDACC__
 // Launch with the programmatic-stream-serialization attribute (PDL).  The kernel MUST call pdl_wait() before its

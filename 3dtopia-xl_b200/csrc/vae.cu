@@ -10,10 +10,6 @@
 
 #include "kernels.cuh"
 
-namespace tpx {
-int launch_pack_conv3(const void* src, int dtype, __half* dst, int Cout, int Cin, int transposed, cudaStream_t st);
-int launch_pack_convt2(const void* src, int dtype, __half* dst, int Cin, int Cout, cudaStream_t st);
-}  // namespace tpx
 using namespace tpx;
 
 struct VaeRes {
@@ -164,8 +160,7 @@ int tpx_vae_create(const tpx_vae_config* c, tpx_vae** out) {
     TPX_CHECK(c->ch_mid == 256 && c->ch_out == 32 && c->out_channels >= 1 && c->out_channels <= 16, TPX_ERR_SHAPE,
               "vae_create: up_channels (%d,%d)/out %d unsupported (kernel set covers the shipped config: (256,32)/6)", c->ch_mid, c->ch_out, c->out_channels);
     TPX_CHECK(c->attn_heads > 0 && c->ch_mid % c->attn_heads == 0 && (c->ch_mid / c->attn_heads) == 32, TPX_ERR_SHAPE, "vae_create: attention head dim must be 32");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
+    TPX_DEVICE_GUARD();
     tpx_vae* h = new tpx_vae();
     h->C0 = c->ch_mid; h->C1 = c->ch_out; h->Cout = c->out_channels; h->heads = c->attn_heads;
     carve(h, nullptr);
@@ -326,60 +321,9 @@ int tpx_vae_decode(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dt
     return TPX_OK;
 }
 
-int tpx_primsdf_query(const float* x, const float* srt, const float* feat, int64_t n, int K, int S, int dim_feat, int inference, float* out, void* stream) {
-    if (n == 0) return TPX_OK;
-    TPX_CHECK(n > 0 && x != nullptr && srt != nullptr && feat != nullptr && out != nullptr, TPX_ERR_ARG, "primsdf_query: null argument or negative n");
-    return launch_primsdf_query(x, srt, feat, n, K, S, dim_feat, inference, out, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_raymarch_preview(const float* tpl, const float* primpos, const float* primrot, const float* primscale, const float* campos, const float* camrot,
-                         const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius, float stepsize, float fadescale,
-                         float fadeexp, float* rgba_out, void* stream) {
-    TPX_CHECK(tpl != nullptr && primpos != nullptr && primrot != nullptr && primscale != nullptr && campos != nullptr && camrot != nullptr && focal != nullptr &&
-                  princpt != nullptr && rgba_out != nullptr,
-              TPX_ERR_ARG, "raymarch_preview: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_raymarch_preview(tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, N, K, S, H, W, volradius, stepsize, fadescale, fadeexp, rgba_out,
-                                   static_cast<cudaStream_t>(stream));
-}
-
-size_t tpx_primsdf_grid_bytes(int64_t cap_entries) { return cap_entries > 0 ? primsdf_grid_bytes(cap_entries) : 0; }
-
-int tpx_primsdf_grid_build(const float* srt, int K, void* grid_ws, size_t grid_bytes, void* stream) {
-    TPX_CHECK(srt != nullptr && grid_ws != nullptr, TPX_ERR_ARG, "primsdf_grid_build: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_primsdf_grid_build(srt, K, grid_ws, grid_bytes, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_primsdf_query_grid(const float* x, const float* srt, const float* feat, const void* grid_ws, size_t grid_bytes, int64_t n, int K, int S, int dim_feat,
-                           int inference, float* out, void* stream) {
-    if (n == 0) return TPX_OK;
-    TPX_CHECK(n > 0 && x != nullptr && srt != nullptr && feat != nullptr && out != nullptr && grid_ws != nullptr, TPX_ERR_ARG,
-              "primsdf_query_grid: null argument or negative n");
-    return launch_primsdf_query_grid(x, srt, feat, grid_ws, grid_bytes, n, K, S, dim_feat, inference, out, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_primsdf_sdf_grid(const float* coords, int R, const float* srt, const float* feat, const void* grid_ws, size_t grid_bytes, int K, int S, int dim_feat,
-                         int inference, float* grid_out, void* stream) {
-    TPX_CHECK(coords != nullptr && srt != nullptr && feat != nullptr && grid_out != nullptr, TPX_ERR_ARG, "primsdf_sdf_grid: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
-    return launch_primsdf_sdf_grid(coords, R, srt, feat, grid_ws, grid_bytes, K, S, dim_feat, inference, grid_out, static_cast<cudaStream_t>(stream));
-}
-
-int tpx_groupnorm_silu(const void* x, const void* gamma, const void* beta, int P, int S3, int C, int groups, float eps, int apply_silu, void* out,
-                       void* stream) {
-    TPX_CHECK(x != nullptr && gamma != nullptr && beta != nullptr && out != nullptr, TPX_ERR_ARG, "groupnorm_silu: null argument");
-    return launch_groupnorm_silu(static_cast<const __half*>(x), static_cast<const __half*>(gamma), static_cast<const __half*>(beta), P, S3, C, groups, eps,
-                                 apply_silu, static_cast<__half*>(out), static_cast<cudaStream_t>(stream));
-}
-
 int tpx_conv3d_k3(const void* x, const void* W, const void* bias, const void* resid, float alpha, void* out, int P, int S, int C, int Cout, void* stream) {
     TPX_CHECK(x != nullptr && W != nullptr && out != nullptr, TPX_ERR_ARG, "conv3d_k3: null argument");
-    int rc = tpx_device_check();
-    if (rc != TPX_OK) return rc;
+    TPX_DEVICE_GUARD();
     const bool plain = resid == nullptr && alpha == 1.0f;
     return conv3(static_cast<const __half*>(x), static_cast<const __half*>(W), static_cast<const __half*>(bias), static_cast<const __half*>(resid), alpha,
                  static_cast<__half*>(out), nullptr, 0, P, S, C, Cout, plain ? EPI_STORE : EPI_RESID_SCALE, static_cast<cudaStream_t>(stream));

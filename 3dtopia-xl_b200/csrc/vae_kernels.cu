@@ -1,8 +1,6 @@
 // VAE-decoder kernels that are not GEMM shaped: the 1->C input convolution, GroupNorm(+SiLU) on
 // channels-last fp16 volumes, and the weight repacks into the implicit-GEMM [Cout, 27*Cin] layout.
 //   reference: models/vae3d_dib.py:93-145 (ResnetBlock), :344 (conv_in), :366-367 (norm_out / conv_out), :429
-#include <cstdlib>
-
 #include "kernels.cuh"
 
 namespace tpx {
@@ -356,13 +354,12 @@ int launch_groupnorm_silu(const __half* x, const __half* gamma, const __half* be
     if (P <= 0) return TPX_OK;
     ProfScope prof(PROF_GROUPNORM, st);
     // streaming path: units of 32 KB (whole primitive) or 64 KB (64-channel slice of a larger primitive)
-    static const bool stream_on = !(getenv("TPX_GN_STREAM") != nullptr && getenv("TPX_GN_STREAM")[0] == '0');
     const int cpg = C / groups;
     int CW = 0;
     if (static_cast<long long>(S3) * C * 2 == 32768) CW = C;
     else if (C % 64 == 0 && static_cast<long long>(S3) * 128 == 65536) CW = 64;
     const bool cpg_ok = cpg == 1 || cpg == 2 || cpg == 4 || cpg == 8;
-    if (stream_on && CW > 0 && cpg_ok && (CW & (CW - 1)) == 0 && CW >= 8 && (S3 <= 256 || S3 % 256 == 0)) {
+    if (CW > 0 && cpg_ok && (CW & (CW - 1)) == 0 && CW >= 8 && (S3 <= 256 || S3 % 256 == 0)) {
         const int unit_bytes = S3 * CW * 2;
         const bool big = unit_bytes > 32768;
         const int NT = big ? 512 : 256;
@@ -449,3 +446,13 @@ int launch_pack_convt2(const void* src, int dtype, __half* dst, int Cin, int Cou
 }
 
 }  // namespace tpx
+
+using namespace tpx;
+
+extern "C" int tpx_groupnorm_silu(const void* x, const void* gamma, const void* beta, int P, int S3, int C, int groups, float eps, int apply_silu,
+                                  void* out, void* stream) {
+    TPX_CHECK(x != nullptr && gamma != nullptr && beta != nullptr && out != nullptr, TPX_ERR_ARG, "groupnorm_silu: null argument");
+    TPX_DEVICE_GUARD();
+    return launch_groupnorm_silu(static_cast<const __half*>(x), static_cast<const __half*>(gamma), static_cast<const __half*>(beta), P, S3, C, groups, eps,
+                                 apply_silu, static_cast<__half*>(out), static_cast<cudaStream_t>(stream));
+}

@@ -208,6 +208,16 @@ int tpx_primsdf_query(const float* x_dev, const float* srt_dev, const float* fea
  * tpx_primsdf_query (same arithmetic in the same order); points outside the grid and over-full lists take the exhaustive loop.
  * grid_ws: 256-B aligned device memory of tpx_primsdf_grid_bytes(cap_entries) bytes (8 M entries cover the shipped 2048 boxes). */
 size_t tpx_primsdf_grid_bytes(int64_t cap_entries);
+int tpx_primsdf_grid_build(const float* srt_dev, int K, void* grid_ws, size_t grid_bytes, void* stream);
+int tpx_primsdf_query_grid(const float* x_dev, const float* srt_dev, const float* feat_dev, const void* grid_ws, size_t grid_bytes, int64_t n, int K, int S,
+                           int dim_feat, int inference, float* out_dev, void* stream);
+/* The sdf column of the same query on the R x R x R lattice (coords[i], coords[j], coords[k]) that extract_texmesh evaluates
+ * (inference.py:106-116: linspace / meshgrid(indexing='ij') points in 8192-point chunks, reshape(R,R,R)), without materialising the
+ * points: grid_out device fp32 [R,R,R], grid_out[i,j,k] = sdf at (x, y, z) = (coords[i], coords[j], coords[k]); coords device fp32 [R]
+ * (the caller's linspace).  Bit-identical to column 0 of tpx_primsdf_query_grid / tpx_primsdf_query on those points.  grid_ws as for
+ * tpx_primsdf_query_grid (built from the same srt), or NULL for the exhaustive loop. */
+int tpx_primsdf_sdf_grid(const float* coords_dev, int R, const float* srt_dev, const float* feat_dev, const void* grid_ws, size_t grid_bytes, int K, int S,
+                         int dim_feat, int inference, float* grid_out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Ray-march preview — RayMarcher.forward (dva/ray_marcher.py:142-229) = compute_raydirs (dva/mvp/extensions/utils/
@@ -222,16 +232,6 @@ size_t tpx_primsdf_grid_bytes(int64_t cap_entries);
 int tpx_raymarch_preview(const float* template_chlast, const float* primpos, const float* primrot, const float* primscale, const float* campos,
                          const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius, float stepsize,
                          float fadescale, float fadeexp, float* rgba_out, void* stream);
-int tpx_primsdf_grid_build(const float* srt_dev, int K, void* grid_ws, size_t grid_bytes, void* stream);
-int tpx_primsdf_query_grid(const float* x_dev, const float* srt_dev, const float* feat_dev, const void* grid_ws, size_t grid_bytes, int64_t n, int K, int S,
-                           int dim_feat, int inference, float* out_dev, void* stream);
-/* The sdf column of the same query on the R x R x R lattice (coords[i], coords[j], coords[k]) that extract_texmesh evaluates
- * (inference.py:106-116: linspace / meshgrid(indexing='ij') points in 8192-point chunks, reshape(R,R,R)), without materialising the
- * points: grid_out device fp32 [R,R,R], grid_out[i,j,k] = sdf at (x, y, z) = (coords[i], coords[j], coords[k]); coords device fp32 [R]
- * (the caller's linspace).  Bit-identical to column 0 of tpx_primsdf_query_grid / tpx_primsdf_query on those points.  grid_ws as for
- * tpx_primsdf_query_grid (built from the same srt), or NULL for the exhaustive loop. */
-int tpx_primsdf_sdf_grid(const float* coords_dev, int R, const float* srt_dev, const float* feat_dev, const void* grid_ws, size_t grid_bytes, int K, int S,
-                         int dim_feat, int inference, float* grid_out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Marching cubes — the `mcubes.marching_cubes(grid, 0.0)` call of extract_texmesh (inference.py:106-124), which copies the SDF grid

@@ -23,19 +23,101 @@ def lib():
     return _lib.load_library()
 
 
-def _header_functions():
+def _header_prototypes():
+    """[(name, return type, [parameter types])] of include/tpx.h, in declaration order."""
     src = open(os.path.join(ROOT, "include", "tpx.h")).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(tpx_[a-z0-9_]+)\s*\(", src)))
+    protos = []
+    for ret, name, params in re.findall(r"^\s*((?:const\s+)?\w+\s*\**)\s*\b(tpx_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", src, flags=re.M):
+        params = " ".join(params.split())
+        types = [] if params in ("", "void") else [re.sub(r"\s*\w+$", "", p.strip()) for p in params.split(",")]
+        protos.append((name, ret.strip(), types))
+    return protos
+
+
+_SCALARS = {"int": ctypes.c_int, "int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64, "size_t": ctypes.c_size_t, "float": ctypes.c_float,
+            "double": ctypes.c_double, "uint8_t": ctypes.c_uint8}
+_STRUCTS = {"tpx_dit_config": _lib.DitConfig, "tpx_vae_config": _lib.VaeConfig, "tpx_sampler_coefs": _lib.SamplerCoefs}
+
+
+def _ctype_matches(c_type: str, ct) -> bool:
+    """Does the ctypes type `ct` pass a value of the C type `c_type` correctly?"""
+    t = " ".join(c_type.replace("const", " ").replace("*", " * ").split())
+    base, stars = t.split(" ")[0], t.count("*")
+    if stars == 0:
+        return ct is None if base == "void" else ct is _SCALARS[base]
+    if stars == 1 and base == "char":
+        return ct is ctypes.c_char_p
+    if stars == 1 and base in _STRUCTS:
+        return ct is ctypes.POINTER(_STRUCTS[base])
+    if stars == 1:      # device / host data or an opaque handle: any pointer, or a typed pointer to the same scalar
+        return ct is ctypes.c_void_p or (base in _SCALARS and ct is ctypes.POINTER(_SCALARS[base]))
+    return stars == 2 and ct in (ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p))
 
 
 def test_library_exports_every_declared_symbol(lib):
-    names = _header_functions()
-    assert len(names) >= 25
+    protos = _header_prototypes()
+    names = [n for n, _, _ in protos]
+    assert len(names) >= 25 and len(set(names)) == len(names)
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/tpx.h but not exported"
-    assert sorted(_lib.SIGNATURES) == names, "ctypes table and header disagree"
+    assert list(_lib.SIGNATURES) == names, "ctypes table and header disagree (names or order)"
+    for name, ret, params in protos:
+        res, args = _lib.SIGNATURES[name]
+        assert _ctype_matches(ret, res), f"{name}: return type {ret} bound as {res}"
+        assert len(args) == len(params), f"{name}: {len(params)} parameters declared, {len(args)} bound"
+        for i, (c_type, ct) in enumerate(zip(params, args)):
+            assert _ctype_matches(c_type, ct), f"{name}: parameter {i} ({c_type}) bound as {ct}"
     assert lib.tpx_version() == 100
+
+
+def test_stateless_entries_check_device_first(lib):
+    """Every stateless entry that enqueues device work runs the device guard (tpx_device_check) after its argument checks and before
+    any other CUDA call: without a usable device, valid arguments fail there with TPX_ERR_CUDA naming cudaGetDevice."""
+    if torch.cuda.is_available():
+        pytest.skip("the dummy device addresses below must never reach a GPU")
+    P = 1 << 20                                    # non-null, 256-B aligned, never dereferenced
+    coefs = _lib.SamplerCoefs()
+    grid_bytes = lib.tpx_primsdf_grid_bytes(1024)
+    mc_bytes = lib.tpx_mc_workspace_bytes(2, 2, 2)
+    cc_bytes, dec_bytes = lib.tpx_mesh_components_workspace_bytes(3, 1), lib.tpx_decimate_workspace_bytes(3, 1)
+    calls = {
+        "tpx_sampler_step": (1, P, P, 1, None, 8, 4, ctypes.byref(coefs), P, P, None),
+        "tpx_latent_split": (P, None, None, 1.0, 2, 8, P, P, None),
+        "tpx_primvolume_pack": (P, P, 1, 2, 8, 4, 0, P, None),
+        "tpx_linear": (P, 128, P, None, P, 128, 128, 128, 128, 0, 1.0, 0, None),
+        "tpx_linear_gated": (P, 128, P, None, P, 0, 1, 128, P, 128, 128, 128, 128, 0, None),
+        "tpx_linear_heads": (P, 128, P, None, P, P, P, 128, 384, 128, 128, 2, 64, 64, 64, 1.0, 0, -1, 0, None),
+        "tpx_ln_modulate": (P, 8, 128, 1e-6, P, P, 0, 8, 1, P, None, None, 0, None),
+        "tpx_attention": (P, P, P, P, 1, 1, 8, 8, 64, 64, 0.125, None),
+        "tpx_attention_tc": (P, P, P, P, 1, 1, 8, 8, 8, 72, 0.125, None),
+        "tpx_cfg_combine": (P, 64, 2.0, P, None),
+        "tpx_groupnorm_silu": (P, P, P, 1, 64, 256, 32, 1e-5, 1, P, None),
+        "tpx_conv3d_k3": (P, P, P, None, 1.0, P, 1, 8, 32, 32, None),
+        "tpx_gelu_erf": (P, 64, None),
+        "tpx_primsdf_query": (P, P, P, 8, 2, 8, 6, 1, P, None),
+        "tpx_primsdf_grid_build": (P, 2, P, grid_bytes, None),
+        "tpx_primsdf_query_grid": (P, P, P, P, grid_bytes, 8, 2, 8, 6, 1, P, None),
+        "tpx_primsdf_sdf_grid": (P, 4, P, P, None, 0, 2, 8, 6, 1, P, None),
+        "tpx_raymarch_preview": (P, P, P, P, P, P, P, P, 1, 2, 8, 8, 8, 1.0, 0.01, 8.0, 8.0, P, None),
+        "tpx_mc_count": (P, 2, 2, 2, 0.0, P, mc_bytes, P, None),
+        "tpx_mc_emit": (P, 2, 2, 2, 0.0, 0.0, 0.0, 0.0, 1.0, 1.0, 1.0, P, mc_bytes, P, P, None),
+        "tpx_mesh_components_count": (P, 3, P, 1, 8, 0.05, P, cc_bytes, P, None),
+        "tpx_mesh_components_emit": (P, 3, 1, P, cc_bytes, P, P, None),
+        "tpx_decimate": (P, 3, P, 1, 0, P, dec_bytes, P, None, 0, None),
+        "tpx_decimate_emit": (3, 1, P, dec_bytes, P, P, None),
+        "tpx_uv_rasterize": (P, 3, P, 1, 8, 8, P, P, None),
+        "tpx_rast_interpolate": (P, 3, 2, P, 1, P, 8, 8, P, None),
+        "tpx_primsdf_bake": (P, 8, 8, P, 3, P, 1, P, P, None, 0, 2, 8, 6, P, P, None),
+        "tpx_texture_inpaint": (P, P, 8, 8, 6, 2, P, lib.tpx_texture_inpaint_bytes(8, 8), None, None),
+    }
+    failed = {}
+    for name, args in calls.items():
+        rc = getattr(lib, name)(*args)
+        msg = lib.tpx_last_error()
+        if rc != -2 or b"cudaGetDevice" not in msg:
+            failed[name] = (rc, msg)
+    assert not failed, failed
 
 
 def test_header_cites_reference_interfaces():
