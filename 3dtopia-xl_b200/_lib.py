@@ -61,6 +61,7 @@ SIGNATURES = {
     "tpx_vae_finalize": (_i, [_vp, _vp]),
     "tpx_vae_workspace_bytes": (_sz, [_vp, _i]),
     "tpx_vae_decode": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _sz, _vp]),
+    "tpx_vae_debug_stage": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "tpx_linear": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp]),
     "tpx_linear_gated": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _vp]),
     "tpx_linear_heads": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _vp]),

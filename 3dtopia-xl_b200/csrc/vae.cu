@@ -150,6 +150,114 @@ int conv3(const __half* x, const __half* W, const __half* bias, const __half* re
     p.args = a;
     return launch_gemm(p, st);
 }
+
+int check_run_args(const tpx_vae* h, const void* z, const void* dst, int P, const void* ws, size_t ws_bytes, const char* what) {
+    TPX_CHECK(h != nullptr && z != nullptr && dst != nullptr && ws != nullptr, TPX_ERR_ARG, "%s: null argument", what);
+    TPX_CHECK(h->finalized, TPX_ERR_STATE, "%s: weights not finalized (load_state_dict first)", what);
+    TPX_CHECK(P > 0, TPX_ERR_SHAPE, "%s: empty batch", what);
+    TPX_CHECK(ws_bytes >= tpx_vae_workspace_bytes(h, P), TPX_ERR_ARG, "%s: workspace too small (%zu < %zu)", what, ws_bytes, tpx_vae_workspace_bytes(h, P));
+    TPX_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "%s: workspace must be 256-B aligned", what);
+    return TPX_OK;
+}
+
+// The decode schedule.  stop < 0 runs it to the end and writes `out`; stop = TPX_VAE_STAGE_* ends after that stage and copies its
+// channels-last fp16 activation into `tap` (tpx_vae_debug_stage).  Both run the same launches up to the stop.
+int vae_run(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, int P, int stop, void* tap, void* ws, cudaStream_t st) {
+    VaeWs w = carve_vws(h, P, static_cast<uint8_t*>(ws));
+    const int C0 = h->C0, C1 = h->C1;
+    const float skip = sqrtf(0.5f);
+    const float eps = 1e-5f;
+    int rc;
+#define TPX_RC(call) do { rc = (call); if (rc != TPX_OK) return rc; } while (0)
+#define TPX_TAP(stage, act, S3, C)                                                                                                   \
+    do {                                                                                                                             \
+        if (stop == (stage)) {                                                                                                       \
+            TPX_CUDA(cudaMemcpyAsync(tap, act, static_cast<size_t>(P) * (S3) * (C) * sizeof(__half), cudaMemcpyDeviceToDevice, st)); \
+            return TPX_OK;                                                                                                           \
+        }                                                                                                                            \
+    } while (0)
+    TPX_RC(launch_vae_conv_in(z, z_dtype, h->w_pq, h->b_pq, h->Win, h->bin, P, C0, w.X, st));
+    __half *X = w.X, *X2 = w.X2;
+    TPX_TAP(TPX_VAE_STAGE_CONV_IN, X, 64, C0);
+    auto res4 = [&](const VaeRes& r) -> int {   // ResnetBlock C0->C0 at 4^3
+        int rc2;
+        if ((rc2 = launch_groupnorm_silu(X, r.n1g, r.n1b, P, 64, C0, 32, eps, 1, w.T1, st)) != TPX_OK) return rc2;
+        if ((rc2 = conv3(w.T1, r.W1, r.b1, nullptr, 1.f, w.T2, nullptr, 0, P, 4, C0, C0, EPI_STORE, st)) != TPX_OK) return rc2;
+        if ((rc2 = launch_groupnorm_silu(w.T2, r.n2g, r.n2b, P, 64, C0, 32, eps, 1, w.T1, st)) != TPX_OK) return rc2;
+        if ((rc2 = conv3(w.T1, r.W2, r.b2, X, skip, X2, nullptr, 0, P, 4, C0, C0, EPI_RESID_SCALE, st)) != TPX_OK) return rc2;
+        std::swap(X, X2);
+        return TPX_OK;
+    };
+    TPX_RC(res4(h->res[0]));
+    TPX_TAP(TPX_VAE_STAGE_MID_RES0, X, 64, C0);
+    {   // VolumeAttention: GN -> qkv -> 64-token attention per primitive -> proj, (x + res) * skip
+        TPX_RC(launch_groupnorm_silu(X, h->ang, h->anb, P, 64, C0, 32, eps, 0, w.T1, st));
+        GemmProblem p{};
+        p.A = w.T1; p.a_mode = AMODE_LINEAR; p.lda = C0; p.W = h->Wqkv; p.M = P * 64; p.N = 3 * C0; p.K = C0; p.BN = 256; p.epi = EPI_HEADS;
+        GemmArgs a{};
+        a.post_scale = 1.0f; a.out0 = w.Q; a.out1 = w.K; a.out2 = w.V; a.split_cols = C0; a.Dh = 32; a.DhP = 32; a.H = h->heads; a.Nseq = 64;
+        p.args = a;
+        TPX_RC(launch_gemm(p, st));
+        TPX_RC(launch_attention(w.Q, w.K, w.V, w.T2, P, h->heads, 64, 64, 32, 32, 1.0f / sqrtf(32.f), st));
+        GemmProblem q{};
+        q.A = w.T2; q.a_mode = AMODE_LINEAR; q.lda = C0; q.W = h->Wap; q.M = P * 64; q.N = C0; q.K = C0; q.BN = 256; q.epi = EPI_RESID_SCALE;
+        GemmArgs b{};
+        b.bias = h->bap; b.post_scale = 1.0f; b.out0 = X2; b.ldo = C0; b.resid = X; b.alpha = skip;
+        q.args = b;
+        TPX_RC(launch_gemm(q, st));
+        std::swap(X, X2);
+    }
+    TPX_TAP(TPX_VAE_STAGE_MID_ATTN, X, 64, C0);
+    TPX_RC(res4(h->res[1]));
+    TPX_TAP(TPX_VAE_STAGE_MID_RES1, X, 64, C0);
+    TPX_RC(res4(h->res[2]));
+    TPX_TAP(TPX_VAE_STAGE_UP0_RES0, X, 64, C0);
+    TPX_RC(res4(h->res[3]));
+    TPX_TAP(TPX_VAE_STAGE_UP0_RES1, X, 64, C0);
+    {   // ConvTranspose3d(k2,s2): 8 independent 1x1 GEMMs, one per output offset (a,b,c); each writes its stride-2 sub-lattice of the
+        // 8^3 volume with bulk tensor stores (full 128-B lines; the single N = 8*C0 GEMM with a per-thread scatter epilogue was store-bound)
+        for (int abc = 0; abc < 8; ++abc) {
+            GemmProblem p{};
+            p.A = X; p.a_mode = AMODE_LINEAR; p.lda = C0; p.W = h->Wup + static_cast<size_t>(abc) * C0 * C0; p.M = P * 64; p.N = C0; p.K = C0; p.BN = 256;
+            p.epi = EPI_STORE;
+            GemmArgs a{};
+            a.bias = h->bup + static_cast<size_t>(abc) * C0; a.post_scale = 1.0f; a.ldo = C0; a.convt_store = 1;
+            a.out0 = w.U + (static_cast<size_t>((abc >> 2) * 8 + ((abc >> 1) & 1)) * 8 + (abc & 1)) * C0;
+            p.args = a;
+            TPX_RC(launch_gemm(p, st));
+        }
+    }
+    TPX_TAP(TPX_VAE_STAGE_UPSAMPLE, w.U, 512, C0);
+    {   // ResnetBlock C0 -> C1 at 8^3 with 1x1 shortcut
+        const VaeRes& r = h->res[4];
+        TPX_RC(launch_groupnorm_silu(w.U, r.n1g, r.n1b, P, 512, C0, 32, eps, 1, w.G, st));
+        TPX_RC(conv3(w.G, r.W1, r.b1, nullptr, 1.f, w.sa, nullptr, 0, P, 8, C0, C1, EPI_STORE, st));
+        TPX_RC(launch_groupnorm_silu(w.sa, r.n2g, r.n2b, P, 512, C1, 32, eps, 1, w.sb, st));
+        GemmProblem p{};
+        p.A = w.U; p.a_mode = AMODE_LINEAR; p.lda = C0; p.W = r.Wsc; p.M = P * 512; p.N = C1; p.K = C0; p.BN = 32; p.epi = EPI_STORE;
+        GemmArgs a{};
+        a.bias = r.bsc; a.post_scale = 1.0f; a.out0 = w.sc; a.ldo = C1;
+        p.args = a;
+        TPX_RC(launch_gemm(p, st));
+        TPX_RC(conv3(w.sb, r.W2, r.b2, w.sc, skip, w.sd, nullptr, 0, P, 8, C1, C1, EPI_RESID_SCALE, st));
+    }
+    TPX_TAP(TPX_VAE_STAGE_UP1_RES0, w.sd, 512, C1);
+    {   // ResnetBlock C1 -> C1 at 8^3
+        const VaeRes& r = h->res[5];
+        TPX_RC(launch_groupnorm_silu(w.sd, r.n1g, r.n1b, P, 512, C1, 32, eps, 1, w.sa, st));
+        TPX_RC(conv3(w.sa, r.W1, r.b1, nullptr, 1.f, w.sb, nullptr, 0, P, 8, C1, C1, EPI_STORE, st));
+        TPX_RC(launch_groupnorm_silu(w.sb, r.n2g, r.n2b, P, 512, C1, 32, eps, 1, w.sa, st));
+        TPX_RC(conv3(w.sa, r.W2, r.b2, w.sd, skip, w.sc, nullptr, 0, P, 8, C1, C1, EPI_RESID_SCALE, st));
+    }
+    TPX_TAP(TPX_VAE_STAGE_UP1_RES1, w.sc, 512, C1);
+    TPX_RC(launch_groupnorm_silu(w.sc, h->nog, h->nob, P, 512, C1, 32, eps, 1, w.sa, st));
+    TPX_TAP(TPX_VAE_STAGE_NORM_OUT, w.sa, 512, C1);
+    TPX_RC(conv3(w.sa, h->Wout, h->bout, nullptr, 1.f, out_dtype == TPX_DTYPE_F16 ? static_cast<__half*>(out) : nullptr,
+                 out_dtype == TPX_DTYPE_F32 ? static_cast<float*>(out) : nullptr, h->Cout, P, 8, C1, 16, EPI_NCDHW, st));
+#undef TPX_TAP
+#undef TPX_RC
+    return TPX_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -236,89 +344,17 @@ size_t tpx_vae_workspace_bytes(const tpx_vae* h, int P) {
 }
 
 int tpx_vae_decode(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, int P, void* ws, size_t ws_bytes, void* stream) {
-    TPX_CHECK(h != nullptr && z != nullptr && out != nullptr && ws != nullptr, TPX_ERR_ARG, "vae_decode: null argument");
-    TPX_CHECK(h->finalized, TPX_ERR_STATE, "vae_decode: weights not finalized (load_state_dict first)");
-    TPX_CHECK(P > 0, TPX_ERR_SHAPE, "vae_decode: empty batch");
-    TPX_CHECK(ws_bytes >= tpx_vae_workspace_bytes(h, P), TPX_ERR_ARG, "vae_decode: workspace too small (%zu < %zu)", ws_bytes, tpx_vae_workspace_bytes(h, P));
-    TPX_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "vae_decode: workspace must be 256-B aligned");
+    const int rc = check_run_args(h, z, out, P, ws, ws_bytes, "vae_decode");
+    if (rc != TPX_OK) return rc;
     TPX_CHECK(out_dtype == TPX_DTYPE_F32 || out_dtype == TPX_DTYPE_F16, TPX_ERR_ARG, "vae_decode: bad output dtype %d", out_dtype);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    VaeWs w = carve_vws(h, P, static_cast<uint8_t*>(ws));
-    const int C0 = h->C0, C1 = h->C1;
-    const float skip = sqrtf(0.5f);
-    const float eps = 1e-5f;
-    int rc;
-#define TPX_RC(call) do { rc = (call); if (rc != TPX_OK) return rc; } while (0)
-    TPX_RC(launch_vae_conv_in(z, z_dtype, h->w_pq, h->b_pq, h->Win, h->bin, P, C0, w.X, st));
-    __half *X = w.X, *X2 = w.X2;
-    auto res4 = [&](const VaeRes& r) -> int {   // ResnetBlock C0->C0 at 4^3
-        int rc2;
-        if ((rc2 = launch_groupnorm_silu(X, r.n1g, r.n1b, P, 64, C0, 32, eps, 1, w.T1, st)) != TPX_OK) return rc2;
-        if ((rc2 = conv3(w.T1, r.W1, r.b1, nullptr, 1.f, w.T2, nullptr, 0, P, 4, C0, C0, EPI_STORE, st)) != TPX_OK) return rc2;
-        if ((rc2 = launch_groupnorm_silu(w.T2, r.n2g, r.n2b, P, 64, C0, 32, eps, 1, w.T1, st)) != TPX_OK) return rc2;
-        if ((rc2 = conv3(w.T1, r.W2, r.b2, X, skip, X2, nullptr, 0, P, 4, C0, C0, EPI_RESID_SCALE, st)) != TPX_OK) return rc2;
-        std::swap(X, X2);
-        return TPX_OK;
-    };
-    TPX_RC(res4(h->res[0]));
-    {   // VolumeAttention: GN -> qkv -> 64-token attention per primitive -> proj, (x + res) * skip
-        TPX_RC(launch_groupnorm_silu(X, h->ang, h->anb, P, 64, C0, 32, eps, 0, w.T1, st));
-        GemmProblem p{};
-        p.A = w.T1; p.a_mode = AMODE_LINEAR; p.lda = C0; p.W = h->Wqkv; p.M = P * 64; p.N = 3 * C0; p.K = C0; p.BN = 256; p.epi = EPI_HEADS;
-        GemmArgs a{};
-        a.post_scale = 1.0f; a.out0 = w.Q; a.out1 = w.K; a.out2 = w.V; a.split_cols = C0; a.Dh = 32; a.DhP = 32; a.H = h->heads; a.Nseq = 64;
-        p.args = a;
-        TPX_RC(launch_gemm(p, st));
-        TPX_RC(launch_attention(w.Q, w.K, w.V, w.T2, P, h->heads, 64, 64, 32, 32, 1.0f / sqrtf(32.f), st));
-        GemmProblem q{};
-        q.A = w.T2; q.a_mode = AMODE_LINEAR; q.lda = C0; q.W = h->Wap; q.M = P * 64; q.N = C0; q.K = C0; q.BN = 256; q.epi = EPI_RESID_SCALE;
-        GemmArgs b{};
-        b.bias = h->bap; b.post_scale = 1.0f; b.out0 = X2; b.ldo = C0; b.resid = X; b.alpha = skip;
-        q.args = b;
-        TPX_RC(launch_gemm(q, st));
-        std::swap(X, X2);
-    }
-    TPX_RC(res4(h->res[1]));
-    TPX_RC(res4(h->res[2]));
-    TPX_RC(res4(h->res[3]));
-    {   // ConvTranspose3d(k2,s2): 8 independent 1x1 GEMMs, one per output offset (a,b,c); each writes its stride-2 sub-lattice of the
-        // 8^3 volume with bulk tensor stores (full 128-B lines; the single N = 8*C0 GEMM with a per-thread scatter epilogue was store-bound)
-        for (int abc = 0; abc < 8; ++abc) {
-            GemmProblem p{};
-            p.A = X; p.a_mode = AMODE_LINEAR; p.lda = C0; p.W = h->Wup + static_cast<size_t>(abc) * C0 * C0; p.M = P * 64; p.N = C0; p.K = C0; p.BN = 256;
-            p.epi = EPI_STORE;
-            GemmArgs a{};
-            a.bias = h->bup + static_cast<size_t>(abc) * C0; a.post_scale = 1.0f; a.ldo = C0; a.convt_store = 1;
-            a.out0 = w.U + (static_cast<size_t>((abc >> 2) * 8 + ((abc >> 1) & 1)) * 8 + (abc & 1)) * C0;
-            p.args = a;
-            TPX_RC(launch_gemm(p, st));
-        }
-    }
-    {   // ResnetBlock C0 -> C1 at 8^3 with 1x1 shortcut
-        const VaeRes& r = h->res[4];
-        TPX_RC(launch_groupnorm_silu(w.U, r.n1g, r.n1b, P, 512, C0, 32, eps, 1, w.G, st));
-        TPX_RC(conv3(w.G, r.W1, r.b1, nullptr, 1.f, w.sa, nullptr, 0, P, 8, C0, C1, EPI_STORE, st));
-        TPX_RC(launch_groupnorm_silu(w.sa, r.n2g, r.n2b, P, 512, C1, 32, eps, 1, w.sb, st));
-        GemmProblem p{};
-        p.A = w.U; p.a_mode = AMODE_LINEAR; p.lda = C0; p.W = r.Wsc; p.M = P * 512; p.N = C1; p.K = C0; p.BN = 32; p.epi = EPI_STORE;
-        GemmArgs a{};
-        a.bias = r.bsc; a.post_scale = 1.0f; a.out0 = w.sc; a.ldo = C1;
-        p.args = a;
-        TPX_RC(launch_gemm(p, st));
-        TPX_RC(conv3(w.sb, r.W2, r.b2, w.sc, skip, w.sd, nullptr, 0, P, 8, C1, C1, EPI_RESID_SCALE, st));
-    }
-    {   // ResnetBlock C1 -> C1 at 8^3
-        const VaeRes& r = h->res[5];
-        TPX_RC(launch_groupnorm_silu(w.sd, r.n1g, r.n1b, P, 512, C1, 32, eps, 1, w.sa, st));
-        TPX_RC(conv3(w.sa, r.W1, r.b1, nullptr, 1.f, w.sb, nullptr, 0, P, 8, C1, C1, EPI_STORE, st));
-        TPX_RC(launch_groupnorm_silu(w.sb, r.n2g, r.n2b, P, 512, C1, 32, eps, 1, w.sa, st));
-        TPX_RC(conv3(w.sa, r.W2, r.b2, w.sd, skip, w.sc, nullptr, 0, P, 8, C1, C1, EPI_RESID_SCALE, st));
-    }
-    TPX_RC(launch_groupnorm_silu(w.sc, h->nog, h->nob, P, 512, C1, 32, eps, 1, w.sa, st));
-    TPX_RC(conv3(w.sa, h->Wout, h->bout, nullptr, 1.f, out_dtype == TPX_DTYPE_F16 ? static_cast<__half*>(out) : nullptr,
-                 out_dtype == TPX_DTYPE_F32 ? static_cast<float*>(out) : nullptr, h->Cout, P, 8, C1, 16, EPI_NCDHW, st));
-#undef TPX_RC
-    return TPX_OK;
+    return vae_run(h, z, z_dtype, out, out_dtype, P, -1, nullptr, ws, static_cast<cudaStream_t>(stream));
+}
+
+int tpx_vae_debug_stage(tpx_vae* h, const void* z, int z_dtype, int P, int stage, void* tap_f16, void* ws, size_t ws_bytes, void* stream) {
+    const int rc = check_run_args(h, z, tap_f16, P, ws, ws_bytes, "vae_debug_stage");
+    if (rc != TPX_OK) return rc;
+    TPX_CHECK(stage >= TPX_VAE_STAGE_CONV_IN && stage <= TPX_VAE_STAGE_NORM_OUT, TPX_ERR_ARG, "vae_debug_stage: bad stage %d", stage);
+    return vae_run(h, z, z_dtype, nullptr, TPX_DTYPE_F16, P, stage, tap_f16, ws, static_cast<cudaStream_t>(stream));
 }
 
 int tpx_conv3d_k3(const void* x, const void* W, const void* bias, const void* resid, float alpha, void* out, int P, int S, int C, int Cout, void* stream) {

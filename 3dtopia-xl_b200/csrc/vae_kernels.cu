@@ -53,6 +53,11 @@ int launch_vae_conv_in(const void* z, int z_dtype, const __half* w_pq, const __h
 // GroupNorm(groups, eps, affine) [+ SiLU] on channels-last fp16 [P, S3, C]; statistics per (primitive, group)
 // in fp32.  One CTA per primitive; each thread streams 16-byte channel octets (coalesced), per-channel
 // partial sums meet in shared memory, then a second streaming pass normalises (the re-read hits L2).
+// Every kernel below accumulates shifted sums S1 = sum(x - p), S2 = sum((x - p)^2) about a pivot p, the group's
+// first channel at voxel 0: mean = p + S1/n, var = S2/n - (S1/n)^2, and the output is (x - p) * scale + shift.  p lies
+// within a few standard deviations of the mean, so a group whose mean is large against its spread keeps its variance
+// (the unshifted E[x^2] - mean^2 loses it to cancellation in fp32 once mean/std reaches a few hundred), and a
+// constant group normalises to exactly beta.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int GN_MAXC = 256;
 // x * sigmoid(x) with MUFU.EX2 + MUFU.RCP (relative error ~2e-7, far below the fp16 rounding of the result)
@@ -74,12 +79,18 @@ __global__ void __launch_bounds__(256, RES > 0 ? 3 : 1) groupnorm_silu_kernel(co
     const int p = blockIdx.x;
     const int oct = C >> 3;                    // 16-byte octets per voxel
     const int total = S3 * oct;
-    const uint4* xp = reinterpret_cast<const uint4*>(x + static_cast<size_t>(p) * S3 * C);
+    const int cpg = C / groups;
+    const __half* xb = x + static_cast<size_t>(p) * S3 * C;
+    const uint4* xp = reinterpret_cast<const uint4*>(xb);
     // blockDim (256) is a multiple of oct (<= 32), so a thread always sees the same octet
     const int my_oct = threadIdx.x % oct;
-    float ls[8], lq[8];
+    float ls[8], lq[8], pv[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) { ls[i] = 0.f; lq[i] = 0.f; }
+    for (int i = 0; i < 8; ++i) {
+        ls[i] = 0.f;
+        lq[i] = 0.f;
+        pv[i] = __half2float(xb[((my_oct * 8 + i) / cpg) * cpg]);   // pivot of the channel's group (groups may straddle octets here)
+    }
     Pack8 keep[RES > 0 ? RES : 1];
     if constexpr (RES > 0) {
 #pragma unroll
@@ -88,7 +99,7 @@ __global__ void __launch_bounds__(256, RES > 0 ? 3 : 1) groupnorm_silu_kernel(co
         for (int j = 0; j < RES; ++j) {
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                const float f = __half2float(keep[j].h[k]);
+                const float f = __half2float(keep[j].h[k]) - pv[k];
                 ls[k] += f;
                 lq[k] = fmaf(f, f, lq[k]);
             }
@@ -100,7 +111,7 @@ __global__ void __launch_bounds__(256, RES > 0 ? 3 : 1) groupnorm_silu_kernel(co
             v.u = xp[i];
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                const float f = __half2float(v.h[k]);
+                const float f = __half2float(v.h[k]) - pv[k];
                 ls[k] += f;
                 lq[k] = fmaf(f, f, lq[k]);
             }
@@ -125,18 +136,17 @@ __global__ void __launch_bounds__(256, RES > 0 ? 3 : 1) groupnorm_silu_kernel(co
         s_sq[c] = b;
     }
     __syncthreads();
-    const int cpg = C / groups;
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
         const int g0 = (c / cpg) * cpg;
         float gs = 0.f, gq = 0.f;
         for (int k = 0; k < cpg; ++k) { gs += s_sum[g0 + k]; gq += s_sq[g0 + k]; }
         const float n = static_cast<float>(S3 * cpg);
-        const float mean = gs / n;
-        const float var = fmaxf(gq / n - mean * mean, 0.f);
+        const float d = gs / n;                // mean - pivot
+        const float var = fmaxf(gq / n - d * d, 0.f);
         const float rstd = rsqrtf(var + eps);
         const float sc = rstd * __half2float(gamma[c]);
         s_scale[c] = sc;
-        s_shift[c] = __half2float(beta[c]) - mean * sc;
+        s_shift[c] = __half2float(beta[c]) - d * sc;   // applied to x - pivot
     }
     __syncthreads();
     float sc[8], sh[8];
@@ -149,7 +159,7 @@ __global__ void __launch_bounds__(256, RES > 0 ? 3 : 1) groupnorm_silu_kernel(co
             Pack8 o;
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                float f = fmaf(__half2float(keep[j].h[k]), sc[k], sh[k]);
+                float f = fmaf(__half2float(keep[j].h[k]) - pv[k], sc[k], sh[k]);
                 if (apply_silu) f = silu_fast(f);
                 o.h[k] = __float2half_rn(f);
             }
@@ -162,7 +172,7 @@ __global__ void __launch_bounds__(256, RES > 0 ? 3 : 1) groupnorm_silu_kernel(co
             v.u = xp[i];
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                float f = fmaf(__half2float(v.h[k]), sc[k], sh[k]);
+                float f = fmaf(__half2float(v.h[k]) - pv[k], sc[k], sh[k]);
                 if (apply_silu) f = silu_fast(f);
                 o.h[k] = __float2half_rn(f);
             }
@@ -226,16 +236,21 @@ groupnorm_stream_kernel(const __grid_constant__ CUtensorMap tmIn, __half* __rest
         const int pp = u / slices, sl = u - pp * slices;
         mbar_wait(&full[st], (i / NS) & 1);
         uint4* up = reinterpret_cast<uint4*>(gsm + static_cast<size_t>(st) * unit_bytes);
-        float ls[8], lq[8];
+        const __half* uh = reinterpret_cast<const __half*>(up);   // row 0 of the staged slice holds every group's pivot
+        float ls[8], lq[8], pv[8];
 #pragma unroll
-        for (int k = 0; k < 8; ++k) { ls[k] = 0.f; lq[k] = 0.f; }
+        for (int k = 0; k < 8; ++k) {
+            ls[k] = 0.f;
+            lq[k] = 0.f;
+            pv[k] = __half2float(uh[my_oct * 8 + (k & ~(cpg - 1))]);
+        }
 #pragma unroll 4
         for (int j = threadIdx.x; j < total; j += NT) {
             Pack8 v;
             v.u = up[j];
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                const float f = __half2float(v.h[k]);
+                const float f = __half2float(v.h[k]) - pv[k];
                 ls[k] += f;
                 lq[k] = fmaf(f, f, lq[k]);
             }
@@ -306,10 +321,10 @@ groupnorm_stream_kernel(const __grid_constant__ CUtensorMap tmIn, __half* __rest
             float scv[8], shv[8];
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
-                const float mean = cs[q] * inv_n;
-                const float rstd = rsqrtf(fmaxf(cq[q] * inv_n - mean * mean, 0.f) + eps);
+                const float d = cs[q] * inv_n;         // mean - pivot
+                const float rstd = rsqrtf(fmaxf(cq[q] * inv_n - d * d, 0.f) + eps);
                 scv[q] = rstd * s_gamma[c0 + q];
-                shv[q] = s_beta[c0 + q] - mean * scv[q];
+                shv[q] = s_beta[c0 + q] - d * scv[q];  // applied to x - pivot
             }
             float4* dst = reinterpret_cast<float4*>(s_ss + threadIdx.x * 16);
             dst[0] = make_float4(scv[0], scv[1], scv[2], scv[3]);
@@ -335,7 +350,7 @@ groupnorm_stream_kernel(const __grid_constant__ CUtensorMap tmIn, __half* __rest
             v.u = up[j];
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                float f = fmaf(__half2float(v.h[k]), sc[k], sh[k]);
+                float f = fmaf(__half2float(v.h[k]) - pv[k], sc[k], sh[k]);
                 if (apply_silu) f = silu_fast(f);
                 o.h[k] = __float2half_rn(f);
             }

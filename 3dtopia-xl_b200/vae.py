@@ -118,35 +118,63 @@ class VAE(nn.Module):
     def __del__(self):
         self._destroy_handle()
 
-    def decode(self, x: torch.Tensor) -> torch.Tensor:
-        """VAE.decode (vae3d_dib.py:437-440)."""
+    def _latents(self, x: torch.Tensor, what: str) -> torch.Tensor:
         if self._handle is None:
             raise _lib.TpxError("VAE is not on a CUDA device: call .to('cuda') first (this implementation has no CPU path)")
         if self._sd is None:
-            raise _lib.TpxError("VAE.decode before load_state_dict")
+            raise _lib.TpxError(f"VAE.{what} before load_state_dict")
         if x.dim() != 5 or tuple(x.shape[1:]) != (self.latent_channels, 4, 4, 4):
             raise ValueError(f"z must be [P,{self.latent_channels},4,4,4], got {tuple(x.shape)}")
-        lib = _lib.lib()
-        dev = self._handle_device
-        z = x.detach().to(dev)
+        z = x.detach().to(self._handle_device)
         if z.dtype not in (torch.float16, torch.float32):
             z = z.float()
-        z = z.contiguous()
+        return z.contiguous()
+
+    def _workspace(self, lib, P: int):
+        """(256-B aligned address, bytes) of the decode scratch for P primitives; the buffer is kept for the next call of the same size."""
+        nbytes = lib.tpx_vae_workspace_bytes(self._handle, P)
+        ws = self._ws.get(P)
+        if ws is None:
+            self._ws.clear()
+            ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=self._handle_device)
+            self._ws[P] = ws
+        return (ws.data_ptr() + 255) & ~255, nbytes
+
+    def decode(self, x: torch.Tensor) -> torch.Tensor:
+        """VAE.decode (vae3d_dib.py:437-440)."""
+        z = self._latents(x, "decode")
+        lib = _lib.lib()
+        dev = self._handle_device
         P = z.shape[0]
         out = torch.empty(P, self.out_channels, 8, 8, 8, dtype=z.dtype, device=dev)
         if P == 0:
             return out
         with torch.cuda.device(dev):
-            nbytes = lib.tpx_vae_workspace_bytes(self._handle, P)
-            ws = self._ws.get(P)
-            if ws is None:
-                self._ws.clear()
-                ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
-                self._ws[P] = ws
-            base = (ws.data_ptr() + 255) & ~255
+            base, nbytes = self._workspace(lib, P)
             _lib.check(lib.tpx_vae_decode(self._handle, z.data_ptr(), _lib.dtype_tag(z), out.data_ptr(), _lib.dtype_tag(out), P, base, nbytes,
                                           _lib.stream_ptr()), "tpx_vae_decode")
         return out
+
+    # (S^3, channels) of the activation after each stage of tpx_vae_debug_stage (include/tpx.h)
+    STAGE_SHAPES = ((64, 256),) * 6 + ((512, 256),) + ((512, 32),) * 3
+
+    def debug_stage(self, x: torch.Tensor, stage: int) -> torch.Tensor:
+        """Channels-last fp16 activation [P, S^3, C] after decoder stage `stage` (0 conv_in ... 9 norm_out + SiLU), computed by
+        the same launches decode makes up to that point (parity tests)."""
+        if not 0 <= stage < len(self.STAGE_SHAPES):
+            raise ValueError(f"stage must be in [0, {len(self.STAGE_SHAPES)}), got {stage}")
+        z = self._latents(x, "debug_stage")
+        lib = _lib.lib()
+        dev = self._handle_device
+        P = z.shape[0]
+        tap = torch.empty(P, *self.STAGE_SHAPES[stage], dtype=torch.float16, device=dev)
+        if P == 0:
+            return tap
+        with torch.cuda.device(dev):
+            base, nbytes = self._workspace(lib, P)
+            _lib.check(lib.tpx_vae_debug_stage(self._handle, z.data_ptr(), _lib.dtype_tag(z), P, stage, tap.data_ptr(), base, nbytes,
+                                               _lib.stream_ptr()), "tpx_vae_debug_stage")
+        return tap
 
     def encode(self, x):
         raise NotImplementedError("VAE.encode is a training-time path (vae3d_dib.py:431-435); the H100 build covers decode only")

@@ -157,6 +157,16 @@ int tpx_vae_finalize(tpx_vae* h, void* stream);
 size_t tpx_vae_workspace_bytes(const tpx_vae* h, int P);
 /* VAE.decode (vae3d_dib.py:437-440): z device [P,1,4,4,4] (dtype z_dtype) -> out device [P,6,8,8,8] (dtype out_dtype). */
 int tpx_vae_decode(tpx_vae* h, const void* z_dev, int z_dtype, void* out_dev, int out_dtype, int P, void* ws, size_t ws_bytes, void* stream);
+/* Debug / parity: run the decode schedule through `stage` (the same launches tpx_vae_decode makes up to that point) and copy that
+ * stage's activation, channels-last fp16 [P, S^3, C], into tap_f16_dev.  Stages (Decoder.forward, vae3d_dib.py:369-387):
+ *   0 conv_in [P,64,256]; 1, 3 mid_block res 0 / 1 and 2 its attention [P,64,256]; 4, 5 up_blocks.0 res 0 / 1 [P,64,256];
+ *   6 up_blocks.0 upsample [P,512,256]; 7, 8 up_blocks.1 res 0 (with its 1x1 shortcut) / 1 [P,512,32]; 9 norm_out + SiLU [P,512,32].
+ * The decoder's output after stage 9 is tpx_vae_decode's. */
+enum {
+    TPX_VAE_STAGE_CONV_IN = 0, TPX_VAE_STAGE_MID_RES0 = 1, TPX_VAE_STAGE_MID_ATTN = 2, TPX_VAE_STAGE_MID_RES1 = 3, TPX_VAE_STAGE_UP0_RES0 = 4,
+    TPX_VAE_STAGE_UP0_RES1 = 5, TPX_VAE_STAGE_UPSAMPLE = 6, TPX_VAE_STAGE_UP1_RES0 = 7, TPX_VAE_STAGE_UP1_RES1 = 8, TPX_VAE_STAGE_NORM_OUT = 9
+};
+int tpx_vae_debug_stage(tpx_vae* h, const void* z_dev, int z_dtype, int P, int stage, void* tap_f16_dev, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Per-kernel entry points (unit parity tests; each is one launch of one hot-path kernel)

@@ -32,8 +32,9 @@ Tensor = torch.Tensor
 
 
 def r16(x: Tensor) -> Tensor:
-    """Round to fp16 and come back (value-preserving container stays fp32)."""
-    return x.to(torch.float16).to(torch.float32)
+    """Round to fp16 and come back: fp64 stays fp64 (so the policies can run in fp64 with fp16 rounding points), anything else
+    comes back as fp32."""
+    return x.to(torch.float16).to(torch.float64 if x.dtype == torch.float64 else torch.float32)
 
 
 class Policy:
