@@ -9,7 +9,7 @@ import types
 
 from . import synth  # noqa: F401
 from . import _lib  # noqa: F401
-from . import bake, diffusion, dinov2, dit, mesh, pipeline, primsdf, ray_marcher, shard, vae  # noqa: F401
+from . import bake, diffusion, dinov2, dit, mesh, pipeline, primsdf, ray_marcher, shard, unwrap, vae  # noqa: F401
 from .diffusion import SpacedDiffusion, create_diffusion  # noqa: F401
 from .dit import DiT  # noqa: F401
 from .pipeline import LatentCodec, PrimXPipeline  # noqa: F401
@@ -20,7 +20,7 @@ from .vae import VAE  # noqa: F401
 __version__ = "0.1.0"
 
 
-def install(mcubes: bool = False, nvdiffrast: bool = False) -> None:
+def install(mcubes: bool = False, nvdiffrast: bool = False, uv_unwrap: bool = False) -> None:
     """Make the reference's import paths resolve to this implementation, so ``inference.py`` / ``app.py`` run
     unchanged:  ``models.dit_crossattn`` -> dit, ``models.vae3d_dib`` -> vae, ``models.diffusion`` -> diffusion,
     ``models.primsdf`` -> primsdf, ``models.conditioner.image_dinov2`` -> dinov2, ``dva.ray_marcher`` -> ray_marcher.
@@ -28,7 +28,9 @@ def install(mcubes: bool = False, nvdiffrast: bool = False) -> None:
     ``models`` package is importable it is imported first so its other members (conditioner, primsdf) keep working.
     ``mcubes=True`` also binds ``sys.modules["mcubes"]`` to a module whose ``marching_cubes`` is the GPU one of ``mesh``, so
     extract_texmesh (inference.py:119) runs without PyMCubes; by default ``mcubes`` is left alone.  ``nvdiffrast=True`` likewise binds
-    ``sys.modules["nvdiffrast"]`` / ``["nvdiffrast.torch"]`` to the forward-only UV-space rasteriser of ``bake`` (inference.py:22,31,172-174)."""
+    ``sys.modules["nvdiffrast"]`` / ``["nvdiffrast.torch"]`` to the forward-only UV-space rasteriser of ``bake`` (inference.py:22,31,172-174).
+    ``uv_unwrap=True`` binds ``sys.modules["utils.uv_unwrap"]`` (and the attribute of an importable ``utils`` package) to the GPU
+    box-projection unwrap of ``unwrap`` (inference.py:142-143)."""
     try:
         import models as ref_models  # the reference checkout, when it is on sys.path
     except Exception:
@@ -58,3 +60,11 @@ def install(mcubes: bool = False, nvdiffrast: bool = False) -> None:
         sys.modules["mcubes"] = mesh.mcubes_module()
     if nvdiffrast:
         sys.modules["nvdiffrast"], sys.modules["nvdiffrast.torch"] = bake.nvdiffrast_modules()
+    if uv_unwrap:
+        m = unwrap.uv_unwrap_module()
+        sys.modules["utils.uv_unwrap"] = m
+        try:
+            import utils as ref_utils
+            setattr(ref_utils, "uv_unwrap", m)
+        except Exception:
+            pass

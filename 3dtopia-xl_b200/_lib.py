@@ -86,6 +86,11 @@ SIGNATURES = {
     "tpx_decimate_workspace_bytes": (_sz, [_i64, _i64]),
     "tpx_decimate": (_i, [_vp, _i64, _vp, _i64, _i64, _vp, _sz, _vp, _vp, _i64, _vp]),
     "tpx_decimate_emit": (_i, [_i64, _i64, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_uv_unwrap_workspace_bytes": (_sz, [_i64, _i64]),
+    "tpx_vertex_normals": (_i, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
+    "tpx_uv_unwrap": (_i, [_vp, _vp, _i64, _vp, _i64, C.c_double, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_uv_unwrap_emit": (_i, [_i64, _i64, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_prim_noise_filter": (_i, [_vp, _i, _vp, _vp, _vp]),
     "tpx_uv_rasterize": (_i, [_vp, _i64, _vp, _i64, _i, _i, _vp, _vp, _vp]),
     "tpx_rast_interpolate": (_i, [_vp, _i64, _i, _vp, _i64, _vp, _i, _i, _vp, _vp]),
     "tpx_primsdf_bake": (_i, [_vp, _i, _i, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _sz, _i, _i, _i, _vp, _vp, _vp]),

@@ -12,7 +12,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from . import _lib, bake, mesh
+from . import _lib, bake, mesh, unwrap
 
 
 class PrimSDF(nn.Module):
@@ -96,7 +96,7 @@ class PrimSDF(nn.Module):
         ``mesh.remove_small_components`` with those thresholds; when ``target_faces`` is set, ``mesh.decimate`` to it (see its note on
         unreachable targets).  ``extract_mesh(256, min_faces=8, min_diameter=0.05, target_faces=100000)`` is the geometry of
         extract_texmesh up to the parts of clean_mesh this package does not implement (DESIGN.md §8).  The defaults run marching cubes
-        only.  The primitive noise filter of extract_texmesh (:90-103) stays with the caller."""
+        only.  The primitive noise filter of extract_texmesh (:90-103) is ``noise_filter_mask``; ``extract_texmesh`` runs it first."""
         R = int(resolution)
         if R < 2:
             raise ValueError(f"resolution must be >= 2, got {resolution}")
@@ -146,6 +146,37 @@ class PrimSDF(nn.Module):
                                             mask.data_ptr(), _lib.stream_ptr()), "tpx_primsdf_bake")
             bake.inpaint(feats, mask, pad)
         return feats, mask.view(torch.bool)
+
+    def noise_filter_mask(self) -> torch.Tensor:
+        """The primitive noise filter of extract_texmesh (inference.py:90-103) on ``srt_param``: bool [K] on the module's device, True
+        for the primitives whose nearest neighbour is closer than the sum of the two scales (``unwrap.noise_filter``)."""
+        if not self.srt_param.is_cuda:
+            raise _lib.TpxError("the noise filter runs on CUDA only (no CPU path): move the module to the GPU")
+        return unwrap.noise_filter(self.srt_param.detach())
+
+    def extract_texmesh(self, resolution: int = 256, target_faces: int = 100000, atlas: int = 1024, island_padding: float = 0.02, min_faces: int = 8,
+                        min_diameter: float = 0.05):
+        """The fast-unwrap branch of extract_texmesh (inference.py:90-222) on the device, without touching this module's parameters:
+        the noise filter, ``extract_mesh(resolution, min_faces=, min_diameter=, target_faces=)`` of the kept primitives, vertex normals,
+        the box-projection unwrap, the per-corner re-indexing of :144-148 and ``bake_texture`` at ``atlas`` x ``atlas``.  Returns a dict
+        of device tensors in the layout :222 hands to Mesh: ``v`` fp32 [V,3] / ``f`` int64 [F,3] (the indexed mesh), ``vt`` fp32 [3F,2],
+        ``ft`` int64 [F,3] (= arange), ``albedo`` and ``metallicRoughness`` fp32 [atlas, atlas, 3] (feats / 255).  The caller's
+        ``srt_param[:, 1:4] *= 0.85`` (inference.py:373) is not applied here."""
+        keep = self.noise_filter_mask()
+        sub = PrimSDF(num_prims=0, dim_feat=self.dim_feat, prim_shape=self.prim_shape, sdf2alpha_var=self.sdf2alpha_var)
+        sub.grid_entries = self.grid_entries
+        sub.srt_param.data = self.srt_param.detach()[keep].contiguous()
+        sub.feat_param.data = self.feat_param.detach()[keep].contiguous()
+        sub.train(self.training)
+        v, f = sub.extract_mesh(resolution, min_faces=min_faces, min_diameter=min_diameter, target_faces=target_faces)
+        if f.shape[0] == 0:
+            raise ValueError("the filtered field has no surface at this resolution")
+        n = unwrap.compute_vertex_normal(v, f)
+        uv, idx = unwrap.box_projection_uv_unwrap(v, n, f, island_padding)
+        vt = uv[idx].reshape(-1, 2)
+        ft = torch.arange(3 * f.shape[0], device=f.device, dtype=torch.int64).reshape(-1, 3)
+        feats, _ = sub.bake_texture(v[f].reshape(-1, 3), ft, vt, ft, atlas)
+        return {"v": v, "f": f, "vt": vt, "ft": ft, "albedo": feats[..., :3] / 255, "metallicRoughness": feats[..., 3:] / 255}
 
     def sdf2alpha(self, sdf):
         return torch.exp(-(sdf / self.sdf2alpha_var) ** 2)

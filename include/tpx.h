@@ -295,6 +295,33 @@ int tpx_decimate(const float* verts_dev, int64_t V, const int64_t* faces_dev, in
 int tpx_decimate_emit(int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out_dev, int64_t* faces_out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Box-projection UV unwrap and the primitive noise filter — the fast-unwrap branch of extract_texmesh (inference.py:140-150:
+ * compute_vertex_normal + box_projection_uv_unwrap, utils/uv_unwrap.py:65-685) and its first block (inference.py:90-103).
+ * verts device fp32 [V,3], faces device int32 [F,3], 1 <= V < 2^31 - 1, 1 <= F < 2^31 / 3; an index outside [0, V) is never read
+ * (the face is treated as (0, 0, 0)) and makes tpx_uv_unwrap report U = -1.  Deterministic: repeated calls, on any stream, give
+ * identical bytes.  The full contract, quirks included, is in DESIGN.md §1 f-8.  Workspace: tpx_uv_unwrap_workspace_bytes(V, F) bytes
+ * of 256-B aligned device memory (0 = too large; about 300 bytes per face), shared by the three unwrap calls.
+ * ---------------------------------------------------------------------------------------------------------- */
+size_t tpx_uv_unwrap_workspace_bytes(int64_t V, int64_t F);
+/* compute_vertex_normal (uv_unwrap.py:65-85): face normals (v1 - v0) x (v2 - v0) summed per vertex in the reference's scatter_add_
+ * order (corner 0 of every face by ascending id, then corner 1, then corner 2), (0,0,1) where |n|^2 <= 1e-20, normalised; normals_dev
+ * fp32 [V,3].  Does not synchronise. */
+int tpx_vertex_normals(const float* verts_dev, int64_t V, const int32_t* faces_dev, int64_t F, void* ws, size_t ws_bytes, float* normals_dev, void* stream);
+/* box_projection_uv_unwrap(v, n, f, island_padding) (uv_unwrap.py:644-685) up to the unique rows: writes counts_dev[0] = U (device
+ * int64; -1 for malformed faces).  taps_host (NULL allowed) is a host array of 6 device pointers, each NULL or receiving a stage output:
+ * [0] slice int32 [F], [1] projected uv fp32 [F,3,2], [2] slice angle fp32 [6], [3] rotated uv fp32 [F,3,2], [4] atlas index int32 [F],
+ * [5] placed uv fp32 [F,3,2].  island_padding in [0, 0.5).  Does not synchronise: the caller reads U back once, allocates, and calls
+ * tpx_uv_unwrap_emit with the same workspace, V and F on the same stream, which writes uv_dev fp32 [U,2] (rows sorted by (u, v)) and
+ * vtex_idx_dev int64 [F,3] (torch.unique(placed.view(-1,2), dim=0, return_inverse=True), uv_unwrap.py:573-580). */
+int tpx_uv_unwrap(const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev, int64_t F, double island_padding, void* ws,
+                  size_t ws_bytes, int64_t* counts_dev, void** taps_host, void* stream);
+int tpx_uv_unwrap_emit(int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* uv_dev, int64_t* vtex_idx_dev, void* stream);
+/* The noise filter of extract_texmesh (inference.py:90-103) on srt_dev fp32 [K,4] = (scale, x, y, z): d_ij = sqrt(sum_d (p_i - p_j)^2)
+ * in fp32 plus 1 on the diagonal, nn_i = first argmin_j d_ij, keep_dev[i] = d_i,nn < s_i + s_nn (uint8 [K]); nn_dev (NULL allowed)
+ * int32 [K] receives nn.  Does not synchronise. */
+int tpx_prim_noise_filter(const float* srt_dev, int K, uint8_t* keep_dev, int32_t* nn_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Texture bake —the back half of extract_texmesh (inference.py:163-211), device-resident.  All tensors contiguous, row-major;
  * atlas H, W in 1..8192; index tensors int32.
  *
