@@ -2,13 +2,18 @@
 //   (contract of xformers.ops.memory_efficient_attention as called at models/attention.py:54,109)
 //
 // One CTA = 128 query rows of one (batch, head); K / V^T stream through a TMA ring in 128-key tiles.
-//   warp 0           TMA producer (Q once, then K and V^T tiles; mbarrier complete_tx); warps 1-3 of its warpgroup only give
-//                    their registers away (setmaxnreg)
+//   warp 0           TMA producer (Q once, then K and V^T tiles, each with its own full / empty mbarriers, so K_{j+4} may land
+//                    while V_j is still read); warps 1-3 of its warpgroup only give their registers away (setmaxnreg)
 //   warpgroups 1, 2  consumers, 64 query rows each:  S = Q K^T  (wgmma m64n128k16 x 5, both operands from shared memory, fp32 in
 //                    registers), online softmax on the accumulator fragment (a row lives in the four threads of a quad: row max
 //                    by two shuffles, row sum kept as per-thread partials until the end), P converted in registers to the fp16 A
-//                    fragments of  O += P V  (wgmma m64n80k16 x 8, A from registers, B = the V^T tile), O in registers.
-// The two consumers run independently, so one's exponentials overlap the other's tensor-core work.
+//                    fragments of  O += P V  (wgmma m64n72k16 x 8, A from registers, B = the V^T tile), O in registers.
+// Overlap of the exponentials with tensor-core work, two ways:
+//   ping-pong        the consumers take turns issuing their wgmma (named-barrier hand-off), so one's softmax runs under the other's
+//                    products;
+//   pipelining       within a consumer, S_{j+1} and PV_j are issued in one turn and S_{j+1}'s softmax runs while PV_j is in flight.
+// The arithmetic is that of a serial loop (same tiles, exponent arguments, partial sums, fp16 P, rescale order): the output does
+// not depend on the schedule.
 //
 // Layouts: q, k  [B,H,N,80] fp16 (d >= 72 zero);  vT [B,H,80,NkPad] fp16 (V transposed: keys contiguous, NkPad % 8 == 0,
 // rows d >= 72 and key columns >= Nk finite/zero);  out [B,Nq,H*72] fp16.
@@ -19,6 +24,7 @@ namespace tpx {
 namespace {
 
 constexpr int TA_DHP = 80;
+constexpr int TA_DO = 72;                               // O columns computed (the stored head dims: 72, or 64 of them)
 constexpr int TA_BQ = 128, TA_BKV = 128;
 constexpr int TA_Q_BYTES = 128 * 128 + 128 * 32;        // 64-wide SW128 part + 16-wide SW32 part
 constexpr int TA_K_BYTES = TA_Q_BYTES;
@@ -48,6 +54,55 @@ __device__ __forceinline__ float quad_max(float v) {
     return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
 
+// S = Q K^T for one 128-key tile (the 64-wide SW128 part of the head dim in four k16 steps, then the 16-wide SW32 part)
+__device__ __forceinline__ void issue_qk(float* s, uint64_t dq, uint64_t dq2, uint32_t ka) {
+    const uint64_t dk = wgmma_desc_kmajor<128>(ka), dk2 = wgmma_desc_kmajor<32>(ka + 128 * 128);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) wgmma_ss<128>(s, dq + 2 * i, dk + 2 * i, i > 0 ? 1u : 0u);
+    wgmma_ss<128>(s, dq2, dk2, 1u);
+}
+
+// O += P V for one 128-key tile: the score fragment of key block c (16 keys) is exactly the m64k16 A fragment; one m64n72k16 per
+// block covers the 72 stored columns (V^T box rows are head dims, 128 B apart)
+__device__ __forceinline__ void issue_pv(float* o, const uint32_t* pa, uint32_t va) {
+#pragma unroll
+    for (int c = 0; c < 8; ++c) wgmma_rs<TA_DO>(o, pa + 4 * c, wgmma_desc_kmajor<128>(va + (c >> 2) * TA_VBOX_BYTES) + 2 * (c & 3), 1u);
+}
+
+// Online softmax of one score tile in place: masks keys >= nvalid, updates the running row max and the per-thread partial row sums,
+// leaves the probabilities in s and returns the rescale factor of O in alpha
+__device__ __forceinline__ void softmax_tile(float* s, int nvalid, int qd, float scale_log2, float* m_run, float* l_part, float* alpha) {
+    if (nvalid < TA_BKV) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i)
+            if (8 * (i >> 2) + 2 * qd + (i & 1) >= nvalid) s[i] = -INFINITY;
+    }
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+    float msc[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
+        alpha[r] = ex2((m_run[r] - m_new) * scale_log2);       // first tile: 2^-inf = 0 (O and the sum are still zero)
+        m_run[r] = m_new;
+        msc[r] = m_new * scale_log2;
+    }
+    float sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+        s[i] = ex2(fmaf(s[i], scale_log2, -msc[(i >> 1) & 1]));
+        sum[(i >> 1) & 1] += s[i];
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) l_part[r] = l_part[r] * alpha[r] + sum[r];
+}
+// the probabilities as the fp16 A fragments of P V
+__device__ __forceinline__ void pack_p(const float* s, uint32_t* pa) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) pa[i] = pack_h2(s[2 * i], s[2 * i + 1]);
+}
+
 __global__ void __launch_bounds__(TA_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQa, const __grid_constant__ CUtensorMap tmQb, const __grid_constant__ CUtensorMap tmKa,
                     const __grid_constant__ CUtensorMap tmKb, const __grid_constant__ CUtensorMap tmV, __half* __restrict__ out, int H, int Nq, int Nk,
@@ -57,9 +112,11 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQa, const __grid_const
     // access to generic LD/ST instead of LDS/STS)
     uint8_t* smem = ta_smem_raw + ((1024u - (smem_u32(ta_smem_raw) & 1023u)) & 1023u);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TA_OFF_BAR);
-    uint64_t* q_full = bars;                         // 1
-    uint64_t* kv_full = bars + 1;                    // TA_KV_STAGES
-    uint64_t* kv_empty = bars + 1 + TA_KV_STAGES;    // TA_KV_STAGES
+    uint64_t* q_full = bars;                             // 1
+    uint64_t* k_full = bars + 1;                         // TA_KV_STAGES each
+    uint64_t* v_full = bars + 1 + TA_KV_STAGES;
+    uint64_t* k_empty = bars + 1 + 2 * TA_KV_STAGES;
+    uint64_t* v_empty = bars + 1 + 3 * TA_KV_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * TA_BQ;
@@ -73,8 +130,10 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQa, const __grid_const
     if (warp == 1 && lane == 0) {
         mbar_init(q_full, 1);
         for (int i = 0; i < TA_KV_STAGES; ++i) {
-            mbar_init(&kv_full[i], 1);
-            mbar_init(&kv_empty[i], 8);      // one lane of each of the eight consumer warps
+            mbar_init(&k_full[i], 1);
+            mbar_init(&v_full[i], 1);
+            mbar_init(&k_empty[i], 8);       // one lane of each of the eight consumer warps
+            mbar_init(&v_empty[i], 8);
         }
         fence_barrier_init();
         fence_proxy_async();
@@ -95,16 +154,22 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQa, const __grid_const
             __syncwarp();
             for (int j = 0; j < nkt; ++j) {
                 const int s = j % TA_KV_STAGES;
-                mbar_wait(&kv_empty[s], ((j / TA_KV_STAGES) & 1) ^ 1);
+                const uint32_t ph = ((j / TA_KV_STAGES) & 1) ^ 1;
+                uint8_t* ks = smem + TA_OFF_KV + s * TA_KV_STAGE;
+                uint8_t* vs = ks + TA_K_BYTES;
+                mbar_wait(&k_empty[s], ph);
                 if (elect_one()) {
-                    uint8_t* ks = smem + TA_OFF_KV + s * TA_KV_STAGE;
-                    uint8_t* vs = ks + TA_K_BYTES;
-                    mbar_arrive_expect_tx(&kv_full[s], TA_KV_STAGE);
+                    mbar_arrive_expect_tx(&k_full[s], TA_K_BYTES);
                     const int krow = bh * Nk + j * TA_BKV;
-                    tma_load_2d(ks, &tmKa, &kv_full[s], 0, krow);
-                    tma_load_2d(ks + 128 * 128, &tmKb, &kv_full[s], 64, krow);
-                    tma_load_2d(vs, &tmV, &kv_full[s], j * TA_BKV, bh * TA_DHP);
-                    tma_load_2d(vs + TA_VBOX_BYTES, &tmV, &kv_full[s], j * TA_BKV + 64, bh * TA_DHP);
+                    tma_load_2d(ks, &tmKa, &k_full[s], 0, krow);
+                    tma_load_2d(ks + 128 * 128, &tmKb, &k_full[s], 64, krow);
+                }
+                __syncwarp();
+                mbar_wait(&v_empty[s], ph);
+                if (elect_one()) {
+                    mbar_arrive_expect_tx(&v_full[s], TA_V_BYTES);
+                    tma_load_2d(vs, &tmV, &v_full[s], j * TA_BKV, bh * TA_DHP);
+                    tma_load_2d(vs + TA_VBOX_BYTES, &tmV, &v_full[s], j * TA_BKV + 64, bh * TA_DHP);
                 }
                 __syncwarp();
             }
@@ -116,72 +181,76 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQa, const __grid_const
         const uint32_t sbase = smem_u32(smem);
         const uint64_t dq = wgmma_desc_kmajor<128>(sbase + TA_OFF_Q + w * 64 * 128);
         const uint64_t dq2 = wgmma_desc_kmajor<32>(sbase + TA_OFF_Q + 128 * 128 + w * 64 * 32);
-        float o[TA_DHP / 2];
+        float o[TA_DO / 2];
 #pragma unroll
-        for (int i = 0; i < TA_DHP / 2; ++i) o[i] = 0.f;
+        for (int i = 0; i < TA_DO / 2; ++i) o[i] = 0.f;
         float m_run[2] = {-INFINITY, -INFINITY}, l_part[2] = {0.f, 0.f};   // rows lane/4 and lane/4 + 8 of this warp's 16
+        float alpha[2];
+        uint32_t pa[32];                             // P of the tile whose PV is issued next
+
+        // Turn r (0 .. nkt) issues S_r = Q K_r^T (r < nkt) and O += P_{r-1} V_{r-1} (r > 0).  Consumer 0 takes turn 0 without waiting;
+        // every other turn waits for the other consumer's pass, and a pass is made only when the other consumer has a turn left.
+        // Both consumers take all nkt + 1 turns whichever of their rows exist, so every bar.arrive meets its bar.sync.
+        const auto turn_begin = [&](int r) { if (w == 1 || r > 0) pp_turn_wait(w); };
+        const auto turn_end = [&](int r) { if (w == 0 || r < nkt) pp_turn_pass(w); };
+        const auto k_addr = [&](int j) { return sbase + TA_OFF_KV + (j % TA_KV_STAGES) * TA_KV_STAGE; };
+        const auto release = [&](uint64_t* empty, int j) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[j % TA_KV_STAGES]);
+        };
 
         mbar_wait(q_full, 0);
-        for (int j = 0; j < nkt; ++j) {
-            const int st = j % TA_KV_STAGES;
-            const int nvalid = Nk - j * TA_BKV;      // keys of this tile that exist (>= 1)
-            mbar_wait(&kv_full[st], (j / TA_KV_STAGES) & 1);
-            const uint32_t ka = sbase + TA_OFF_KV + st * TA_KV_STAGE, va = ka + TA_K_BYTES;
-            const uint64_t dk = wgmma_desc_kmajor<128>(ka), dk2 = wgmma_desc_kmajor<32>(ka + 128 * 128);
-            float s[64];
+        mbar_wait(&k_full[0], 0);
+        float s[64];
+        turn_begin(0);
+        wgmma_fence();
+        issue_qk(s, dq, dq2, k_addr(0));
+        wgmma_commit();
+        turn_end(0);
+        wgmma_wait<0>();
+        acc_fence<64>(s);
+        release(k_empty, 0);
+        softmax_tile(s, Nk, qd, scale_log2, m_run, l_part, alpha);   // O is still zero: no rescale
+        pack_p(s, pa);
+        mbar_wait(&v_full[0], 0);
+
+        // FA3 order: S_j's softmax runs while PV_{j-1} is in flight, and O is rescaled by alpha_j once PV_{j-1} has landed, so
+        // O_j = O_{j-1} alpha_j + P_j V_j exactly as a serial loop computes it
+        for (int j = 1; j < nkt; ++j) {
+            const uint32_t ph = (j / TA_KV_STAGES) & 1;
+            mbar_wait(&k_full[j % TA_KV_STAGES], ph);
+            float s[64];                             // fresh each tile: the first wgmma overwrites it (scale-d 0)
+            turn_begin(j);
             wgmma_fence();
-#pragma unroll
-            for (int i = 0; i < 4; ++i) wgmma_ss<128>(s, dq + 2 * i, dk + 2 * i, i > 0 ? 1u : 0u);
-            wgmma_ss<128>(s, dq2, dk2, 1u);
+            issue_qk(s, dq, dq2, k_addr(j));
             wgmma_commit();
-            wgmma_wait<0>();
+            issue_pv(o, pa, k_addr(j - 1) + TA_K_BYTES);
+            wgmma_commit();
+            turn_end(j);
+            wgmma_wait<1>();                         // S_j complete; PV_{j-1} may still run
             acc_fence<64>(s);
-
-            if (nvalid < TA_BKV) {
-#pragma unroll
-                for (int i = 0; i < 64; ++i)
-                    if (8 * (i >> 2) + 2 * qd + (i & 1) >= nvalid) s[i] = -INFINITY;
-            }
-            float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-            for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
-            float msc[2], alpha[2];
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
-                alpha[r] = ex2((m_run[r] - m_new) * scale_log2);       // first tile: 2^-inf = 0 (O and the sum are still zero)
-                m_run[r] = m_new;
-                msc[r] = m_new * scale_log2;
-            }
-            float sum[2] = {0.f, 0.f};
-#pragma unroll
-            for (int i = 0; i < 64; ++i) {
-                s[i] = ex2(fmaf(s[i], scale_log2, -msc[(i >> 1) & 1]));
-                sum[(i >> 1) & 1] += s[i];
-            }
-#pragma unroll
-            for (int r = 0; r < 2; ++r) l_part[r] = l_part[r] * alpha[r] + sum[r];
-#pragma unroll
-            for (int i = 0; i < TA_DHP / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
-
-            // O += P V: the score fragment of key block c (16 keys) is exactly the m64k16 A fragment (packed before the fence: a
-            // register written between two wgmma of a group would make the compiler split the group)
-            uint32_t pa[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) pa[i] = pack_h2(s[2 * i], s[2 * i + 1]);
-            wgmma_fence();
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                const uint64_t dv = wgmma_desc_kmajor<128>(va + (c >> 2) * TA_VBOX_BYTES) + 2 * (c & 3);
-                wgmma_rs<64>(o, pa + 4 * c, dv, 1u);
-                wgmma_rs<16>(o + 32, pa + 4 * c, dv + ((64 * 128) >> 4), 1u);
-            }
-            wgmma_commit();
+            release(k_empty, j);
+            softmax_tile(s, Nk - j * TA_BKV, qd, scale_log2, m_run, l_part, alpha);
+            // V_j for the next turn.  Waited between the softmax (pinned ahead of it) and the wait for PV_{j-1}: its spin loop is what
+            // keeps ptxas from hoisting that wgmma wait above the exponentials, which would serialise them behind PV_{j-1}
+            acc_fence<64>(s);
+            mbar_wait(&v_full[j % TA_KV_STAGES], ph);
             wgmma_wait<0>();
-            acc_fence<TA_DHP / 2>(o);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&kv_empty[st]);
+            acc_fence<TA_DO / 2>(o);
+            release(v_empty, j - 1);
+#pragma unroll
+            for (int i = 0; i < TA_DO / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+            pack_p(s, pa);                           // only now: P_{j-1} in pa is read by its wgmma until the wait above
         }
+
+        turn_begin(nkt);
+        wgmma_fence();
+        issue_pv(o, pa, k_addr(nkt - 1) + TA_K_BYTES);
+        wgmma_commit();
+        turn_end(nkt);
+        wgmma_wait<0>();
+        acc_fence<TA_DO / 2>(o);
+        release(v_empty, nkt - 1);
 
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
@@ -193,7 +262,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQa, const __grid_const
             if (row < Nq) {
                 __half* orow = out + (static_cast<size_t>(b) * Nq + row) * (H * Dh) + h * Dh + 2 * qd;
 #pragma unroll
-                for (int nb = 0; nb < TA_DHP / 8; ++nb)
+                for (int nb = 0; nb < TA_DO / 8; ++nb)
                     if (8 * nb < Dh) *reinterpret_cast<__half2*>(orow + 8 * nb) = __floats2half2_rn(o[4 * nb + 2 * r] * inv, o[4 * nb + 2 * r + 1] * inv);
             }
         }

@@ -438,10 +438,6 @@ __device__ __forceinline__ void epilogue_heads_tma(const GemmArgs& g, const CUte
 
 // named barrier of one consumer warpgroup (ids 1, 2; id 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar_sync(int cw) { asm volatile("bar.sync %0, 128;" ::"r"(cw + 1) : "memory"); }
-// ping-pong hand-off of the tensor cores (ids 3, 4): consumer cw waits on 3 + cw until the other one has issued its mainloop; every
-// arrive is matched by exactly one wait (an arrive is made only when the other consumer has a next tile)
-__device__ __forceinline__ void pp_turn_wait(int cw) { asm volatile("bar.sync %0, 256;" ::"r"(cw + 3) : "memory"); }
-__device__ __forceinline__ void pp_turn_pass(int cw) { asm volatile("bar.arrive %0, 256;" ::"r"((cw ^ 1) + 3) : "memory"); }
 
 template <int BN, int BK, int AMODE, int EPI>
 __global__ void __launch_bounds__(384, 1)

@@ -197,7 +197,7 @@ __device__ __forceinline__ uint64_t wgmma_desc_kmajor(uint32_t smem_addr, uint32
     return d;
 }
 
-// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T  (N in {8, 16, 32, 64, 128, 144} for _ss).  d: this thread's N/2 accumulator registers (row lane/4 (+8) of the warp's 16 rows,
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T  (N in {8, 16, 32, 64, 128, 144} for _ss, 72 for _rs).  d: this thread's N/2 accumulator registers (row lane/4 (+8) of the warp's 16 rows,
 // columns 8 j + 2 (lane%4) (+1) for d[4 j .. 4 j + 3]); scale_d = 0 overwrites D.  _ss: A and B from shared memory;
 // _rs: A from registers (the m64k16 fragment: a[0], a[2] row lane/4, a[1], a[3] row lane/4 + 8; k = 2 (lane%4) (+8)).
 template <int N>
@@ -253,21 +253,19 @@ __device__ __forceinline__ void wgmma_ss<144>(float* d, uint64_t da, uint64_t db
         : "l"(da), "l"(db), "r"(scale_d));
 }
 template <>
-__device__ __forceinline__ void wgmma_rs<16>(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
+__device__ __forceinline__ void wgmma_rs<72>(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %41, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n72k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35}, {%36, %37, %38, %39}, %40, p, 1, 1, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
 }
-template <>
-__device__ __forceinline__ void wgmma_rs<64>(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
-}
+
+// Ping-pong hand-off of the tensor cores between the two consumer warpgroups of a CTA (named barriers 3, 4; id 0 is __syncthreads):
+// consumer cw waits on 3 + cw until the other one has issued its wgmma for the current turn, then passes the turn back.  Every
+// arrive must be matched by exactly one wait, or the CTA hangs.
+__device__ __forceinline__ void pp_turn_wait(int cw) { asm volatile("bar.sync %0, 256;" ::"r"(cw + 3) : "memory"); }
+__device__ __forceinline__ void pp_turn_pass(int cw) { asm volatile("bar.arrive %0, 256;" ::"r"((cw ^ 1) + 3) : "memory"); }
 
 // A 64 x N product for any N that is a multiple of 8, as the widest instructions that tile it (144 is one instruction); the B
 // descriptor advances by n rows of b_row_bytes (n stays a multiple of 8, so every piece starts on an 8-row group).
