@@ -51,7 +51,8 @@ SIGNATURES = {
     "tpx_dit_timesteps_bytes": (_sz, [_vp, _i]),
     "tpx_dit_set_timesteps": (_i, [_vp, C.POINTER(_i64), _i, _vp, _sz, _vp]),
     "tpx_dit_forward_step": (_i, [_vp, _vp, _i64, _i, _i, _f, _vp, _vp, _sz, _vp]),
-    "tpx_dit_debug_residual": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "tpx_dit_debug_stage": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "tpx_dit_debug_tap": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "tpx_sampler_step": (_i, [_i, _vp, _vp, _i, _vp, _i64, _i, C.POINTER(SamplerCoefs), _vp, _vp, _vp]),
     "tpx_latent_split": (_i, [_vp, _vp, _vp, _f, _i64, _i, _vp, _vp, _vp]),
     "tpx_primvolume_pack": (_i, [_vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp]),

@@ -328,9 +328,12 @@ int tpx_dit_set_cond(tpx_dit* h, const float* y, int n_cross, int M, void* cond_
 
 // One forward.  The modulation vectors of the step come either from `t` (device timesteps: timestep MLP + the adaLN GEMV pass run here and
 // fill the workspace's [B, Ltot] table) or, when `t` is null, from `mod_rows` = one precomputed row shared by the whole batch (tpx_dit_forward_step).
+// stop_stage < 0 runs the whole schedule and writes `out`; stop_stage = TPX_DIT_STAGE_* returns right after that stage of block stop_block
+// (tpx_dit_debug_stage) and leaves the workspace as it stands.  Both run the same launches up to the stop.
 static int dit_forward_impl(tpx_dit* h, const float* x, const int64_t* t, const __half* mod_rows, int B, int use_cfg, float cfg_scale, void* out, void* ws,
-                            size_t ws_bytes, void* stream) {
-    TPX_CHECK(h != nullptr && x != nullptr && (t != nullptr || mod_rows != nullptr) && out != nullptr && ws != nullptr, TPX_ERR_ARG, "dit_forward: null argument");
+                            size_t ws_bytes, void* stream, int stop_block = -1, int stop_stage = -1) {
+    TPX_CHECK(h != nullptr && x != nullptr && (t != nullptr || mod_rows != nullptr) && (out != nullptr || stop_stage >= 0) && ws != nullptr, TPX_ERR_ARG,
+              "dit_forward: null argument");
     TPX_CHECK(h->finalized, TPX_ERR_STATE, "dit_forward: weights not finalized");
     TPX_CHECK(B >= 1 && B <= 8, TPX_ERR_SHAPE, "dit_forward: batch %d must be in [1,8]", B);
     TPX_CHECK(use_cfg >= 0 && use_cfg <= 2, TPX_ERR_ARG, "dit_forward: use_cfg %d", use_cfg);
@@ -378,6 +381,7 @@ static int dit_forward_impl(tpx_dit* h, const float* x, const int64_t* t, const 
     }
     // token embedding, fp32, written to both CFG halves
     TPX_RC(launch_x_embed(x, h->Wx, h->bx, B * N, h->Cin, D, w.xres, use_cfg ? static_cast<long long>(B) * N * D : 0, st));
+    if (stop_stage == TPX_DIT_STAGE_EMBED) return TPX_OK;
 
     const size_t per_layer_kv = static_cast<size_t>(h->cond_n) * h->H * M * h->DhP;
     const size_t per_layer_v = h->tc_attn ? static_cast<size_t>(h->cond_n) * h->H * h->cond_MP * h->DhP : per_layer_kv;
@@ -400,6 +404,7 @@ static int dit_forward_impl(tpx_dit* h, const float* x, const int64_t* t, const 
             a.gate = mod + 2 * D; a.gate_bstride = mod_bs; a.rows_per_batch = N; a.gate_batches = B;
             TPX_RC(gemm_linear(w.ao, D, l.Wcp, Sc * N, D, D, EPI_GATED, a, 0, st));
         }
+        if (i == stop_block && stop_stage == TPX_DIT_STAGE_CROSS) return TPX_OK;
         // ---- self-attention branch (all sequences); the collapsed cross-attention of the null half is added here ----
         TPX_RC(launch_ln_modulate(w.xres, S * N, D, 1e-6f, mod + 3 * D, mod + 4 * D, mod_bs, N, B, w.h16, Sc < S ? mod + 2 * D : nullptr,
                                   h->uconst + static_cast<size_t>(i) * D, Sc * N, st));
@@ -418,6 +423,7 @@ static int dit_forward_impl(tpx_dit* h, const float* x, const int64_t* t, const 
             a.gate = mod + 5 * D; a.gate_bstride = mod_bs; a.rows_per_batch = N; a.gate_batches = B;
             TPX_RC(gemm_linear(w.ao, D, l.Wsp, S * N, D, D, EPI_GATED, a, 0, st));
         }
+        if (i == stop_block && stop_stage == TPX_DIT_STAGE_SELF) return TPX_OK;
         // ---- MLP branch ----
         TPX_RC(launch_ln_modulate(w.xres, S * N, D, 1e-6f, mod + 6 * D, mod + 7 * D, mod_bs, N, B, w.h16, nullptr, nullptr, 0, st));
         {
@@ -431,6 +437,7 @@ static int dit_forward_impl(tpx_dit* h, const float* x, const int64_t* t, const 
             a.gate = mod + 8 * D; a.gate_bstride = mod_bs; a.rows_per_batch = N; a.gate_batches = B;
             TPX_RC(gemm_linear(w.hid, h->Dm, l.W2, S * N, D, h->Dm, EPI_GATED, a, 0, st));
         }
+        if (i == stop_block && stop_stage == TPX_DIT_STAGE_MLP) return TPX_OK;
     }
     // ---- final layer ----
     const __half* fmod = mod_base + static_cast<size_t>(h->L) * 9 * D;
@@ -496,10 +503,28 @@ int tpx_dit_forward_step(tpx_dit* h, const float* x, int64_t t, int B, int use_c
     return dit_forward_impl(h, x, nullptr, h->ts_table + row * static_cast<size_t>(h->Ltot), B, use_cfg, cfg_scale, out, ws, ws_bytes, stream);
 }
 
-int tpx_dit_debug_residual(const tpx_dit* h, const void* ws, int n_seq, float* out, void* stream) {
-    TPX_CHECK(h != nullptr && ws != nullptr && out != nullptr, TPX_ERR_ARG, "dit_debug_residual: null argument");
+int tpx_dit_debug_stage(tpx_dit* h, const float* x, const int64_t* t, int B, int use_cfg, int block, int stage, void* ws, size_t ws_bytes, void* stream) {
+    TPX_CHECK(stage >= TPX_DIT_STAGE_EMBED && stage <= TPX_DIT_STAGE_MLP, TPX_ERR_ARG, "dit_debug_stage: bad stage %d", stage);
+    TPX_CHECK(h != nullptr && t != nullptr, TPX_ERR_ARG, "dit_debug_stage: null argument");
+    TPX_CHECK(stage == TPX_DIT_STAGE_EMBED || (block >= 0 && block < h->L), TPX_ERR_ARG, "dit_debug_stage: bad block %d (depth %d)", block, h->L);
+    return dit_forward_impl(h, x, t, nullptr, B, use_cfg, 0.0f, nullptr, ws, ws_bytes, stream, stage == TPX_DIT_STAGE_EMBED ? -1 : block, stage);
+}
+
+int tpx_dit_debug_tap(const tpx_dit* h, const void* ws, int n_seq, int which, int count, void* dst, void* stream) {
+    TPX_CHECK(which >= TPX_DIT_TAP_RESIDUAL && which <= TPX_DIT_TAP_PRE_CFG, TPX_ERR_ARG, "dit_debug_tap: bad tap %d", which);
+    TPX_CHECK(n_seq >= 1 && count >= 1 && count <= n_seq, TPX_ERR_ARG, "dit_debug_tap: count %d must be in [1, n_seq = %d]", count, n_seq);
+    TPX_CHECK(h != nullptr && ws != nullptr && dst != nullptr, TPX_ERR_ARG, "dit_debug_tap: null argument");
     const DitWs w = carve_ws(h, n_seq, static_cast<uint8_t*>(const_cast<void*>(ws)));
-    TPX_CUDA(cudaMemcpyAsync(out, w.xres, static_cast<size_t>(n_seq) * h->N * h->D * 4, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+    const size_t T = static_cast<size_t>(count) * h->N;
+    const void* src = which == TPX_DIT_TAP_RESIDUAL ? static_cast<const void*>(w.xres)
+                      : which == TPX_DIT_TAP_ATTN_OUT ? static_cast<const void*>(w.ao)
+                      : which == TPX_DIT_TAP_MOD    ? static_cast<const void*>(w.mod)
+                                                    : static_cast<const void*>(w.fin);
+    const size_t bytes = which == TPX_DIT_TAP_RESIDUAL ? T * h->D * 4
+                         : which == TPX_DIT_TAP_ATTN_OUT ? T * h->D * 2
+                         : which == TPX_DIT_TAP_MOD    ? static_cast<size_t>(count) * h->Ltot * 2
+                                                       : T * h->Cout * 2;
+    TPX_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
     return TPX_OK;
 }
 

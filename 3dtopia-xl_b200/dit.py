@@ -260,7 +260,9 @@ class DiT(nn.Module):
             _lib.check(lib.tpx_dit_set_timesteps(self._handle, arr, len(ts), self._aligned(self._ts_ws), nbytes, _lib.stream_ptr()), "tpx_dit_set_timesteps")
         self._ts_key = ts
 
-    def _run(self, x, t, y, use_cfg: int, cfg_scale: float, enable_amp: bool, t_host: Optional[int] = None):
+    def _prepare(self, x, t, y, use_cfg: int):
+        """Validate one call's inputs and bring them to the device; (re)compute the conditioning store.  Returns x, t on the device,
+        the sequence count and the workspace (aligned address, bytes)."""
         self._require_handle()
         if x.dim() != 3 or x.shape[1] != self.seq_length or x.shape[2] != self.in_channels:
             raise ValueError(f"x must be [B,{self.seq_length},{self.in_channels}], got {tuple(x.shape)}")
@@ -271,25 +273,29 @@ class DiT(nn.Module):
         if use_cfg and self.cond_drop_prob <= 0:
             raise AttributeError("'DiT' object has no attribute 'null_cond_embedding'")   # as the reference would (dit_crossattn.py:208)
         lib = _lib.lib()
+        B = x.shape[0]
+        xx = x.detach().to(self._handle_device, torch.float32).contiguous()
+        tt = t.detach().to(self._handle_device, torch.int64).contiguous()
+        if tt.shape != (B,):
+            raise ValueError(f"t must have shape [{B}], got {tuple(tt.shape)}")
+        self._set_cond(y, with_null=(use_cfg == 2))
+        n_seq = 2 * B if use_cfg else B
+        return xx, tt, n_seq, self._aligned(self._workspace(n_seq)), lib.tpx_dit_workspace_bytes(self._handle, n_seq)
+
+    def _run(self, x, t, y, use_cfg: int, cfg_scale: float, enable_amp: bool, t_host: Optional[int] = None):
+        lib = _lib.lib()
         dev = self._handle_device
         with torch.cuda.device(dev):
-            B = x.shape[0]
-            xx = x.detach().to(dev, torch.float32).contiguous()
-            tt = t.detach().to(dev, torch.int64).contiguous()
-            if tt.shape != (B,):
-                raise ValueError(f"t must have shape [{B}], got {tuple(tt.shape)}")
-            self._set_cond(y, with_null=(use_cfg == 2))
-            n_seq = 2 * B if use_cfg else B
-            ws = self._workspace(n_seq)
+            xx, tt, n_seq, ws, nbytes = self._prepare(x, t, y, use_cfg)
+            B = xx.shape[0]
             out = torch.empty(B, self.seq_length, self.out_channels, dtype=torch.float16, device=dev)
-            nbytes = lib.tpx_dit_workspace_bytes(self._handle, n_seq)
             if t_host is not None and self._ts_key is not None and int(t_host) in self._ts_key:
                 # the caller states (on the host) that every sample of the batch sits at timestep t_host and its modulation row is in the
                 # table: no timestep MLP, no adaLN pass, and the device tensor t is not read
                 _lib.check(lib.tpx_dit_forward_step(self._handle, xx.data_ptr(), int(t_host), B, use_cfg, float(cfg_scale), out.data_ptr(),
-                                                    self._aligned(ws), nbytes, _lib.stream_ptr()), "tpx_dit_forward_step")
+                                                    ws, nbytes, _lib.stream_ptr()), "tpx_dit_forward_step")
             else:
-                _lib.check(lib.tpx_dit_forward(self._handle, xx.data_ptr(), tt.data_ptr(), B, use_cfg, float(cfg_scale), out.data_ptr(), self._aligned(ws),
+                _lib.check(lib.tpx_dit_forward(self._handle, xx.data_ptr(), tt.data_ptr(), B, use_cfg, float(cfg_scale), out.data_ptr(), ws,
                                                nbytes, _lib.stream_ptr()), "tpx_dit_forward")
         # the reference returns fp16 under autocast and fp32 otherwise (dit_crossattn.py:197-202)
         return out if enable_amp else out.float()
@@ -319,9 +325,47 @@ class DiT(nn.Module):
         self._precision_notice(precision_dtype, enable_amp)
         return self._run(x, t, y, 1 if self.collapse_null_branch else 2, cfg_scale, enable_amp, t_host)
 
+    # stop points of tpx_dit_debug_stage and buffers of tpx_dit_debug_tap (include/tpx.h)
+    STAGES = {"embed": 0, "cross": 1, "self": 2, "mlp": 3}
+    TAPS = {"residual": 0, "ao": 1, "mod": 2, "pre_cfg": 3}
+
+    def debug_stage(self, x, t, y, stage: str, block: int = 0, use_cfg: int = 0) -> torch.Tensor:
+        """Run the forward's schedule (use_cfg 0: forward; 1: forward_with_cfg; 2: forward_with_cfg with real cross-attention over the
+        null context) up to `stage` ("embed", or "cross" / "self" / "mlp" of block `block`) with the same launches, and return the fp32
+        residual stream [n_seq, N, D] there (parity tests).  The workspace's other buffers stay readable through debug_tap."""
+        if stage not in self.STAGES:
+            raise ValueError(f"stage must be one of {list(self.STAGES)}, got {stage!r}")
+        lib = _lib.lib()
+        with torch.cuda.device(self._handle_device):
+            xx, tt, n_seq, ws, nbytes = self._prepare(x, t, y, use_cfg)
+            _lib.check(lib.tpx_dit_debug_stage(self._handle, xx.data_ptr(), tt.data_ptr(), xx.shape[0], use_cfg, block, self.STAGES[stage], ws, nbytes,
+                                               _lib.stream_ptr()), "tpx_dit_debug_stage")
+        return self.debug_tap(n_seq, "residual")
+
+    def debug_tap(self, n_seq: int, which: str, count: Optional[int] = None) -> torch.Tensor:
+        """The leading `count` (default n_seq) sequences, or samples for "mod", of one buffer of the workspace of n_seq sequences, as the
+        last forward or debug_stage left it: "residual" fp32 [count, N, D], "ao" fp16 [count, N, D], "mod" fp16 [count, Ltot],
+        "pre_cfg" fp16 [count, N, out_channels] (tpx_dit_debug_tap)."""
+        self._require_handle()
+        count = n_seq if count is None else count
+        N, D = self.seq_length, self.hidden_size
+        shape, dtype = {"residual": ((count, N, D), torch.float32), "ao": ((count, N, D), torch.float16),
+                        "mod": ((count, self.depth * 9 * D + 2 * D), torch.float16),
+                        "pre_cfg": ((count, N, self.out_channels), torch.float16)}[which]
+        out = torch.empty(shape, dtype=dtype, device=self._handle_device)
+        with torch.cuda.device(self._handle_device):
+            _lib.check(_lib.lib().tpx_dit_debug_tap(self._handle, self._aligned(self._workspace(n_seq)), n_seq, self.TAPS[which], count, out.data_ptr(),
+                                                    _lib.stream_ptr()), "tpx_dit_debug_tap")
+        return out
+
+    def debug_timestep_table(self) -> torch.Tensor:
+        """The modulation rows [K, Ltot] fp16 that set_timesteps computed, one per timestep in its order (a view of the table)."""
+        if self._ts_key is None:
+            raise _lib.TpxError("debug_timestep_table: no timestep table (call set_timesteps)")
+        off = self._aligned(self._ts_ws) - self._ts_ws.data_ptr()       # the table opens the store (tpx_dit_set_timesteps)
+        K, Ltot = len(self._ts_key), self.depth * 9 * self.hidden_size + 2 * self.hidden_size
+        return self._ts_ws[off:off + K * Ltot * 2].view(torch.float16).view(K, Ltot)
+
     def debug_residual(self, n_seq: int) -> torch.Tensor:
         """fp32 residual stream [n_seq, N, D] left by the last forward (parity tests)."""
-        self._require_handle()
-        out = torch.empty(n_seq, self.seq_length, self.hidden_size, dtype=torch.float32, device=self._handle_device)
-        _lib.check(_lib.lib().tpx_dit_debug_residual(self._handle, self._aligned(self._workspace(n_seq)), n_seq, out.data_ptr(), _lib.stream_ptr()))
-        return out
+        return self.debug_tap(n_seq, "residual")

@@ -101,8 +101,21 @@ size_t tpx_dit_timesteps_bytes(const tpx_dit* h, int K);
 int tpx_dit_set_timesteps(tpx_dit* h, const int64_t* t_host, int K, void* ts_ws, size_t ts_bytes, void* stream);
 int tpx_dit_forward_step(tpx_dit* h, const float* x_dev, int64_t t, int B, int use_cfg, float cfg_scale, void* out_f16_dev, void* ws, size_t ws_bytes,
                          void* stream);
-/* Debug / parity: copy the fp32 residual stream [n_seq, N, hidden] left in `ws` by the last forward. */
-int tpx_dit_debug_residual(const tpx_dit* h, const void* ws, int n_seq, float* out_dev, void* stream);
+/* Debug / parity.  tpx_dit_debug_stage runs tpx_dit_forward's schedule (same arguments, same launches) up to a stop and returns,
+ * leaving the workspace as it stands: TPX_DIT_STAGE_EMBED after the token embedding (`block` is ignored), or after the gated GEMM
+ * that adds block `block`'s CROSS, SELF or MLP branch to the residual stream.  A bad stage or block is TPX_ERR_ARG.
+ * tpx_dit_debug_tap copies the leading `count` (1..n_seq) sequences or samples of one buffer of the workspace `ws` carved for n_seq
+ * sequences into dst_dev:
+ *   RESIDUAL  fp32 [count, N, hidden]   the residual stream;
+ *   ATTN_OUT  fp16 [count, N, hidden]   the attention output before proj, head j in columns [j*Dh, (j+1)*Dh), after a CROSS stop
+ *                                       (the first n_cross sequences hold it) or a SELF stop;
+ *   MOD       fp16 [count, 28*9*D + 2*D] the modulation rows of the batch's samples (a forward given device timesteps);
+ *   PRE_CFG   fp16 [count, N, out_channels] the [cond; uncond] output before guidance, after a full forward with use_cfg != 0. */
+enum { TPX_DIT_STAGE_EMBED = 0, TPX_DIT_STAGE_CROSS = 1, TPX_DIT_STAGE_SELF = 2, TPX_DIT_STAGE_MLP = 3 };
+enum { TPX_DIT_TAP_RESIDUAL = 0, TPX_DIT_TAP_ATTN_OUT = 1, TPX_DIT_TAP_MOD = 2, TPX_DIT_TAP_PRE_CFG = 3 };
+int tpx_dit_debug_stage(tpx_dit* h, const float* x_dev, const int64_t* t_dev, int B, int use_cfg, int block, int stage, void* ws, size_t ws_bytes,
+                        void* stream);
+int tpx_dit_debug_tap(const tpx_dit* h, const void* ws, int n_seq, int which, int count, void* dst_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Sampler update — models/diffusion/gaussian_diffusion.py:255-338 (p_mean_variance, LEARNED_RANGE variance),

@@ -53,17 +53,19 @@ class Policy:
         return r16(x) if self.amp else x
 
 
-def timestep_embedding(t: Tensor, dim: int = 256, max_period: float = 10000.0) -> Tensor:
-    """models/utils.py:41-59."""
+def timestep_embedding(t: Tensor, dim: int = 256, max_period: float = 10000.0, dtype: torch.dtype = torch.float32) -> Tensor:
+    """models/utils.py:41-59.  The reference evaluates the sinusoid in fp32; dtype=torch.float64 gives the exact one."""
     half = dim // 2
-    freqs = torch.exp(-math.log(max_period) * torch.arange(0, half, dtype=torch.float32) / half).to(t.device)
-    args = t[:, None].float() * freqs[None]
+    freqs = torch.exp(-math.log(max_period) * torch.arange(0, half, dtype=dtype) / half).to(t.device)
+    args = t[:, None].to(dtype) * freqs[None]
     return torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
 
 
-def t_embedder(sd: Dict[str, Tensor], t: Tensor) -> Tensor:
-    """models/utils.py:61-64 — always fp32 (outside the autocast region, dit_crossattn.py:192)."""
-    h = F.linear(timestep_embedding(t), sd["t_embedder.mlp.0.weight"], sd["t_embedder.mlp.0.bias"])
+def t_embedder(sd: Dict[str, Tensor], t: Tensor, dtype: torch.dtype = torch.float32) -> Tensor:
+    """models/utils.py:61-64 — always fp32 (outside the autocast region, dit_crossattn.py:192); the sinusoid in `dtype`, cast to the
+    weights' dtype."""
+    w0 = sd["t_embedder.mlp.0.weight"]
+    h = F.linear(timestep_embedding(t, dtype=dtype).to(w0.dtype), w0, sd["t_embedder.mlp.0.bias"])
     h = F.silu(h)
     return F.linear(h, sd["t_embedder.mlp.2.weight"], sd["t_embedder.mlp.2.bias"])
 
@@ -91,8 +93,8 @@ def layer_norm(x: Tensor) -> Tensor:
     return F.layer_norm(x, (x.shape[-1],), eps=1e-6)
 
 
-def cross_attention(sd, pre: str, x: Tensor, y: Tensor, H: int, pol: Policy) -> Tensor:
-    """models/attention.py:96-114."""
+def cross_attention(sd, pre: str, x: Tensor, y: Tensor, H: int, pol: Policy, taps: dict | None = None) -> Tensor:
+    """models/attention.py:96-114.  taps (optional): receives "ao", the attention core's output [B,N,D] before proj."""
     B, N, D = x.shape
     M = y.shape[1]
     Dh = D // H
@@ -101,15 +103,19 @@ def cross_attention(sd, pre: str, x: Tensor, y: Tensor, H: int, pol: Policy) -> 
     k = pol.linear(y, sd[pre + "to_k.weight"], sd.get(pre + "to_k.bias")).reshape(B, M, H, Dh)
     v = pol.linear(y, sd[pre + "to_v.weight"], sd.get(pre + "to_v.bias")).reshape(B, M, H, Dh)
     o = attention_core(q, k, v, pol).reshape(B, N, D)
+    if taps is not None:
+        taps["ao"] = o
     return pol.linear(o, sd[pre + "proj.weight"], sd.get(pre + "proj.bias"))
 
 
-def self_attention(sd, pre: str, x: Tensor, H: int, pol: Policy) -> Tensor:
-    """models/attention.py:48-59."""
+def self_attention(sd, pre: str, x: Tensor, H: int, pol: Policy, taps: dict | None = None) -> Tensor:
+    """models/attention.py:48-59.  taps: as for cross_attention."""
     B, N, D = x.shape
     qkv = pol.linear(x, sd[pre + "qkv.weight"], sd.get(pre + "qkv.bias")).reshape(B, N, 3, H, D // H)
     q, k, v = torch.unbind(qkv, 2)
     o = attention_core(q, k, v, pol).reshape(B, N, D)
+    if taps is not None:
+        taps["ao"] = o
     return pol.linear(o, sd[pre + "proj.weight"], sd.get(pre + "proj.bias"))
 
 
@@ -120,24 +126,54 @@ def mlp(sd, pre: str, x: Tensor, pol: Policy) -> Tensor:
     return pol.linear(h, sd[pre + "fc2.weight"], sd[pre + "fc2.bias"])
 
 
-def dit_block(sd, i: int, x: Tensor, y: Tensor, t_emb: Tensor, H: int, pol: Policy) -> Tensor:
-    """models/dit_crossattn.py:51-58 — order is cross-attn, self-attn, MLP; 9 chunks
-    (shift,scale,gate) x (mca,msa,mlp)."""
+def block_modulation(sd, i: int, t_emb: Tensor, pol: Policy):
+    """The 9 adaLN chunks of block i (dit_crossattn.py:54): (shift, scale, gate) x (mca, msa, mlp), each [B, D]."""
     p = f"blocks.{i}."
     mod = pol.linear(F.silu(t_emb), sd[p + "adaLN_modulation.1.weight"], sd[p + "adaLN_modulation.1.bias"])
-    sh_ca, sc_ca, g_ca, sh_sa, sc_sa, g_sa, sh_m, sc_m, g_m = mod.chunk(9, dim=1)
-    x = x + pol.rnd(g_ca.unsqueeze(1) * cross_attention(sd, p + "crossattn.", modulate(layer_norm(x), sh_ca, sc_ca, pol), y, H, pol))
-    x = x + pol.rnd(g_sa.unsqueeze(1) * self_attention(sd, p + "attn.", modulate(layer_norm(x), sh_sa, sc_sa, pol), H, pol))
-    x = x + pol.rnd(g_m.unsqueeze(1) * mlp(sd, p + "mlp.", modulate(layer_norm(x), sh_m, sc_m, pol), pol))
+    return mod.chunk(9, dim=1)
+
+
+# The three branches of DiTBlock._forward (dit_crossattn.py:55-57).  Each returns its increment, the gated amount it adds to the
+# residual stream x; mod_chunks are the block's 9 chunks.  They compute in the dtype of x and sd (fp64 for the stage tests).
+def cross_branch(sd, i: int, x: Tensor, y: Tensor, mod_chunks, H: int, pol: Policy, taps: dict | None = None) -> Tensor:
+    sh, sc, g = mod_chunks[0:3]
+    return pol.rnd(g.unsqueeze(1) * cross_attention(sd, f"blocks.{i}.crossattn.", modulate(layer_norm(x), sh, sc, pol), y, H, pol, taps))
+
+
+def self_branch(sd, i: int, x: Tensor, mod_chunks, H: int, pol: Policy, taps: dict | None = None) -> Tensor:
+    sh, sc, g = mod_chunks[3:6]
+    return pol.rnd(g.unsqueeze(1) * self_attention(sd, f"blocks.{i}.attn.", modulate(layer_norm(x), sh, sc, pol), H, pol, taps))
+
+
+def mlp_branch(sd, i: int, x: Tensor, mod_chunks, pol: Policy) -> Tensor:
+    sh, sc, g = mod_chunks[6:9]
+    return pol.rnd(g.unsqueeze(1) * mlp(sd, f"blocks.{i}.mlp.", modulate(layer_norm(x), sh, sc, pol), pol))
+
+
+def dit_block(sd, i: int, x: Tensor, y: Tensor, t_emb: Tensor, H: int, pol: Policy) -> Tensor:
+    """models/dit_crossattn.py:51-58 — order is cross-attn, self-attn, MLP."""
+    m = block_modulation(sd, i, t_emb, pol)
+    x = x + cross_branch(sd, i, x, y, m, H, pol)
+    x = x + self_branch(sd, i, x, m, H, pol)
+    x = x + mlp_branch(sd, i, x, m, pol)
     return x
+
+
+def final_modulation(sd, t_emb: Tensor, pol: Policy):
+    """(shift, scale) of the final layer (dit_crossattn.py:75), each [B, D]."""
+    mod = pol.linear(F.silu(t_emb), sd["final_layer.adaLN_modulation.1.weight"], sd["final_layer.adaLN_modulation.1.bias"])
+    return mod.chunk(2, dim=1)
+
+
+def final_apply(sd, x: Tensor, shift: Tensor, scale: Tensor, pol: Policy) -> Tensor:
+    """models/dit_crossattn.py:76-78 on given modulation chunks."""
+    return pol.linear(modulate(layer_norm(x), shift, scale, pol), sd["final_layer.linear.weight"], sd["final_layer.linear.bias"])
 
 
 def final_layer(sd, x: Tensor, t_emb: Tensor, pol: Policy) -> Tensor:
     """models/dit_crossattn.py:74-78."""
-    mod = pol.linear(F.silu(t_emb), sd["final_layer.adaLN_modulation.1.weight"], sd["final_layer.adaLN_modulation.1.bias"])
-    shift, scale = mod.chunk(2, dim=1)
-    x = modulate(layer_norm(x), shift, scale, pol)
-    return pol.linear(x, sd["final_layer.linear.weight"], sd["final_layer.linear.bias"])
+    shift, scale = final_modulation(sd, t_emb, pol)
+    return final_apply(sd, x, shift, scale, pol)
 
 
 def depth_of(sd) -> int:

@@ -158,6 +158,27 @@ def test_compute_path_fails_loudly_without_gpu():
     assert raw.tpx_dit_forward_step(None, None, 0, 1, 1, 6.0, None, None, 0, None) == -1
 
 
+def test_dit_debug_entries_reject_bad_arguments(lib):
+    """tpx_dit_debug_stage / tpx_dit_debug_tap check the stop point and the tap before anything else, then their pointers; none of
+    these calls reaches the device.  (A block outside the model's depth needs a handle: tests/test_gpu_dit_stages.py.)"""
+    P = 1 << 20
+    for stage in (-1, 4):
+        assert lib.tpx_dit_debug_stage(P, P, P, 1, 0, 0, stage, P, 1 << 20, None) == -1
+        assert b"bad stage" in lib.tpx_last_error()
+    for h, t in ((None, P), (P, None)):
+        assert lib.tpx_dit_debug_stage(h, P, t, 1, 0, 0, 1, P, 1 << 20, None) == -1
+        assert b"null" in lib.tpx_last_error()
+    for which in (-1, 4):
+        assert lib.tpx_dit_debug_tap(P, P, 2, which, 1, P, None) == -1
+        assert b"bad tap" in lib.tpx_last_error()
+    for n_seq, count in ((2, 0), (2, 3), (0, 0)):
+        assert lib.tpx_dit_debug_tap(P, P, n_seq, 0, count, P, None) == -1
+        assert b"count" in lib.tpx_last_error()
+    for h, ws, dst in ((None, P, P), (P, None, P), (P, P, None)):
+        assert lib.tpx_dit_debug_tap(h, ws, 2, 0, 2, dst, None) == -1
+        assert b"null" in lib.tpx_last_error()
+
+
 def test_schedule_matches_reference_fixture(golden_dir):
     g = np.load(os.path.join(golden_dir, "sampler.npz"))
     for k in (25, 50, 100, 200):

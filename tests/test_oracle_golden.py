@@ -89,6 +89,40 @@ def test_schedule_tables_and_timestep_maps(golden_dir):
         np.testing.assert_allclose(getattr(s, nm), g[nm + "_ddim25"], rtol=1e-12)
 
 
+def _forward_unsplit(sd, x, t, y, H, pol):
+    """DiT.forward written out as one block body (dit_crossattn.py:51-58, 74-78), without the oracle's branch functions."""
+    F = torch.nn.functional
+    d = oracle.dit
+    sd = {k: v.float() for k, v in sd.items()}
+    h = F.linear(x, sd["x_embedder.weight"], sd["x_embedder.bias"])
+    t_emb = d.t_embedder(sd, t)
+    for i in range(d.depth_of(sd)):
+        p = f"blocks.{i}."
+        mod = pol.linear(F.silu(t_emb), sd[p + "adaLN_modulation.1.weight"], sd[p + "adaLN_modulation.1.bias"])
+        sh_ca, sc_ca, g_ca, sh_sa, sc_sa, g_sa, sh_m, sc_m, g_m = mod.chunk(9, dim=1)
+        h = h + pol.rnd(g_ca.unsqueeze(1) * d.cross_attention(sd, p + "crossattn.", d.modulate(d.layer_norm(h), sh_ca, sc_ca, pol), y, H, pol))
+        h = h + pol.rnd(g_sa.unsqueeze(1) * d.self_attention(sd, p + "attn.", d.modulate(d.layer_norm(h), sh_sa, sc_sa, pol), H, pol))
+        h = h + pol.rnd(g_m.unsqueeze(1) * d.mlp(sd, p + "mlp.", d.modulate(d.layer_norm(h), sh_m, sc_m, pol), pol))
+    mod = pol.linear(F.silu(t_emb), sd["final_layer.adaLN_modulation.1.weight"], sd["final_layer.adaLN_modulation.1.bias"])
+    shift, scale = mod.chunk(2, dim=1)
+    return pol.linear(d.modulate(d.layer_norm(h), shift, scale, pol), sd["final_layer.linear.weight"], sd["final_layer.linear.bias"])
+
+
+@pytest.mark.parametrize("precision", ["fp32", "fp16"])
+def test_dit_branch_functions_compose_to_forward_bit_for_bit(golden_dir, precision):
+    """oracle.dit.forward, built from cross_branch / self_branch / mlp_branch / final_apply (the pieces the GPU stage tests run one at
+    a time), equals the undivided block body bit for bit in fp32, under both policies."""
+    g = _load(golden_dir, "dit_cfg1.npz")
+    cfg = json.loads(str(g["cfg"]))
+    sd = synth.synth_state_dict(synth.dit_shapes(**cfg), int(g["seed"]))
+    x, y = synth.synth_inputs(2, cfg["seq_length"], cfg["in_channels"], int(g["M"]), cfg["condition_channels"], 77)
+    t = torch.tensor([0, 999])
+    with torch.no_grad():
+        want = _forward_unsplit(sd, x, t, y, cfg["num_heads"], oracle.dit.Policy(precision))
+        got = oracle.dit.forward(sd, x, t, y, cfg["num_heads"], precision)
+    assert got.dtype == torch.float32 and torch.equal(got, want)
+
+
 def _tiny_model(golden_dir):
     g = _load(golden_dir, "dit_tiny.npz")
     cfg = json.loads(str(g["cfg"]))
