@@ -20,7 +20,7 @@ from .vae import VAE  # noqa: F401
 __version__ = "0.1.0"
 
 
-def install(mcubes: bool = False, nvdiffrast: bool = False, uv_unwrap: bool = False) -> None:
+def install(mcubes: bool = False, nvdiffrast: bool = False, uv_unwrap: bool = False, meshutils: bool = False) -> None:
     """Make the reference's import paths resolve to this implementation, so ``inference.py`` / ``app.py`` run
     unchanged:  ``models.dit_crossattn`` -> dit, ``models.vae3d_dib`` -> vae, ``models.diffusion`` -> diffusion,
     ``models.primsdf`` -> primsdf, ``models.conditioner.image_dinov2`` -> dinov2, ``dva.ray_marcher`` -> ray_marcher.
@@ -30,7 +30,8 @@ def install(mcubes: bool = False, nvdiffrast: bool = False, uv_unwrap: bool = Fa
     extract_texmesh (inference.py:119) runs without PyMCubes; by default ``mcubes`` is left alone.  ``nvdiffrast=True`` likewise binds
     ``sys.modules["nvdiffrast"]`` / ``["nvdiffrast.torch"]`` to the forward-only UV-space rasteriser of ``bake`` (inference.py:22,31,172-174).
     ``uv_unwrap=True`` binds ``sys.modules["utils.uv_unwrap"]`` (and the attribute of an importable ``utils`` package) to the GPU
-    box-projection unwrap of ``unwrap`` (inference.py:142-143)."""
+    box-projection unwrap of ``unwrap`` (inference.py:142-143).  ``meshutils=True`` binds ``sys.modules["utils.meshutils"]`` (and the
+    attribute) to ``clean_mesh`` / ``decimate_mesh`` of ``mesh`` (inference.py:126-129), so the export path needs no pymeshlab."""
     try:
         import models as ref_models  # the reference checkout, when it is on sys.path
     except Exception:
@@ -60,11 +61,12 @@ def install(mcubes: bool = False, nvdiffrast: bool = False, uv_unwrap: bool = Fa
         sys.modules["mcubes"] = mesh.mcubes_module()
     if nvdiffrast:
         sys.modules["nvdiffrast"], sys.modules["nvdiffrast.torch"] = bake.nvdiffrast_modules()
-    if uv_unwrap:
-        m = unwrap.uv_unwrap_module()
-        sys.modules["utils.uv_unwrap"] = m
-        try:
-            import utils as ref_utils
-            setattr(ref_utils, "uv_unwrap", m)
-        except Exception:
-            pass
+    for flag, name, make in ((uv_unwrap, "uv_unwrap", unwrap.uv_unwrap_module), (meshutils, "meshutils", mesh.meshutils_module)):
+        if flag:
+            m = make()
+            sys.modules["utils." + name] = m
+            try:
+                import utils as ref_utils
+                setattr(ref_utils, name, m)
+            except Exception:
+                pass

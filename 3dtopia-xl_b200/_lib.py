@@ -87,6 +87,12 @@ SIGNATURES = {
     "tpx_decimate_workspace_bytes": (_sz, [_i64, _i64]),
     "tpx_decimate": (_i, [_vp, _i64, _vp, _i64, _i64, _vp, _sz, _vp, _vp, _i64, _vp]),
     "tpx_decimate_emit": (_i, [_i64, _i64, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_mesh_weld_workspace_bytes": (_sz, [_i64, _i64]),
+    "tpx_mesh_weld_count": (_i, [_vp, _i64, _vp, _i64, C.c_double, _vp, _sz, _vp, _vp]),
+    "tpx_mesh_weld_emit": (_i, [_vp, _i64, _i64, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_mesh_repair_workspace_bytes": (_sz, [_i64, _i64]),
+    "tpx_mesh_repair_count": (_i, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
+    "tpx_mesh_repair_emit": (_i, [_vp, _i64, _i64, _vp, _sz, _vp, _vp, _vp]),
     "tpx_uv_unwrap_workspace_bytes": (_sz, [_i64, _i64]),
     "tpx_vertex_normals": (_i, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
     "tpx_uv_unwrap": (_i, [_vp, _vp, _i64, _vp, _i64, C.c_double, _vp, _sz, _vp, _vp, _vp]),

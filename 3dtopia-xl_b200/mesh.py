@@ -7,7 +7,9 @@ in index units, component d along array axis d, shared between triangles; faces 
 this differs from PyMCubes.
 
 ``remove_small_components`` and ``decimate`` (csrc/mesh_simplify.cu) are the clean_mesh / decimate_mesh calls extract_texmesh makes
-next (inference.py:126-129, pymeshlab there); see INTEGRATION.md for how they differ from pymeshlab.
+next (inference.py:126-129, pymeshlab there); see INTEGRATION.md for how they differ from pymeshlab.  ``clean_mesh`` and
+``decimate_mesh`` are the whole utils/meshutils.py calls (close-vertex merge, duplicate / null faces, components, non-manifold repair);
+``install(meshutils=True)`` binds them as ``utils.meshutils``.
 """
 from __future__ import annotations
 
@@ -73,8 +75,9 @@ def marching_cubes(volume, isovalue: float = 0.0):
     return verts.cpu().numpy().astype(np.float64), faces.cpu().numpy()
 
 
-def _check_mesh(verts: torch.Tensor, faces: torch.Tensor):
-    """ValueError unless verts is fp32 [V,3] and faces int64 [F,3] with every index in [0, V) and three distinct indices per face."""
+def _check_mesh(verts: torch.Tensor, faces: torch.Tensor, allow_repeat: bool = False):
+    """ValueError unless verts is fp32 [V,3] and faces int64 [F,3] with every index in [0, V) and (unless allow_repeat) three distinct
+    indices per face."""
     if verts.dim() != 2 or verts.shape[1] != 3 or verts.dtype != torch.float32:
         raise ValueError(f"verts must be float32 [V,3], got {verts.dtype} {tuple(verts.shape)}")
     if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype != torch.int64:
@@ -85,7 +88,7 @@ def _check_mesh(verts: torch.Tensor, faces: torch.Tensor):
     if F:
         if int(faces.min()) < 0 or int(faces.max()) >= V:
             raise ValueError(f"a face index is outside [0, {V})")
-        if bool(((faces[:, 0] == faces[:, 1]) | (faces[:, 1] == faces[:, 2]) | (faces[:, 2] == faces[:, 0])).any()):
+        if not allow_repeat and bool(((faces[:, 0] == faces[:, 1]) | (faces[:, 1] == faces[:, 2]) | (faces[:, 2] == faces[:, 0])).any()):
             raise ValueError("a face repeats a vertex index")
 
 
@@ -133,7 +136,63 @@ def _decimate(verts: torch.Tensor, faces: torch.Tensor, target: int, trace: list
     return vo, fo
 
 
-def _mesh_call(fn, verts, faces, *args):
+def _weld(verts: torch.Tensor, faces: torch.Tensor, merge_distance: float, info: dict | None = None):
+    """CUDA verts / faces (range-checked; faces may repeat an index) -> the merged mesh without duplicate or null faces, on their
+    device; ``info`` (a dict) receives the merge rounds."""
+    dev = verts.device
+    V, F = verts.shape[0], faces.shape[0]
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        nbytes = int(lib.tpx_mesh_weld_workspace_bytes(V, F))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        counts = torch.empty(3, dtype=torch.int64, device=dev)
+        st = _lib.stream_ptr()
+        _lib.check(lib.tpx_mesh_weld_count(verts.data_ptr(), V, faces.data_ptr(), F, float(merge_distance), ws.data_ptr(), nbytes, counts.data_ptr(), st),
+                   "tpx_mesh_weld_count")
+        Vo, Fo, rounds = counts.tolist()
+        if Vo < 0:
+            raise ValueError("a face index is outside [0, V)")
+        if info is not None:
+            info["rounds"] = rounds
+        vo = torch.empty(Vo, 3, dtype=torch.float32, device=dev)
+        fo = torch.empty(Fo, 3, dtype=torch.int64, device=dev)
+        _lib.check(lib.tpx_mesh_weld_emit(verts.data_ptr(), V, F, ws.data_ptr(), nbytes, vo.data_ptr(), fo.data_ptr(), st), "tpx_mesh_weld_emit")
+    return vo, fo
+
+
+def _repair(verts: torch.Tensor, faces: torch.Tensor):
+    """CUDA verts / faces (checked) -> the mesh with non-manifold edges and vertices repaired, on their device."""
+    dev = verts.device
+    V, F = verts.shape[0], faces.shape[0]
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        nbytes = int(lib.tpx_mesh_repair_workspace_bytes(V, F))
+        if nbytes == 0:
+            raise ValueError(f"repair: {F} faces: must be below 2^30")
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        counts = torch.empty(2, dtype=torch.int64, device=dev)
+        st = _lib.stream_ptr()
+        _lib.check(lib.tpx_mesh_repair_count(verts.data_ptr(), V, faces.data_ptr(), F, ws.data_ptr(), nbytes, counts.data_ptr(), st), "tpx_mesh_repair_count")
+        Vo, Fo = counts.tolist()
+        if Vo < 0:
+            raise ValueError("a face index is outside [0, V) or a face repeats an index")
+        vo = torch.empty(Vo, 3, dtype=torch.float32, device=dev)
+        fo = torch.empty(Fo, 3, dtype=torch.int64, device=dev)
+        _lib.check(lib.tpx_mesh_repair_emit(verts.data_ptr(), V, F, ws.data_ptr(), nbytes, vo.data_ptr(), fo.data_ptr(), st), "tpx_mesh_repair_emit")
+    return vo, fo
+
+
+def _clean(verts: torch.Tensor, faces: torch.Tensor, merge_distance: float, min_faces: int, min_diameter: float, repair: bool):
+    """The steps of clean_mesh in the reference's order: weld / duplicate / null faces, components, then the non-manifold repair."""
+    v, f = _weld(verts, faces, merge_distance)
+    if min_faces > 0 or min_diameter > 0:
+        v, f = _remove_small(v, f, min_faces, min_diameter)
+    if repair:
+        v, f = _repair(v, f)
+    return v, f
+
+
+def _mesh_call(fn, verts, faces, *args, allow_repeat: bool = False):
     """The marching_cubes convention: CUDA tensors in, CUDA tensors out; numpy in, numpy float64 / int64 out from the current device."""
     if isinstance(verts, torch.Tensor) or isinstance(faces, torch.Tensor):
         if not (isinstance(verts, torch.Tensor) and isinstance(faces, torch.Tensor)):
@@ -143,7 +202,7 @@ def _mesh_call(fn, verts, faces, *args):
         if verts.device != faces.device:
             raise ValueError(f"verts on {verts.device}, faces on {faces.device}")
         verts, faces = verts.contiguous(), faces.contiguous()
-        _check_mesh(verts, faces)
+        _check_mesh(verts, faces, allow_repeat)
         return fn(verts, faces, *args)
     v, f = np.asarray(verts), np.asarray(faces)
     if v.ndim != 2 or v.shape[1] != 3 or f.ndim != 2 or f.shape[1] != 3 or not np.issubdtype(f.dtype, np.integer):
@@ -152,7 +211,7 @@ def _mesh_call(fn, verts, faces, *args):
     dev = torch.device("cuda", torch.cuda.current_device())
     vt = torch.from_numpy(np.ascontiguousarray(v, dtype=np.float32)).to(dev)
     ft = torch.from_numpy(np.ascontiguousarray(f, dtype=np.int64)).to(dev)
-    _check_mesh(vt, ft)
+    _check_mesh(vt, ft, allow_repeat)
     vo, fo = fn(vt, ft, *args)
     return vo.cpu().numpy().astype(np.float64), fo.cpu().numpy()
 
@@ -179,6 +238,44 @@ def decimate(verts, faces, target_faces: int):
     if int(target_faces) < 0:
         raise ValueError(f"target_faces must be >= 0, got {target_faces}")
     return _mesh_call(_decimate, verts, faces, int(target_faces))
+
+
+def clean_mesh(verts, faces, v_pct=1, min_f=64, min_d=20, repair=True, remesh=True, remesh_size=0.01, remesh_iters=3):
+    """clean_mesh of utils/meshutils.py:118-193 (called at inference.py:126 as clean_mesh(v, t, min_f=8, min_d=5, repair=True,
+    remesh=False)), with its signature and defaults, on the GPU.  In the reference's order: unreferenced vertices dropped; vertices
+    within ``v_pct`` % of the box diagonal merged greedily onto the earliest seed (skipped for v_pct = 0); faces that repeat an index,
+    duplicate faces (same vertex set; the lowest face id stays) and zero-area faces removed; components below ``min_d`` % of the diagonal
+    and below ``min_f`` faces removed; with ``repair``, faces removed from non-manifold edges and non-manifold vertices split.  The rules
+    are this package's reading of pymeshlab / VCG (DESIGN.md §1 "clean-up contract").  Isotropic remeshing is not implemented:
+    ``remesh=True`` (the default, as in the reference) raises NotImplementedError; pass remesh=False as inference.py does.
+    Unlike ``remove_small_components`` the faces may repeat an index.  Output: the surviving vertices in ascending original id, then
+    the split copies; the faces in their original order, remapped, winding unchanged; no face repeats an index, so the result feeds
+    ``decimate``.  Inputs and outputs otherwise as ``remove_small_components``."""
+    if remesh:
+        raise NotImplementedError("clean_mesh: isotropic remeshing is not implemented; pass remesh=False (as inference.py:126 does)")
+    if v_pct < 0 or min_f < 0 or min_d < 0:
+        raise ValueError(f"v_pct, min_f and min_d must be >= 0, got {v_pct}, {min_f}, {min_d}")
+    return _mesh_call(_clean, verts, faces, float(v_pct) / 100.0, int(min_f), float(min_d) / 100.0, bool(repair), allow_repeat=True)
+
+
+def decimate_mesh(verts, faces, target=5e4, backend="pymeshlab", remesh=False, optimalplacement=True):
+    """decimate_mesh of utils/meshutils.py:63-115 (inference.py:129): ``decimate`` to int(target) faces.  backend="pyfqmr",
+    remesh=True and optimalplacement=False are not implemented and raise NotImplementedError."""
+    if backend != "pymeshlab":
+        raise NotImplementedError(f"decimate_mesh: backend {backend!r} is not implemented (the quadric decimation of `decimate` stands in for pymeshlab)")
+    if remesh:
+        raise NotImplementedError("decimate_mesh: isotropic remeshing is not implemented; pass remesh=False")
+    if not optimalplacement:
+        raise NotImplementedError("decimate_mesh: only optimal placement is implemented")
+    return decimate(verts, faces, int(target))
+
+
+def meshutils_module() -> types.ModuleType:
+    """A module named ``utils.meshutils`` exposing ``clean_mesh`` and ``decimate_mesh``: what extract_texmesh imports (inference.py:126-129)."""
+    m = types.ModuleType("utils.meshutils", "GPU mesh clean-up and decimation of 3dtopia-xl_b200 (tpxl_b200.mesh) under the reference's import name.")
+    m.clean_mesh = clean_mesh
+    m.decimate_mesh = decimate_mesh
+    return m
 
 
 def mcubes_module() -> types.ModuleType:

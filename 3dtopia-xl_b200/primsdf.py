@@ -89,24 +89,34 @@ class PrimSDF(nn.Module):
         return grid
 
     def extract_mesh(self, resolution: int = 256, isovalue: float = 0.0, bound: float = 1.0, *, min_faces: int = 0, min_diameter: float = 0.0,
-                     target_faces: int | None = None):
+                     target_faces: int | None = None, merge_distance: float = 0.0, repair: bool = False):
         """Surface of the sdf field on the GPU: ``sdf_grid`` + marching cubes, in world coordinates (origin -bound, spacing
         2 bound / (R - 1)), i.e. inference.py:107-124 without the host copy.  Returns (verts fp32 [V,3], faces int64 [F,3]) on the
-        module's device.  Then, in the order of inference.py:126-129: when ``min_faces`` > 0 or ``min_diameter`` > 0,
-        ``mesh.remove_small_components`` with those thresholds; when ``target_faces`` is set, ``mesh.decimate`` to it (see its note on
-        unreachable targets).  ``extract_mesh(256, min_faces=8, min_diameter=0.05, target_faces=100000)`` is the geometry of
-        extract_texmesh up to the parts of clean_mesh this package does not implement (DESIGN.md §8).  The defaults run marching cubes
-        only.  The primitive noise filter of extract_texmesh (:90-103) is ``noise_filter_mask``; ``extract_texmesh`` runs it first."""
+        module's device.  Then, in the order of inference.py:126-129 (clean_mesh, then decimate_mesh): when ``merge_distance`` > 0 or
+        ``repair`` is set, the close-vertex merge (``merge_distance`` a fraction of the box diagonal, 0.01 for v_pct = 1; 0 merges
+        nothing) with duplicate and zero-area faces removed; when ``min_faces`` > 0 or ``min_diameter`` > 0,
+        ``mesh.remove_small_components`` with those thresholds; when ``repair`` is set, the non-manifold edge and vertex repair; when
+        ``target_faces`` is set, ``mesh.decimate`` to it (see its note on unreachable targets).
+        ``extract_mesh(256, min_faces=8, min_diameter=0.05, target_faces=100000, merge_distance=0.01, repair=True)`` is the geometry of
+        extract_texmesh as this package reads clean_mesh (DESIGN.md §1 "clean-up contract"; remeshing is off there).  The defaults run
+        marching cubes only.  The primitive noise filter of extract_texmesh (:90-103) is ``noise_filter_mask``; ``extract_texmesh``
+        runs it first."""
         R = int(resolution)
         if R < 2:
             raise ValueError(f"resolution must be >= 2, got {resolution}")
         if target_faces is not None and int(target_faces) < 0:
             raise ValueError(f"target_faces must be >= 0, got {target_faces}")
+        if not merge_distance >= 0:
+            raise ValueError(f"merge_distance must be >= 0, got {merge_distance}")
         grid = self.sdf_grid(R, bound)
         step = 2.0 * bound / (R - 1)
         v, f = mesh._mesh(grid, isovalue, origin=(-bound,) * 3, spacing=(step,) * 3)
+        if merge_distance > 0 or repair:
+            v, f = mesh._weld(v, f, float(merge_distance))
         if min_faces > 0 or min_diameter > 0:
             v, f = mesh._remove_small(v, f, int(min_faces), float(min_diameter))
+        if repair:
+            v, f = mesh._repair(v, f)
         if target_faces is not None:
             v, f = mesh._decimate(v, f, int(target_faces))
         return v, f
@@ -155,9 +165,11 @@ class PrimSDF(nn.Module):
         return unwrap.noise_filter(self.srt_param.detach())
 
     def extract_texmesh(self, resolution: int = 256, target_faces: int = 100000, atlas: int = 1024, island_padding: float = 0.02, min_faces: int = 8,
-                        min_diameter: float = 0.05):
+                        min_diameter: float = 0.05, merge_distance: float = 0.0, repair: bool = False):
         """The fast-unwrap branch of extract_texmesh (inference.py:90-222) on the device, without touching this module's parameters:
-        the noise filter, ``extract_mesh(resolution, min_faces=, min_diameter=, target_faces=)`` of the kept primitives, vertex normals,
+        the noise filter, ``extract_mesh(resolution, min_faces=, min_diameter=, target_faces=, merge_distance=, repair=)`` of the kept
+        primitives (the reference's clean_mesh is ``extract_texmesh(256, 100000, 1024, 0.02, 8, 0.05, merge_distance=0.01,
+        repair=True)``; the defaults leave the close-vertex merge and the repair out), vertex normals,
         the box-projection unwrap, the per-corner re-indexing of :144-148 and ``bake_texture`` at ``atlas`` x ``atlas``.  Returns a dict
         of device tensors in the layout :222 hands to Mesh: ``v`` fp32 [V,3] / ``f`` int64 [F,3] (the indexed mesh), ``vt`` fp32 [3F,2],
         ``ft`` int64 [F,3] (= arange), ``albedo`` and ``metallicRoughness`` fp32 [atlas, atlas, 3] (feats / 255).  The caller's
@@ -168,7 +180,8 @@ class PrimSDF(nn.Module):
         sub.srt_param.data = self.srt_param.detach()[keep].contiguous()
         sub.feat_param.data = self.feat_param.detach()[keep].contiguous()
         sub.train(self.training)
-        v, f = sub.extract_mesh(resolution, min_faces=min_faces, min_diameter=min_diameter, target_faces=target_faces)
+        v, f = sub.extract_mesh(resolution, min_faces=min_faces, min_diameter=min_diameter, target_faces=target_faces, merge_distance=merge_distance,
+                                repair=repair)
         if f.shape[0] == 0:
             raise ValueError("the filtered field has no surface at this resolution")
         n = unwrap.compute_vertex_normal(v, f)

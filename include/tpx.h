@@ -306,6 +306,33 @@ size_t tpx_decimate_workspace_bytes(int64_t V, int64_t F);
 int tpx_decimate(const float* verts_dev, int64_t V, const int64_t* faces_dev, int64_t F, int64_t target, void* ws, size_t ws_bytes, int64_t* counts_dev,
                  int64_t* trace_host, int64_t trace_cap, void* stream);
 int tpx_decimate_emit(int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out_dev, int64_t* faces_out_dev, void* stream);
+/* clean_mesh(v, t, v_pct, ..., repair=True, remesh=False) (utils/meshutils.py:118-193, called at inference.py:126), the filters before and
+ * after the component filter, as this package reads VCG (DESIGN.md §1 "clean-up contract"; pymeshlab itself is not run anywhere here).
+ * Weld: meshing_remove_unreferenced_vertices, meshing_merge_close_vertices(PercentageValue(100 merge_distance)),
+ * meshing_remove_duplicate_faces, meshing_remove_null_faces.  Faces may repeat an index (such faces are dropped); an index outside [0, V)
+ * makes _count write -1, -1.  merge_distance = 0 merges nothing.  Greedy in ascending id: a referenced vertex is a seed iff no earlier
+ * seed lies within r = merge_distance x the box diagonal of the referenced vertices (fp64 dx² + dy² + dz² < r²), otherwise it takes
+ * the smallest such seed's id; faces onto the seeds, then a face is kept iff its indices are distinct, no lower face id has the same
+ * index set and (v1 - v0) x (v2 - v0) is not exactly zero.  _count writes counts_dev[0] = V_out, [1] = F_out, [2] = merge rounds
+ * and SYNCHRONISES (it reads the undecided count back every 8 rounds, and once at the end); _emit does not synchronise.
+ * About 100 bytes of workspace per face plus 180 per vertex. */
+size_t tpx_mesh_weld_workspace_bytes(int64_t V, int64_t F);
+int tpx_mesh_weld_count(const float* verts_dev, int64_t V, const int64_t* faces_dev, int64_t F, double merge_distance, void* ws, size_t ws_bytes,
+                        int64_t* counts_dev, void* stream);
+int tpx_mesh_weld_emit(const float* verts_dev, int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out_dev, int64_t* faces_out_dev,
+                       void* stream);
+/* clean_mesh's repair=True (utils/meshutils.py:118-193, inference.py:126): meshing_repair_non_manifold_edges(method=0) then
+ * meshing_repair_non_manifold_vertices(vertdispratio=0).  Input as the component filter (no repeated index; F below 2^30).  The faces
+ * on an edge with more than two faces are visited in ascending (doubled area, face id); one is deleted iff one of its edges still has
+ * more than two faces.  Then every vertex whose faces form more than one fan (edge-connected around it) keeps the fan with the smallest
+ * face id; each other fan gets a copy at the same position, appended after the surviving vertices in (vertex id, smallest face id of
+ * the fan) order.  _count writes counts_dev[0] = V_out, [1] = F_out (both -1 for malformed faces); neither call synchronises.
+ * About 270 bytes of workspace per face. */
+size_t tpx_mesh_repair_workspace_bytes(int64_t V, int64_t F);
+int tpx_mesh_repair_count(const float* verts_dev, int64_t V, const int64_t* faces_dev, int64_t F, void* ws, size_t ws_bytes, int64_t* counts_dev,
+                          void* stream);
+int tpx_mesh_repair_emit(const float* verts_dev, int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out_dev, int64_t* faces_out_dev,
+                         void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Box-projection UV unwrap and the primitive noise filter — the fast-unwrap branch of extract_texmesh (inference.py:140-150:
