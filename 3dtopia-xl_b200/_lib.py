@@ -93,6 +93,13 @@ SIGNATURES = {
     "tpx_mesh_repair_workspace_bytes": (_sz, [_i64, _i64]),
     "tpx_mesh_repair_count": (_i, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
     "tpx_mesh_repair_emit": (_i, [_vp, _i64, _i64, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_remesh_workspace_bytes": (_sz, [_i64, _i64]),
+    "tpx_remesh_grid_bytes": (_sz, [_i64]),
+    "tpx_remesh_begin": (_i, [_vp, _i64, _vp, _i64, C.c_double, _vp, _sz, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_remesh_closest": (_i, [_vp, _i64, _vp, _i64, _i64, _vp, _sz, _vp, _vp, _vp]),
+    "tpx_remesh_split_count": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, C.c_double, _vp, _sz, _vp, _vp]),
+    "tpx_remesh_split_emit": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "tpx_remesh_relax": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _sz, C.c_double, C.c_double, _vp, _sz, _vp, _vp]),
     "tpx_uv_unwrap_workspace_bytes": (_sz, [_i64, _i64]),
     "tpx_vertex_normals": (_i, [_vp, _i64, _vp, _i64, _vp, _sz, _vp, _vp]),
     "tpx_uv_unwrap": (_i, [_vp, _vp, _i64, _vp, _i64, C.c_double, _vp, _sz, _vp, _vp, _vp]),

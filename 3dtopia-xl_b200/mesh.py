@@ -14,6 +14,8 @@ next (inference.py:126-129, pymeshlab there); see INTEGRATION.md for how they di
 from __future__ import annotations
 
 import ctypes as C
+import math
+import time
 import types
 
 import numpy as np
@@ -182,6 +184,91 @@ def _repair(verts: torch.Tensor, faces: torch.Tensor):
     return vo, fo
 
 
+def _remesh(verts: torch.Tensor, faces: torch.Tensor, target_len: float, iterations: int, feature_deg: float, info: list | None = None):
+    """CUDA verts / faces (checked) -> the remeshed, compacted mesh on their device; ``info`` (a list) receives per iteration
+    dict(F=[faces after split, collapse, flip], V=vertex slots, collapse_rounds, flip_rounds, split_ms, relax_ms) (host clock around a
+    synchronise)."""
+    dev = verts.device
+    V0, F0 = verts.shape[0], faces.shape[0]
+    lib = _lib.lib()
+    cosf = math.cos(math.radians(feature_deg))
+    v, f = verts, faces
+    with torch.cuda.device(dev):
+        st = _lib.stream_ptr()
+        gbytes = int(lib.tpx_remesh_grid_bytes(F0))
+        nbytes = int(lib.tpx_remesh_workspace_bytes(V0, F0))
+        if gbytes == 0 or nbytes == 0:
+            raise ValueError(f"remesh: {F0} faces: must be below 2^28")
+        grid = torch.empty(gbytes, dtype=torch.uint8, device=dev)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        creases = torch.empty(max(3 * F0, 1), dtype=torch.int64, device=dev)
+        counts = torch.empty(3, dtype=torch.int64, device=dev)
+        _lib.check(lib.tpx_remesh_begin(verts.data_ptr(), V0, faces.data_ptr(), F0, cosf, grid.data_ptr(), gbytes, ws.data_ptr(), nbytes,
+                                        creases.data_ptr(), counts.data_ptr(), st), "tpx_remesh_begin")
+        nC = int(counts[0])
+        if nC < 0:
+            raise ValueError("a face index is outside [0, V) or a face repeats an index")
+        creases = creases[:nC]
+        v = verts.clone()
+        for _ in range(iterations):
+            t0 = time.perf_counter()
+            V, F = v.shape[0], f.shape[0]
+            nbytes = int(lib.tpx_remesh_workspace_bytes(V, F))
+            if nbytes == 0:
+                raise _lib.TpxError(f"remesh: {V} vertices / {F} faces exceed the index range")
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            _lib.check(lib.tpx_remesh_split_count(v.data_ptr(), V, f.data_ptr(), F, creases.data_ptr(), nC, float(target_len), ws.data_ptr(), nbytes,
+                                                  counts.data_ptr(), st), "tpx_remesh_split_count")
+            Vs, Fs, nCs = counts.tolist()
+            if Vs >= _INDEX_LIMIT or 2 * Fs >= _INDEX_LIMIT:
+                raise _lib.TpxError(f"remesh: the split gives {Vs} vertices / {Fs} faces, over the index range")
+            vs = torch.empty(Vs, 3, dtype=torch.float32, device=dev)
+            fs = torch.empty(Fs, 3, dtype=torch.int64, device=dev)
+            cs = torch.empty(max(nCs, 1), dtype=torch.int64, device=dev)
+            _lib.check(lib.tpx_remesh_split_emit(v.data_ptr(), V, F, creases.data_ptr(), nC, nCs, ws.data_ptr(), nbytes, vs.data_ptr(), fs.data_ptr(),
+                                                 cs.data_ptr(), st), "tpx_remesh_split_emit")
+            v, f, creases, nC = vs, fs, cs[:nCs], nCs
+            if info is not None:
+                torch.cuda.synchronize(dev)
+            t1 = time.perf_counter()
+            nbytes = int(lib.tpx_remesh_workspace_bytes(Vs, Fs))
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            _lib.check(lib.tpx_remesh_relax(v.data_ptr(), Vs, f.data_ptr(), Fs, creases.data_ptr(), nC, verts.data_ptr(), V0, F0, grid.data_ptr(), gbytes,
+                                            float(target_len), cosf, ws.data_ptr(), nbytes, counts.data_ptr(), st), "tpx_remesh_relax")
+            Fr, rc, rf = counts.tolist()
+            if info is not None:
+                info.append(dict(F=[Fs, Fr, Fr], V=Vs, collapse_rounds=rc, flip_rounds=rf, split_ms=round((t1 - t0) * 1e3, 2),
+                                 relax_ms=round((time.perf_counter() - t1) * 1e3, 2)))
+            f = f[:Fr]
+    return _remove_small(v, f.contiguous(), 0, 0.0)          # the compaction: referenced vertices in ascending id, faces in order
+
+
+def _closest(verts: torch.Tensor, faces: torch.Tensor, pts: torch.Tensor):
+    """CUDA verts / faces (checked), pts fp32 [n,3] on their device -> (closest points fp32 [n,3], face ids int64 [n]) of the mesh: the
+    projection step of ``remesh`` on its own, through the same grid."""
+    dev = verts.device
+    V, F, n = verts.shape[0], faces.shape[0], pts.shape[0]
+    lib = _lib.lib()
+    with torch.cuda.device(dev):
+        gbytes, nbytes = int(lib.tpx_remesh_grid_bytes(F)), int(lib.tpx_remesh_workspace_bytes(V, F))
+        if gbytes == 0 or nbytes == 0:
+            raise ValueError(f"closest: {F} faces: must be below 2^28")
+        grid = torch.empty(gbytes, dtype=torch.uint8, device=dev)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        creases = torch.empty(max(3 * F, 1), dtype=torch.int64, device=dev)
+        counts = torch.empty(1, dtype=torch.int64, device=dev)
+        st = _lib.stream_ptr()
+        _lib.check(lib.tpx_remesh_begin(verts.data_ptr(), V, faces.data_ptr(), F, 1.0, grid.data_ptr(), gbytes, ws.data_ptr(), nbytes, creases.data_ptr(),
+                                        counts.data_ptr(), st), "tpx_remesh_begin")
+        if int(counts[0]) < 0:
+            raise ValueError("a face index is outside [0, V) or a face repeats an index")
+        out = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        fid = torch.empty(n, dtype=torch.int64, device=dev)
+        _lib.check(lib.tpx_remesh_closest(pts.data_ptr(), n, verts.data_ptr(), V, F, grid.data_ptr(), gbytes, out.data_ptr(), fid.data_ptr(), st),
+                   "tpx_remesh_closest")
+    return out, fid
+
+
 def _clean(verts: torch.Tensor, faces: torch.Tensor, merge_distance: float, min_faces: int, min_diameter: float, repair: bool):
     """The steps of clean_mesh in the reference's order: weld / duplicate / null faces, components, then the non-manifold repair."""
     v, f = _weld(verts, faces, merge_distance)
@@ -240,14 +327,36 @@ def decimate(verts, faces, target_faces: int):
     return _mesh_call(_decimate, verts, faces, int(target_faces))
 
 
+def remesh(verts, faces, target_len: float, iterations: int = 3, feature_deg: float = 30.0, info: list | None = None):
+    """Isotropic remeshing toward edges of length ``target_len``: the GPU stand-in for pymeshlab's
+    meshing_isotropic_explicit_remeshing(iterations, targetlen) that decimate_mesh(..., remesh=True) runs after the decimation
+    (utils/meshutils.py:101-105, inference.py:128-129, where targetlen is PercentageValue(1), 1 % of the box diagonal).  Per iteration,
+    in VCG's order: split edges above 4/3 target_len, collapse edges below 4/5 target_len, flip edges toward valence 6 (4 at the
+    border), one tangential smoothing pass, then project every moved vertex onto the closest point of the input mesh.  Border,
+    non-manifold vertices and the ends of crease edges (faces meeting beyond ``feature_deg`` degrees) never move.  The rules are this
+    package's reading of VCG (DESIGN.md §1 "Isotropic remeshing contract"), not checked against pymeshlab.  ``iterations = 0`` returns
+    the input without its unreferenced vertices.  ``info`` (a list) receives per iteration the face counts after split, collapse and
+    flip and the round counts.  Inputs and outputs as ``remove_small_components``; ValueError also for a ``target_len`` that is not
+    finite and positive, ``iterations < 0`` or ``feature_deg`` outside [0, 180]."""
+    L, it, fd = float(target_len), int(iterations), float(feature_deg)
+    if not (math.isfinite(L) and L > 0):
+        raise ValueError(f"target_len must be finite and > 0, got {target_len}")
+    if it < 0:
+        raise ValueError(f"iterations must be >= 0, got {iterations}")
+    if not 0.0 <= fd <= 180.0:
+        raise ValueError(f"feature_deg must be in [0, 180], got {feature_deg}")
+    return _mesh_call(_remesh, verts, faces, L, it, fd, info)
+
+
 def clean_mesh(verts, faces, v_pct=1, min_f=64, min_d=20, repair=True, remesh=True, remesh_size=0.01, remesh_iters=3):
     """clean_mesh of utils/meshutils.py:118-193 (called at inference.py:126 as clean_mesh(v, t, min_f=8, min_d=5, repair=True,
     remesh=False)), with its signature and defaults, on the GPU.  In the reference's order: unreferenced vertices dropped; vertices
     within ``v_pct`` % of the box diagonal merged greedily onto the earliest seed (skipped for v_pct = 0); faces that repeat an index,
     duplicate faces (same vertex set; the lowest face id stays) and zero-area faces removed; components below ``min_d`` % of the diagonal
     and below ``min_f`` faces removed; with ``repair``, faces removed from non-manifold edges and non-manifold vertices split.  The rules
-    are this package's reading of pymeshlab / VCG (DESIGN.md §1 "clean-up contract").  Isotropic remeshing is not implemented:
-    ``remesh=True`` (the default, as in the reference) raises NotImplementedError; pass remesh=False as inference.py does.
+    are this package's reading of pymeshlab / VCG (DESIGN.md §1 "clean-up contract").  ``remesh=True`` (the default, as in the
+    reference) raises NotImplementedError; pass remesh=False as inference.py does, and call ``remesh`` for the isotropic remeshing
+    (binding it here is left to a later change).
     Unlike ``remove_small_components`` the faces may repeat an index.  Output: the surviving vertices in ascending original id, then
     the split copies; the faces in their original order, remapped, winding unchanged; no face repeats an index, so the result feeds
     ``decimate``.  Inputs and outputs otherwise as ``remove_small_components``."""
@@ -260,7 +369,8 @@ def clean_mesh(verts, faces, v_pct=1, min_f=64, min_d=20, repair=True, remesh=Tr
 
 def decimate_mesh(verts, faces, target=5e4, backend="pymeshlab", remesh=False, optimalplacement=True):
     """decimate_mesh of utils/meshutils.py:63-115 (inference.py:129): ``decimate`` to int(target) faces.  backend="pyfqmr",
-    remesh=True and optimalplacement=False are not implemented and raise NotImplementedError."""
+    remesh=True and optimalplacement=False are not implemented and raise NotImplementedError (for remesh=True call ``remesh`` on the
+    result; binding it here is left to a later change)."""
     if backend != "pymeshlab":
         raise NotImplementedError(f"decimate_mesh: backend {backend!r} is not implemented (the quadric decimation of `decimate` stands in for pymeshlab)")
     if remesh:

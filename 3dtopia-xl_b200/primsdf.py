@@ -9,6 +9,8 @@ Mesh-based initialisation (``_init_param``) is training-time and absent, as in t
 """
 from __future__ import annotations
 
+import math
+
 import torch
 import torch.nn as nn
 
@@ -89,14 +91,18 @@ class PrimSDF(nn.Module):
         return grid
 
     def extract_mesh(self, resolution: int = 256, isovalue: float = 0.0, bound: float = 1.0, *, min_faces: int = 0, min_diameter: float = 0.0,
-                     target_faces: int | None = None, merge_distance: float = 0.0, repair: bool = False):
+                     target_faces: int | None = None, merge_distance: float = 0.0, repair: bool = False, remesh_pct: float | None = None,
+                     remesh_iters: int = 3):
         """Surface of the sdf field on the GPU: ``sdf_grid`` + marching cubes, in world coordinates (origin -bound, spacing
         2 bound / (R - 1)), i.e. inference.py:107-124 without the host copy.  Returns (verts fp32 [V,3], faces int64 [F,3]) on the
         module's device.  Then, in the order of inference.py:126-129 (clean_mesh, then decimate_mesh): when ``merge_distance`` > 0 or
         ``repair`` is set, the close-vertex merge (``merge_distance`` a fraction of the box diagonal, 0.01 for v_pct = 1; 0 merges
         nothing) with duplicate and zero-area faces removed; when ``min_faces`` > 0 or ``min_diameter`` > 0,
         ``mesh.remove_small_components`` with those thresholds; when ``repair`` is set, the non-manifold edge and vertex repair; when
-        ``target_faces`` is set, ``mesh.decimate`` to it (see its note on unreachable targets).
+        ``target_faces`` is set, ``mesh.decimate`` to it (see its note on unreachable targets); when ``remesh_pct`` is set,
+        ``mesh.remesh`` with ``remesh_iters`` iterations toward ``remesh_pct`` % of the box diagonal of the mesh at that point
+        (decimate_mesh(..., remesh=True), utils/meshutils.py:101-105: PercentageValue(1) is remesh_pct = 1).  As in inference.py:128-129,
+        where the remesh belongs to the decimation call, with ``target_faces`` set it runs only when the mesh had more faces than that.
         ``extract_mesh(256, min_faces=8, min_diameter=0.05, target_faces=100000, merge_distance=0.01, repair=True)`` is the geometry of
         extract_texmesh as this package reads clean_mesh (DESIGN.md §1 "clean-up contract"; remeshing is off there).  The defaults run
         marching cubes only.  The primitive noise filter of extract_texmesh (:90-103) is ``noise_filter_mask``; ``extract_texmesh``
@@ -117,8 +123,15 @@ class PrimSDF(nn.Module):
             v, f = mesh._remove_small(v, f, int(min_faces), float(min_diameter))
         if repair:
             v, f = mesh._repair(v, f)
+        if remesh_pct is not None and not (math.isfinite(remesh_pct) and remesh_pct > 0):
+            raise ValueError(f"remesh_pct must be finite and > 0, got {remesh_pct}")
+        decimated = target_faces is None or f.shape[0] > int(target_faces)
         if target_faces is not None:
             v, f = mesh._decimate(v, f, int(target_faces))
+        if remesh_pct is not None and decimated and f.shape[0]:
+            d = v.max(0).values.double() - v.min(0).values.double()
+            diag = float(torch.sqrt((d * d).sum()))
+            v, f = mesh.remesh(v, f, remesh_pct / 100.0 * diag, int(remesh_iters))
         return v, f
 
     def bake_texture(self, v, f, vt, ft, resolution=1024, pad: int = 32):
@@ -165,11 +178,12 @@ class PrimSDF(nn.Module):
         return unwrap.noise_filter(self.srt_param.detach())
 
     def extract_texmesh(self, resolution: int = 256, target_faces: int = 100000, atlas: int = 1024, island_padding: float = 0.02, min_faces: int = 8,
-                        min_diameter: float = 0.05, merge_distance: float = 0.0, repair: bool = False):
+                        min_diameter: float = 0.05, merge_distance: float = 0.0, repair: bool = False, remesh: bool = False):
         """The fast-unwrap branch of extract_texmesh (inference.py:90-222) on the device, without touching this module's parameters:
         the noise filter, ``extract_mesh(resolution, min_faces=, min_diameter=, target_faces=, merge_distance=, repair=)`` of the kept
         primitives (the reference's clean_mesh is ``extract_texmesh(256, 100000, 1024, 0.02, 8, 0.05, merge_distance=0.01,
-        repair=True)``; the defaults leave the close-vertex merge and the repair out), vertex normals,
+        repair=True)``; the defaults leave the close-vertex merge and the repair out; ``remesh=True`` is the "Remesh: Yes" of app.py, 3
+        iterations of ``mesh.remesh`` at 1 % of the diagonal after the decimation, run only when the decimation ran), vertex normals,
         the box-projection unwrap, the per-corner re-indexing of :144-148 and ``bake_texture`` at ``atlas`` x ``atlas``.  Returns a dict
         of device tensors in the layout :222 hands to Mesh: ``v`` fp32 [V,3] / ``f`` int64 [F,3] (the indexed mesh), ``vt`` fp32 [3F,2],
         ``ft`` int64 [F,3] (= arange), ``albedo`` and ``metallicRoughness`` fp32 [atlas, atlas, 3] (feats / 255).  The caller's
@@ -181,7 +195,7 @@ class PrimSDF(nn.Module):
         sub.feat_param.data = self.feat_param.detach()[keep].contiguous()
         sub.train(self.training)
         v, f = sub.extract_mesh(resolution, min_faces=min_faces, min_diameter=min_diameter, target_faces=target_faces, merge_distance=merge_distance,
-                                repair=repair)
+                                repair=repair, remesh_pct=1.0 if remesh else None)
         if f.shape[0] == 0:
             raise ValueError("the filtered field has no surface at this resolution")
         n = unwrap.compute_vertex_normal(v, f)

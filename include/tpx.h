@@ -333,6 +333,34 @@ int tpx_mesh_repair_count(const float* verts_dev, int64_t V, const int64_t* face
                           void* stream);
 int tpx_mesh_repair_emit(const float* verts_dev, int64_t V, int64_t F, const void* ws, size_t ws_bytes, float* verts_out_dev, int64_t* faces_out_dev,
                          void* stream);
+/* Isotropic remeshing: meshing_isotropic_explicit_remeshing(iterations, targetlen) as decimate_mesh(..., remesh=True) runs it after the
+ * decimation (utils/meshutils.py:101-105, inference.py:128-129; clean_mesh's remesh=True, utils/meshutils.py:179-183, is the same filter),
+ * as this package reads VCG's IsotropicRemeshing (DESIGN.md §1 "Isotropic remeshing contract").  The host drives the iterations:
+ * _begin once, then per iteration _split_count / _split_emit (the mesh grows) and _relax (in place), then a compaction.
+ * Creases are a sorted list of int64 edge keys (min << 32 | max), at most 3F of them.  Every call takes a workspace of
+ * tpx_remesh_workspace_bytes(V, F) for the mesh it reads (about 250 bytes per face); the grid over the input mesh
+ * (tpx_remesh_grid_bytes(F0), about 40 MB plus 150 bytes per face) lives from _begin to the last _relax, with the input vertices.
+ * _begin checks the input faces, writes the creases (cos_feature = cos(feature angle)) and builds the grid; counts_dev[0] = nC, -1 for
+ * malformed faces.  _split_count: counts_dev[0..2] = V', F', nC' (-1 for malformed faces); _split_emit (nC_out = nC') writes the split
+ * mesh and its creases from the same workspace.  Neither of the three synchronises.  _relax runs the collapse rounds, the flip rounds,
+ * the smoothing and the projection in place on verts_dev [V,3] and faces_dev (the live faces end up in its first F' rows) and writes
+ * counts_dev[0..2] = F', collapse rounds, flip rounds; it SYNCHRONISES once per round and at its end (malformed faces: TPX_ERR_ARG). */
+size_t tpx_remesh_workspace_bytes(int64_t V, int64_t F);
+size_t tpx_remesh_grid_bytes(int64_t F);
+int tpx_remesh_begin(const float* verts_dev, int64_t V, const int64_t* faces_dev, int64_t F, double cos_feature, void* grid, size_t grid_bytes, void* ws,
+                     size_t ws_bytes, int64_t* creases_out_dev, int64_t* counts_dev, void* stream);
+/* The projection on its own: for each of the n points pts_dev [n,3], the closest point of the input mesh of _begin (verts0_dev, F0 faces,
+ * its grid) into out_dev [n,3] and that face's id into face_out_dev [n] (smallest squared distance, then smallest face id; -1 and the
+ * point itself when the input has no face of non-zero area).  Does not synchronise. */
+int tpx_remesh_closest(const float* pts_dev, int64_t n, const float* verts0_dev, int64_t V0, int64_t F0, const void* grid, size_t grid_bytes,
+                       float* out_dev, int64_t* face_out_dev, void* stream);
+int tpx_remesh_split_count(const float* verts_dev, int64_t V, const int64_t* faces_dev, int64_t F, const int64_t* creases_dev, int64_t nC, double target_len,
+                           void* ws, size_t ws_bytes, int64_t* counts_dev, void* stream);
+int tpx_remesh_split_emit(const float* verts_dev, int64_t V, int64_t F, const int64_t* creases_dev, int64_t nC, int64_t nC_out, const void* ws, size_t ws_bytes,
+                          float* verts_out_dev, int64_t* faces_out_dev, int64_t* creases_out_dev, void* stream);
+int tpx_remesh_relax(float* verts_dev, int64_t V, int64_t* faces_dev, int64_t F, const int64_t* creases_dev, int64_t nC, const float* verts0_dev, int64_t V0,
+                     int64_t F0, const void* grid, size_t grid_bytes, double target_len, double cos_feature, void* ws, size_t ws_bytes, int64_t* counts_dev,
+                     void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Box-projection UV unwrap and the primitive noise filter — the fast-unwrap branch of extract_texmesh (inference.py:140-150:
