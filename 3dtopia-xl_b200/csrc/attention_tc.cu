@@ -15,8 +15,8 @@
 // The arithmetic is that of a serial loop (same tiles, exponent arguments, partial sums, fp16 P, rescale order): the output does
 // not depend on the schedule.
 //
-// Layouts: q, k  [B,H,N,80] fp16 (d >= 72 zero);  vT [B,H,80,NkPad] fp16 (V transposed: keys contiguous, NkPad % 8 == 0,
-// rows d >= 72 and key columns >= Nk finite/zero);  out [B,Nq,H*72] fp16.
+// Layouts: q, k  [B,H,N,80] fp16 (d >= Dh zero: S = Q K^T runs over all 80);  vT [B,H,80,NkPad] fp16 (V transposed: keys contiguous,
+// NkPad % 8 == 0, rows d >= Dh and key columns >= Nk finite);  out [B,Nq,H*Dh] fp16.
 #include "kernels.cuh"
 
 namespace tpx {

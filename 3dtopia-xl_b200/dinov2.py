@@ -1,6 +1,7 @@
-"""Host-side mirror of the reference's image encoder (SURVEY.md §8f-2), built from the DiT kernels.  EXPERIMENTAL: written after
-the round's GPU time was spent — parity-tested on CPU only through its oracle (oracle/dinov2.py, tests/golden/dinov2.npz); its
-GPU test is tests/test_gpu_zz_extra.py.  ``install()`` does not alias it.
+"""Host-side mirror of the reference's image encoder (SURVEY.md §8f-2), built from the DiT kernels.  Parity: its oracle
+(oracle/dinov2.py) is pinned to the reference's own output (tests/golden/dinov2.npz); on the GPU, tests/test_gpu_dinov2_stages.py
+checks every stage of every block against that oracle in fp64 (DESIGN.md §2) and tests/test_gpu_zz_extra.py the output against the
+fixture.  ``install()`` does not alias it.
 
 Drop-in for ``models.conditioner.image_dinov2.Dinov2Wrapper('dinov2_vitb14_reg', freeze=True)``
 (/root/reference/models/conditioner/image_dinov2.py:10-61): same state_dict keys (``model.cls_token`` ...), same
@@ -13,10 +14,12 @@ accumulation, like the DiT (10-bit-mantissa inputs, as TF32).  Launch plan per i
     12 x block        tpx_ln_modulate (LayerNorm affine as shift = beta, scale = gamma - 1) -> tpx_linear_heads (qkv, 12 heads x 64,
                       padded to 80, V transposed) -> tpx_attention_tc (wgmma) -> tpx_linear_gated (proj, LayerScale as the gate, fp32 residual)
                       -> tpx_ln_modulate -> tpx_linear (fc1) -> tpx_gelu_erf -> tpx_linear_gated (fc2, LayerScale)
-    final norm        tpx_ln_modulate, then class token + patch tokens are gathered (register tokens dropped)
+    final norm        tpx_ln_modulate with zero shift / scale (plain LN to fp16), then class token + patch tokens are gathered
+                      (register tokens dropped) and the LayerNorm affine applied in fp32
 """
 from __future__ import annotations
 
+import contextlib
 from collections import OrderedDict
 from typing import Optional
 
@@ -46,6 +49,18 @@ def _shapes() -> "OrderedDict[str, tuple]":
             s[b + nm] = shp
     s[m + "norm.weight"], s[m + "norm.bias"] = (DIM,), (DIM,)
     return s
+
+
+class _Stop(Exception):
+    """Raised by a tap at the requested stop of Dinov2Wrapper._forward."""
+
+
+@contextlib.contextmanager
+def _stopped():
+    try:
+        yield
+    except _Stop:
+        pass
 
 
 class Dinov2Wrapper(nn.Module):
@@ -91,23 +106,24 @@ class Dinov2Wrapper(nn.Module):
     def _operands(self, dev: torch.device):
         if self._dev_w is not None and self._dev == dev:
             return self._dev_w
-        sd = {k: v.detach().to(dev, torch.float32) for k, v in self.state_dict().items()}
+        # folded in fp64, so every fp16 / fp32 operand is one rounding of its exact value
+        sd = {k: v.detach().to(dev, torch.float64) for k, v in self.state_dict().items()}
         m = "model."
         w = {}
         # Normalize((x - mean) / std) folded into the patch embedding: conv(W, (p - mean)/std) + b = conv(W/std, p) + (b - sum W*mean/std);
         # the patch vector is laid out (i, j, c) — the order of a [14,14,3] window of the NHWC picture — and zero padded to KPAD
         W = sd[m + "patch_embed.proj.weight"]
-        std = torch.tensor(STD, device=dev).view(1, 3, 1, 1)
-        mean = torch.tensor(MEAN, device=dev).view(1, 3, 1, 1)
+        std = torch.tensor(STD, dtype=torch.float64, device=dev).view(1, 3, 1, 1)
+        mean = torch.tensor(MEAN, dtype=torch.float64, device=dev).view(1, 3, 1, 1)
         Wn = W / std
-        wp = torch.zeros(DIM, KPAD, device=dev)
+        wp = torch.zeros(DIM, KPAD, dtype=torch.float64, device=dev)
         wp[:, :KPATCH] = Wn.permute(0, 2, 3, 1).reshape(DIM, KPATCH)
         w["patch_w"] = wp.half().contiguous()
         w["patch_b"] = (sd[m + "patch_embed.proj.bias"] - (Wn * mean).sum(dim=(1, 2, 3))).half().contiguous()
         pos = sd[m + "pos_embed"][0]
-        w["row0"] = (sd[m + "cls_token"][0, 0] + pos[0]).contiguous()                 # class token + its position, fp32
-        w["regs"] = sd[m + "register_tokens"][0].contiguous()                          # registers carry no position (vision_transformer.py:222-231)
-        w["pos_patches"] = pos[1:].contiguous()
+        w["row0"] = (sd[m + "cls_token"][0, 0] + pos[0]).float().contiguous()                 # class token + its position, fp32
+        w["regs"] = sd[m + "register_tokens"][0].float().contiguous()                          # registers carry no position (vision_transformer.py:222-231)
+        w["pos_patches"] = pos[1:].float().contiguous()
         w["ones"] = torch.ones(1, DIM, device=dev, dtype=torch.float16)
         for i in range(DEPTH):
             b = f"{m}blocks.{i}."
@@ -118,8 +134,11 @@ class Dinov2Wrapper(nn.Module):
                 w[f"{i}.ln{n}.scale"] = (sd[b + f"norm{n}.weight"] - 1.0).half().view(1, DIM).contiguous()     # LN * h(1 + scale) + shift
                 w[f"{i}.ln{n}.shift"] = sd[b + f"norm{n}.bias"].half().view(1, DIM).contiguous()
                 w[f"{i}.ls{n}"] = sd[b + f"ls{n}.gamma"].half().view(1, DIM).contiguous()
-        w["norm.scale"] = (sd[m + "norm.weight"] - 1.0).half().view(1, DIM).contiguous()
-        w["norm.shift"] = sd[m + "norm.bias"].half().view(1, DIM).contiguous()
+        # final norm: plain LN to fp16 (zero shift and scale), then the affine in fp32 on the host side, so that a gain far below 1 keeps
+        # its relative precision (as modulation h(1 + h(g - 1)) its absolute error of ~2^-12 would be a large fraction of such a gain)
+        w["zeros"] = torch.zeros(1, DIM, device=dev, dtype=torch.float16)
+        w["norm.weight"] = sd[m + "norm.weight"].float().contiguous()
+        w["norm.bias"] = sd[m + "norm.bias"].float().contiguous()
         self._dev_w, self._dev = w, dev
         return w
 
@@ -127,6 +146,14 @@ class Dinov2Wrapper(nn.Module):
     def forward(self, image: torch.Tensor, mod: torch.Tensor = None) -> torch.Tensor:
         assert image.shape[-1] == 3, "image: [N, H, W, C] (image_dinov2.py:46-47)"
         assert mod is None, "Unexpected modulation input in dinov2 forward."
+        return self._forward(image)
+
+    def _forward(self, image: torch.Tensor, taps: Optional[dict] = None, stop: Optional[tuple] = None) -> Optional[torch.Tensor]:
+        """The launch plan.  taps (parity tests): a dict that receives clones of the buffers as the launches leave them — "embed" (the
+        fp32 token block after the patch embedding), per block i (i, "ln1"), (i, "q"), (i, "k"), (i, "vT"), (i, "att"), (i, "res1")
+        (residual after proj), (i, "ln2"), (i, "fc1"), (i, "hid") (after the GELU), (i, "res2") (residual after fc2), then "out16" (the
+        normalised tokens before the affine).  stop = one of those keys ends the run after that tap and returns None.  Without taps
+        the launches are the same."""
         if not image.is_cuda:
             raise _lib.TpxError("Dinov2Wrapper runs on CUDA only (no CPU path): move the module and the image to the GPU")
         if image.shape[1] != image.shape[2]:
@@ -154,29 +181,51 @@ class Dinov2Wrapper(nn.Module):
         att = torch.empty(rows, DIM, dtype=torch.float16, device=dev)
         hid = torch.empty(rows, 4 * DIM, dtype=torch.float16, device=dev)
         out16 = torch.empty(rows, DIM, dtype=torch.float16, device=dev)
-        with torch.cuda.device(dev):
+
+        def tap(key, buf):
+            if taps is not None:
+                taps[key] = buf.clone()
+            if key == stop:
+                raise _Stop
+
+        with torch.cuda.device(dev), _stopped():
             st = _lib.stream_ptr()
             for b in range(n):                      # patch tokens of picture b: rows 5.. of its token block, added onto the position embedding
                 _lib.check(lib.tpx_linear_gated(patches[b * np_:].data_ptr(), KPAD, w["patch_w"].data_ptr(), w["patch_b"].data_ptr(),
                                                 w["ones"].data_ptr(), DIM, 1, np_, tok[b, 1 + N_REG:].data_ptr(), DIM, np_, DIM, KPAD, 0, st),
                            "patch embedding")
             xr = tok.view(rows, DIM)
+            tap("embed", tok)
             for i in range(DEPTH):
                 _lib.check(lib.tpx_ln_modulate(xr.data_ptr(), rows, DIM, 1e-6, w[f"{i}.ln1.shift"].data_ptr(), w[f"{i}.ln1.scale"].data_ptr(), DIM, rows, 1,
                                                ln.data_ptr(), None, None, 0, st), "norm1")
+                tap((i, "ln1"), ln)
                 _lib.check(lib.tpx_linear_heads(ln.data_ptr(), DIM, w[f"{i}.attn.qkv.weight"].data_ptr(), w[f"{i}.attn.qkv.bias"].data_ptr(), q.data_ptr(),
                                                 k.data_ptr(), vT.data_ptr(), rows, 3 * DIM, DIM, DIM, HEADS, DH, DHP, nt, 1.0, 0, 2, ntp, st), "qkv")
+                tap((i, "q"), q)
+                tap((i, "k"), k)
+                tap((i, "vT"), vT)
                 _lib.check(lib.tpx_attention_tc(q.data_ptr(), k.data_ptr(), vT.data_ptr(), att.data_ptr(), n, HEADS, nt, nt, ntp, DH, DH ** -0.5, st), "attention")
+                tap((i, "att"), att)
                 _lib.check(lib.tpx_linear_gated(att.data_ptr(), DIM, w[f"{i}.attn.proj.weight"].data_ptr(), w[f"{i}.attn.proj.bias"].data_ptr(),
                                                 w[f"{i}.ls1"].data_ptr(), DIM, 1, rows, xr.data_ptr(), DIM, rows, DIM, DIM, 0, st), "proj")
+                tap((i, "res1"), tok)
                 _lib.check(lib.tpx_ln_modulate(xr.data_ptr(), rows, DIM, 1e-6, w[f"{i}.ln2.shift"].data_ptr(), w[f"{i}.ln2.scale"].data_ptr(), DIM, rows, 1,
                                                ln.data_ptr(), None, None, 0, st), "norm2")
+                tap((i, "ln2"), ln)
                 _lib.check(lib.tpx_linear(ln.data_ptr(), DIM, w[f"{i}.mlp.fc1.weight"].data_ptr(), w[f"{i}.mlp.fc1.bias"].data_ptr(), hid.data_ptr(), 4 * DIM,
                                           rows, 4 * DIM, DIM, 0, 1.0, 0, st), "fc1")
+                tap((i, "fc1"), hid)
                 _lib.check(lib.tpx_gelu_erf(hid.data_ptr(), rows * 4 * DIM, st), "gelu")
+                tap((i, "hid"), hid)
                 _lib.check(lib.tpx_linear_gated(hid.data_ptr(), 4 * DIM, w[f"{i}.mlp.fc2.weight"].data_ptr(), w[f"{i}.mlp.fc2.bias"].data_ptr(),
                                                 w[f"{i}.ls2"].data_ptr(), DIM, 1, rows, xr.data_ptr(), DIM, rows, DIM, 4 * DIM, 0, st), "fc2")
-            _lib.check(lib.tpx_ln_modulate(xr.data_ptr(), rows, DIM, 1e-6, w["norm.shift"].data_ptr(), w["norm.scale"].data_ptr(), DIM, rows, 1,
+                tap((i, "res2"), tok)
+            _lib.check(lib.tpx_ln_modulate(xr.data_ptr(), rows, DIM, 1e-6, w["zeros"].data_ptr(), w["zeros"].data_ptr(), DIM, rows, 1,
                                            out16.data_ptr(), None, None, 0, st), "final norm")
+            tap("out16", out16)
+        if stop is not None:
+            return None
         o = out16.view(n, nt, DIM)
-        return torch.cat([o[:, :1], o[:, 1 + N_REG:]], dim=1).float()        # [N, 1370, 768], class token first (image_dinov2.py:56-60)
+        o = torch.cat([o[:, :1], o[:, 1 + N_REG:]], dim=1).float()          # [N, 1370, 768], class token first (image_dinov2.py:56-60)
+        return o * w["norm.weight"] + w["norm.bias"]                         # the final norm's affine in fp32

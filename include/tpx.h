@@ -203,7 +203,8 @@ int tpx_ln_modulate(float* x, int rows, int D, float eps, const void* shift_f16,
 /* memory_efficient_attention contract (attention.py:54,109): q [B,H,Nq,DhP], k/v [B,H,Nk,DhP] -> out [B,Nq,H*Dh] */
 int tpx_attention(const void* q, const void* k, const void* v, void* out, int B, int H, int Nq, int Nk, int Dh, int DhP, float scale, void* stream);
 /* Same contract on the wgmma path (Dh == 72, the released model's head size, or 64): q,k [B,H,N,80]; vT = V transposed
- * [B,H,80,NkPad], NkPad % 8 == 0, padding rows/columns finite. */
+ * [B,H,80,NkPad], NkPad % 8 == 0.  q / k columns d >= Dh must be zero (q k^T runs over all 80); vT rows d >= Dh and key columns
+ * >= Nk only have to be finite. */
 int tpx_attention_tc(const void* q, const void* k, const void* vT, void* out, int B, int H, int Nq, int Nk, int NkPad, int Dh, float scale, void* stream);
 /* out = h(uncond + h(s * h(cond - uncond)))  over [cond; uncond] halves of n_half elements (dit_crossattn.py:210-213) */
 int tpx_cfg_combine(const void* both_f16, int64_t n_half, float s, void* out_f16, void* stream);
@@ -425,7 +426,8 @@ int tpx_primsdf_bake(const float* rast_dev, int H, int W, const float* v_dev, in
 size_t tpx_texture_inpaint_bytes(int H, int W);
 int tpx_texture_inpaint(float* feats_dev, const uint8_t* mask_dev, int H, int W, int C, int pad, void* ws, size_t ws_bytes, int32_t* src_dev, void* stream);
 
-/* nn.GELU() (erf form) in place on an fp16 tensor of n elements (n % 8 == 0, 16-B aligned) — the activation of the DINOv2 MLP
+/* nn.GELU() (erf form) in place on an fp16 tensor of n elements (n % 8 == 0, 16-B aligned), within one fp16 ulp of the exact GELU
+ * of every finite input — the activation of the DINOv2 MLP
  * (models/conditioner/dinov2/layers/mlp.py:33-39); the rest of that encoder (SURVEY.md §8f-2) is built from the entry points above. */
 int tpx_gelu_erf(void* x_f16, int64_t n, void* stream);
 

@@ -7,28 +7,14 @@ import importlib
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 import oracle
 import tpxl_b200  # noqa: F401
+from oracle import dinov2 as odn
+from oracle.dit import Policy, r16
 
 d = importlib.import_module("tpxl_b200.dinov2")
-
-
-def _h(t):
-    return t.half().float()
-
-
-def _linear(A, W, b):                       # tpx_linear: fp16 operands, fp32 accumulate, one rounding of acc + bias
-    return _h(A.float() @ W.float().t() + b.float())
-
-
-def _gated(A, W, b, gate, xres):            # tpx_linear_gated: xres(fp32) += h(gate * h(A W^T + b))
-    xres += _h(gate.float() * _linear(A, W, b))
-
-
-def _lnmod(x, shift, scale):                # tpx_ln_modulate: h(LN(x) * h(1 + scale) + shift)
-    return _h(F.layer_norm(x, (x.shape[-1],), eps=1e-6) * _h(1 + scale.float()) + shift.float())
+POLICY = Policy("fp16")      # the launch plan's rounding points (oracle/dinov2.py); on fp32 tensors an fp32 emulation of them
 
 
 def test_state_dict_contract_and_errors():
@@ -48,10 +34,13 @@ def test_state_dict_contract_and_errors():
         m(torch.zeros(1, 518, 518, 3))
 
 
-def test_launch_plan_algebra_matches_oracle():
+def test_launch_plan_matches_policy_oracle():
+    """The wrapper's operands against the policy's definition (Normalize folded into the patch weights, (i, j, c) patch layout, token
+    assembly, LayerNorm affine as modulation, LayerScale as the gate, the final norm's affine kept for the host), then the whole policy
+    pipeline against the fp32 oracle."""
     torch.set_grad_enabled(False)
     try:
-        sd = oracle.dinov2.synth_weights(105)
+        sd = odn.synth_weights(105)
         m = d.Dinov2Wrapper()
         m.load_state_dict(sd)
         w = m._operands(torch.device("cpu"))
@@ -62,20 +51,37 @@ def test_launch_plan_algebra_matches_oracle():
         patches[:, :d.KPATCH] = (img / 255.0).reshape(n, g, 14, g, 14, 3).permute(0, 1, 3, 2, 4, 5).reshape(n * np_, d.KPATCH).half()
         tok = torch.empty(n, nt, 768)
         tok[:, 0], tok[:, 1:5], tok[:, 5:] = w["row0"], w["regs"], w["pos_patches"]
-        _gated(patches, w["patch_w"], w["patch_b"], w["ones"], tok[0, 5:])
-        xr = tok.view(-1, 768)
+        tok[0, 5:] += r16(patches.float() @ w["patch_w"].float().t() + w["patch_b"].float())      # tpx_linear_gated, gate 1
+        pe = odn.patch_embed(sd, img, POLICY)
+        assert float((tok - pe).norm() / pe.norm()) < 1e-4          # accumulation order only: an fp16 rounding flip here and there
         for i in range(d.DEPTH):
-            ln = _lnmod(xr, w[f"{i}.ln1.shift"], w[f"{i}.ln1.scale"])
-            qkv = _linear(ln, w[f"{i}.attn.qkv.weight"], w[f"{i}.attn.qkv.bias"]).reshape(n, nt, 3, 12, 64).permute(2, 0, 3, 1, 4)
-            a = _h(F.scaled_dot_product_attention(qkv[0], qkv[1], qkv[2])).transpose(1, 2).reshape(n * nt, 768)
-            _gated(a, w[f"{i}.attn.proj.weight"], w[f"{i}.attn.proj.bias"], w[f"{i}.ls1"], xr)
-            ln = _lnmod(xr, w[f"{i}.ln2.shift"], w[f"{i}.ln2.scale"])
-            hid = _h(F.gelu(_linear(ln, w[f"{i}.mlp.fc1.weight"], w[f"{i}.mlp.fc1.bias"])))
-            _gated(hid, w[f"{i}.mlp.fc2.weight"], w[f"{i}.mlp.fc2.bias"], w[f"{i}.ls2"], xr)
-        o = _lnmod(xr, w["norm.shift"], w["norm.scale"]).view(n, nt, 768)
+            b = f"model.blocks.{i}."
+            for nn_ in ("1", "2"):
+                assert torch.equal(w[f"{i}.ln{nn_}.scale"].float(), r16(sd[b + f"norm{nn_}.weight"] - 1).view(1, -1))
+                assert torch.equal(w[f"{i}.ln{nn_}.shift"].float(), r16(sd[b + f"norm{nn_}.bias"]).view(1, -1))
+                assert torch.equal(w[f"{i}.ls{nn_}"].float(), r16(sd[b + f"ls{nn_}.gamma"]).view(1, -1))
+        assert not w["zeros"].any()
+        assert torch.equal(w["norm.weight"], sd["model.norm.weight"]) and torch.equal(w["norm.bias"], sd["model.norm.bias"])
+        x = tok
+        for i in range(d.DEPTH):
+            x = odn.block(sd, i, x, POLICY)
+        o = odn.final_norm(sd, x, POLICY)
         out = torch.cat([o[:, :1], o[:, 5:]], 1)
-        ref = oracle.dinov2.forward(sd, img)
+        ref = odn.forward(sd, img)
         rel = float((out - ref).norm() / ref.norm())
         assert rel < 3e-3, rel                                   # fp16-input contract against the fp32 oracle: ~1e-3
+        worst = float(((out - ref).norm(dim=(0, 1)) / ref.norm(dim=(0, 1))).max())
+        assert worst < 4e-3, worst                               # per channel (the final norm's affine in fp32: ~2e-3)
     finally:
         torch.set_grad_enabled(True)
+
+
+def test_oracle_runs_in_the_image_dtype():
+    """fp64 weights and an fp64 image run the exact encoder in fp64 (depth 1 to keep it short); the fp32 path is unchanged by it."""
+    sd = odn.synth_weights(5, depth=1)
+    img = torch.from_numpy(np.random.RandomState(3).uniform(0, 255, size=(1, 518, 518, 3)))
+    with torch.no_grad():
+        o64 = odn.forward({k: v.double() for k, v in sd.items()}, img, depth=1)
+        o32 = odn.forward(sd, img.float(), depth=1)
+    assert o64.dtype == torch.float64 and o32.dtype == torch.float32
+    assert float((o32.double() - o64).norm() / o64.norm()) < 1e-5

@@ -66,14 +66,16 @@ def test_dinov2_encoder_against_reference_fixture(golden_dir):
         out = m(torch.from_numpy(img).cuda())
         small = np.ascontiguousarray(np.clip(img[:, ::2, ::2][:, :224, :224], 0, 255))
         out_small = m(torch.from_numpy(small).cuda())
-        two = m(torch.from_numpy(np.concatenate([img, img[:, ::-1].copy()], 0)).cuda())        # batch of 2: per-picture token blocks
+        flipped = img[:, ::-1].copy()
+        two = m(torch.from_numpy(np.concatenate([img, flipped], 0)).cuda())                     # batch of 2: per-picture token blocks
+        out_flipped = m(torch.from_numpy(flipped).cuda())
     torch.cuda.synchronize()
     assert out.shape == (1, 1370, 768) and out.dtype == torch.float32
     r = dict(full=rel_l2(out[:, ::6], torch.from_numpy(g["out"]).cuda()), small=rel_l2(out_small[:, ::24], torch.from_numpy(g["out_small"]).cuda()),
-             batch=rel_l2(two[0:1], out))
+             batch0=rel_l2(two[0:1], out), batch1=rel_l2(two[1:2], out_flipped))
     print(r)
     assert r["full"] < 5e-3 and r["small"] < 5e-3
-    assert r["batch"] < 1e-4                                   # the same picture gives the same tokens whatever shares the batch
+    assert r["batch0"] < 1e-4 and r["batch1"] < 1e-4           # each picture gives the same tokens whatever shares the batch
                                                                # (tile widths depend on the row count, so not necessarily bit-identical)
 
 
