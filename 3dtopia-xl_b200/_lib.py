@@ -63,6 +63,13 @@ SIGNATURES = {
     "tpx_vae_workspace_bytes": (_sz, [_vp, _i]),
     "tpx_vae_decode": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _sz, _vp]),
     "tpx_vae_debug_stage": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "tpx_vae_encoder_create": (_i, [C.POINTER(VaeConfig), C.POINTER(_vp)]),
+    "tpx_vae_encoder_destroy": (None, [_vp]),
+    "tpx_vae_encoder_set_weight": (_i, [_vp, C.c_char_p, _vp, _i, C.POINTER(_i64), _i, _vp]),
+    "tpx_vae_encoder_finalize": (_i, [_vp, _vp]),
+    "tpx_vae_encoder_workspace_bytes": (_sz, [_vp, _i]),
+    "tpx_vae_encode": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _sz, _vp]),
+    "tpx_vae_encode_debug_stage": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "tpx_linear": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp]),
     "tpx_linear_gated": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _vp]),
     "tpx_linear_heads": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _vp]),

@@ -205,7 +205,8 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const CUtens
 int launch_gemm(const GemmProblem& p, cudaStream_t stream) {
     TPX_CHECK(p.M > 0 && p.N > 0 && p.K > 0, TPX_ERR_SHAPE, "gemm: empty problem %d x %d x %d", p.M, p.N, p.K);
     TPX_CHECK(p.N % 8 == 0 && p.K % 8 == 0, TPX_ERR_SHAPE, "gemm: N (%d) and K (%d) must be multiples of 8", p.N, p.K);
-    const int bk = (p.a_mode == AMODE_CONV3 && p.conv_C == 32) ? 32 : 64;
+    // 32-channel operands (conv input or a linear K of 32, the encoder's 1x1 shortcut) load 64-B rows; everything else 128-B rows
+    const int bk = (p.a_mode == AMODE_CONV3 ? p.conv_C == 32 : p.K == 32) ? 32 : 64;
     ProfScope prof(p.a_mode == AMODE_CONV3 ? PROF_CONV_GEMM : PROF_GEMM, stream);
     GemmArgs a = p.args;
     a.M = p.M;
@@ -258,6 +259,10 @@ int launch_gemm(const GemmProblem& p, cudaStream_t stream) {
     TPX_CASE(32, 32, AMODE_CONV3, EPI_STORE)
     TPX_CASE(32, 32, AMODE_CONV3, EPI_RESID_SCALE)
     TPX_CASE(16, 32, AMODE_CONV3, EPI_NCDHW)
+    // VAE encoder: conv1 of the 32 -> 256 block at 4^3 and its K = 32 shortcut; conv_out (2 of 16 rows) + quant_conv
+    TPX_CASE(256, 32, AMODE_CONV3, EPI_STORE)
+    TPX_CASE(256, 32, AMODE_LINEAR, EPI_STORE)
+    TPX_CASE(16, 64, AMODE_CONV3, EPI_MOMENTS)
 #undef TPX_CASE
     set_error("gemm: no kernel instantiated for BN=%d BK=%d amode=%d epi=%d", p.BN, bk, p.a_mode, p.epi);
     return TPX_ERR_SHAPE;

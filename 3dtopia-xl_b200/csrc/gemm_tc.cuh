@@ -31,6 +31,8 @@ enum GemmEpiMode : int {
     EPI_GATED = 3,       // xres[row*ldx+col] += float( h( gate[b,col] * h(acc+bias) ) )
     EPI_RESID_SCALE = 4, // out0 = h( (acc + bias + resid[row*ldo+col]) * alpha )
     EPI_NCDHW = 6,       // out[(p*Cout+co)*S3 + vox] = acc + bias   (fp32 or fp16 out, co < n_valid)
+    EPI_MOMENTS = 7,     // VAE encoder tail: h = h(acc + bias) on columns 0, 1 (conv_out), then the 1x1 quant_conv 2 -> 2 on h:
+                         // out[(p*2+c)*S3 + vox] = h(quant[2c] h0 + quant[2c+1] h1 + quant[4+c])   (fp32 or fp16 out)
 };
 enum GemmAMode : int { AMODE_LINEAR = 0, AMODE_CONV3 = 1 };
 
@@ -57,6 +59,7 @@ struct GemmArgs {
     int convt_store;  // EPI_STORE: 1 = rows are (primitive, 4^3 voxel) and the output map is the 5-D stride-2 lattice of one (a,b,c) offset of
                       // a ConvTranspose3d(k2,s2): a warp's 32 rows are one [2 z][4 y][4 x] box (vae3d_dib.py:220-226)
     int heads_tma;    // EPI_HEADS: 1 = outputs leave as 24-column bulk tensor stores (launcher checked the geometry, padding is pre-zeroed)
+    const __half* quant;   // EPI_MOMENTS: quant_conv as [w00, w01, w10, w11, b0, b1] (vae3d_dib.py:428)
 };
 
 constexpr bool gemm_pingpong(int bn, int amode) { return amode == AMODE_LINEAR && (bn == 128 || bn == 144); }
@@ -247,6 +250,20 @@ __device__ __forceinline__ void epi_chunk(const GemmArgs& g, const float* __rest
                 const size_t off = (static_cast<size_t>(p) * g.n_valid + co) * g.S3 + vox;
                 if (g.out32 != nullptr) g.out32[off] = v[i];
                 else g.out0[off] = __float2half_rn(v[i]);
+            }
+        }
+    } else if constexpr (EPI == EPI_MOMENTS) {
+        // conv_out's two channels at their fp16 rounding point (autocast), then quant_conv on those rounded values (not folded into
+        // conv_out's weights: the reference rounds in between); channel 0 = mean, 1 = logvar (vae3d_dib.py:52-53)
+        if (row_ok && col0 == 0) {
+            const int p = row / g.S3, vox = row - p * g.S3;
+            const float h0 = h2f_round(v[0]), h1 = h2f_round(v[1]);
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const float m = h2f_round(fmaf(__half2float(g.quant[2 * c + 1]), h1, fmaf(__half2float(g.quant[2 * c]), h0, __half2float(g.quant[4 + c]))));
+                const size_t off = (static_cast<size_t>(p) * 2 + c) * g.S3 + vox;
+                if (g.out32 != nullptr) g.out32[off] = m;
+                else g.out0[off] = __float2half_rn(m);
             }
         }
     }

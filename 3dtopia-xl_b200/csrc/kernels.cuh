@@ -43,5 +43,8 @@ int launch_groupnorm_silu(const __half* x, const __half* gamma, const __half* be
                           __half* out, cudaStream_t st);
 int launch_pack_conv3(const void* src, int dtype, __half* dst, int Cout, int Cin, int transposed, cudaStream_t st);
 int launch_pack_convt2(const void* src, int dtype, __half* dst, int Cin, int Cout, cudaStream_t st);
+int launch_vae_enc_conv_in(const void* x, int x_dtype, const __half* W, const __half* bias, int P, __half* out, cudaStream_t st);
+int launch_space_to_depth2(const __half* in, __half* out, int P, int C, cudaStream_t st);
+int launch_pack_conv3_s2d(const void* src, int dtype, __half* dst, int Cout, int Cin, cudaStream_t st);
 
 }  // namespace tpx

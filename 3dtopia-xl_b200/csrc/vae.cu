@@ -1,6 +1,7 @@
-// VAE decoder handle: repacked fp16 parameters keyed by the reference's state_dict names and the decode schedule.
+// VAE decoder and encoder handles: repacked fp16 parameters keyed by the reference's state_dict names, and the decode / encode schedules.
 //   reference: models/vae3d_dib.py:437-440 (VAE.decode), :369-387 (Decoder.forward), :220-226 (MidBlock),
-//              :259-267 (UpBlock), :128-145 (ResnetBlock), :34-48 (VolumeAttention)
+//              :259-267 (UpBlock), :128-145 (ResnetBlock), :34-48 (VolumeAttention);
+//              :431-435 (VAE.encode), :310-327 (Encoder.forward), :178-184 (DownBlock), :428 (quant_conv)
 // Activations are channels-last fp16 [P, S^3, C]; every primitive is independent (GroupNorm statistics are
 // per primitive), so the whole decoder is a batch of P tiny volumes.
 #include <cmath>
@@ -26,6 +27,25 @@ struct tpx_vae {
     __half *ang, *anb, *Wqkv, *Wap, *bap;    // mid attention
     __half *Wup, *bup;                       // [8*C0, C0], [8*C0]
     __half *nog, *nob, *Wout, *bout;         // norm_out, conv_out (padded to 16 rows)
+    std::vector<std::string> required;
+    std::vector<uint8_t> seen;
+    bool finalized = false;
+};
+
+
+// Encoder of the released layout (down_channels [32, 256], in_channels 6, latent 1): conv_in 6 -> 32 at 8^3, two 32-channel
+// ResnetBlocks, the stride-2 downsample to 4^3, a 32 -> 256 block with its 1x1 shortcut, a 256 block, the mid block (res, attention,
+// res), norm_out + SiLU and conv_out 256 -> 2 with quant_conv in its epilogue.
+struct tpx_vae_encoder {
+    int Cin = 6, C0 = 32, C1 = 256, heads = 8;
+    __half* store = nullptr;
+    size_t store_halves = 0;
+    __half *Win, *bin;                       // conv_in [32, 6*27] (the reference's own layout), bias
+    VaeRes res[6];                           // down0.0, down0.1 (32, 8^3), down1.0 (32 -> 256), down1.1, mid0, mid1 (256, 4^3)
+    __half *Wds, *bds;                       // downsample, repacked for the space-to-depth input: [32, 27*256]
+    __half *ang, *anb, *Wqkv, *Wap, *bap;    // mid attention
+    __half *nog, *nob, *Wout, *bout;         // norm_out, conv_out (padded to 16 rows)
+    __half* quant;                           // quant_conv [w00, w01, w10, w11, b0, b1]
     std::vector<std::string> required;
     std::vector<uint8_t> seen;
     bool finalized = false;
@@ -151,6 +171,52 @@ int conv3(const __half* x, const __half* W, const __half* bias, const __half* re
     return launch_gemm(p, st);
 }
 
+// ---- blocks both schedules run (weights come as structs, scratch as pointers: no handle) ------------------------------------
+struct VaeAttn {
+    __half *ng, *nb, *Wqkv, *Wproj, *bproj;
+    int heads;
+};
+struct BlockScratch {
+    __half *T1, *T2, *Q, *K, *V;   // [P, S^3, C] each
+};
+constexpr float kSkip = 0.70710678118654752f;   // sqrtf(0.5f): skip_scale (vae3d_dib.py:338, :395)
+constexpr float kEps = 1e-5f;
+
+// ResnetBlock C -> C at S^3 (vae3d_dib.py:128-145): GN+SiLU -> conv1 -> GN+SiLU -> conv2 + x, * skip.  X2 receives the result and the two
+// pointers are swapped, so X is the block's output on return.  4 launches.
+int resnet_block(const VaeRes& r, int S, __half*& X, __half*& X2, const BlockScratch& sc, int P, cudaStream_t st) {
+    const int S3 = S * S * S, C = r.cin;
+    int rc;
+    if ((rc = launch_groupnorm_silu(X, r.n1g, r.n1b, P, S3, C, 32, kEps, 1, sc.T1, st)) != TPX_OK) return rc;
+    if ((rc = conv3(sc.T1, r.W1, r.b1, nullptr, 1.f, sc.T2, nullptr, 0, P, S, C, C, EPI_STORE, st)) != TPX_OK) return rc;
+    if ((rc = launch_groupnorm_silu(sc.T2, r.n2g, r.n2b, P, S3, C, 32, kEps, 1, sc.T1, st)) != TPX_OK) return rc;
+    if ((rc = conv3(sc.T1, r.W2, r.b2, X, kSkip, X2, nullptr, 0, P, S, C, C, EPI_RESID_SCALE, st)) != TPX_OK) return rc;
+    std::swap(X, X2);
+    return TPX_OK;
+}
+
+// VolumeAttention at 4^3 (vae3d_dib.py:34-48): GN -> qkv -> 64-token attention per primitive -> proj, (x + res) * skip.  Result in X
+// (swapped as above).  4 launches.
+int attention_block(const VaeAttn& at, __half*& X, __half*& X2, const BlockScratch& sc, int P, int C, cudaStream_t st) {
+    int rc;
+    if ((rc = launch_groupnorm_silu(X, at.ng, at.nb, P, 64, C, 32, kEps, 0, sc.T1, st)) != TPX_OK) return rc;
+    GemmProblem p{};
+    p.A = sc.T1; p.a_mode = AMODE_LINEAR; p.lda = C; p.W = at.Wqkv; p.M = P * 64; p.N = 3 * C; p.K = C; p.BN = 256; p.epi = EPI_HEADS;
+    GemmArgs a{};
+    a.post_scale = 1.0f; a.out0 = sc.Q; a.out1 = sc.K; a.out2 = sc.V; a.split_cols = C; a.Dh = 32; a.DhP = 32; a.H = at.heads; a.Nseq = 64;
+    p.args = a;
+    if ((rc = launch_gemm(p, st)) != TPX_OK) return rc;
+    if ((rc = launch_attention(sc.Q, sc.K, sc.V, sc.T2, P, at.heads, 64, 64, 32, 32, 1.0f / sqrtf(32.f), st)) != TPX_OK) return rc;
+    GemmProblem q{};
+    q.A = sc.T2; q.a_mode = AMODE_LINEAR; q.lda = C; q.W = at.Wproj; q.M = P * 64; q.N = C; q.K = C; q.BN = 256; q.epi = EPI_RESID_SCALE;
+    GemmArgs b{};
+    b.bias = at.bproj; b.post_scale = 1.0f; b.out0 = X2; b.ldo = C; b.resid = X; b.alpha = kSkip;
+    q.args = b;
+    if ((rc = launch_gemm(q, st)) != TPX_OK) return rc;
+    std::swap(X, X2);
+    return TPX_OK;
+}
+
 int check_run_args(const tpx_vae* h, const void* z, const void* dst, int P, const void* ws, size_t ws_bytes, const char* what) {
     TPX_CHECK(h != nullptr && z != nullptr && dst != nullptr && ws != nullptr, TPX_ERR_ARG, "%s: null argument", what);
     TPX_CHECK(h->finalized, TPX_ERR_STATE, "%s: weights not finalized (load_state_dict first)", what);
@@ -165,8 +231,8 @@ int check_run_args(const tpx_vae* h, const void* z, const void* dst, int P, cons
 int vae_run(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, int P, int stop, void* tap, void* ws, cudaStream_t st) {
     VaeWs w = carve_vws(h, P, static_cast<uint8_t*>(ws));
     const int C0 = h->C0, C1 = h->C1;
-    const float skip = sqrtf(0.5f);
-    const float eps = 1e-5f;
+    const float skip = kSkip;
+    const float eps = kEps;
     int rc;
 #define TPX_RC(call) do { rc = (call); if (rc != TPX_OK) return rc; } while (0)
 #define TPX_TAP(stage, act, S3, C)                                                                                                   \
@@ -178,41 +244,17 @@ int vae_run(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, in
     } while (0)
     TPX_RC(launch_vae_conv_in(z, z_dtype, h->w_pq, h->b_pq, h->Win, h->bin, P, C0, w.X, st));
     __half *X = w.X, *X2 = w.X2;
+    const BlockScratch sc{w.T1, w.T2, w.Q, w.K, w.V};
     TPX_TAP(TPX_VAE_STAGE_CONV_IN, X, 64, C0);
-    auto res4 = [&](const VaeRes& r) -> int {   // ResnetBlock C0->C0 at 4^3
-        int rc2;
-        if ((rc2 = launch_groupnorm_silu(X, r.n1g, r.n1b, P, 64, C0, 32, eps, 1, w.T1, st)) != TPX_OK) return rc2;
-        if ((rc2 = conv3(w.T1, r.W1, r.b1, nullptr, 1.f, w.T2, nullptr, 0, P, 4, C0, C0, EPI_STORE, st)) != TPX_OK) return rc2;
-        if ((rc2 = launch_groupnorm_silu(w.T2, r.n2g, r.n2b, P, 64, C0, 32, eps, 1, w.T1, st)) != TPX_OK) return rc2;
-        if ((rc2 = conv3(w.T1, r.W2, r.b2, X, skip, X2, nullptr, 0, P, 4, C0, C0, EPI_RESID_SCALE, st)) != TPX_OK) return rc2;
-        std::swap(X, X2);
-        return TPX_OK;
-    };
-    TPX_RC(res4(h->res[0]));
+    TPX_RC(resnet_block(h->res[0], 4, X, X2, sc, P, st));
     TPX_TAP(TPX_VAE_STAGE_MID_RES0, X, 64, C0);
-    {   // VolumeAttention: GN -> qkv -> 64-token attention per primitive -> proj, (x + res) * skip
-        TPX_RC(launch_groupnorm_silu(X, h->ang, h->anb, P, 64, C0, 32, eps, 0, w.T1, st));
-        GemmProblem p{};
-        p.A = w.T1; p.a_mode = AMODE_LINEAR; p.lda = C0; p.W = h->Wqkv; p.M = P * 64; p.N = 3 * C0; p.K = C0; p.BN = 256; p.epi = EPI_HEADS;
-        GemmArgs a{};
-        a.post_scale = 1.0f; a.out0 = w.Q; a.out1 = w.K; a.out2 = w.V; a.split_cols = C0; a.Dh = 32; a.DhP = 32; a.H = h->heads; a.Nseq = 64;
-        p.args = a;
-        TPX_RC(launch_gemm(p, st));
-        TPX_RC(launch_attention(w.Q, w.K, w.V, w.T2, P, h->heads, 64, 64, 32, 32, 1.0f / sqrtf(32.f), st));
-        GemmProblem q{};
-        q.A = w.T2; q.a_mode = AMODE_LINEAR; q.lda = C0; q.W = h->Wap; q.M = P * 64; q.N = C0; q.K = C0; q.BN = 256; q.epi = EPI_RESID_SCALE;
-        GemmArgs b{};
-        b.bias = h->bap; b.post_scale = 1.0f; b.out0 = X2; b.ldo = C0; b.resid = X; b.alpha = skip;
-        q.args = b;
-        TPX_RC(launch_gemm(q, st));
-        std::swap(X, X2);
-    }
+    TPX_RC(attention_block(VaeAttn{h->ang, h->anb, h->Wqkv, h->Wap, h->bap, h->heads}, X, X2, sc, P, C0, st));
     TPX_TAP(TPX_VAE_STAGE_MID_ATTN, X, 64, C0);
-    TPX_RC(res4(h->res[1]));
+    TPX_RC(resnet_block(h->res[1], 4, X, X2, sc, P, st));
     TPX_TAP(TPX_VAE_STAGE_MID_RES1, X, 64, C0);
-    TPX_RC(res4(h->res[2]));
+    TPX_RC(resnet_block(h->res[2], 4, X, X2, sc, P, st));
     TPX_TAP(TPX_VAE_STAGE_UP0_RES0, X, 64, C0);
-    TPX_RC(res4(h->res[3]));
+    TPX_RC(resnet_block(h->res[3], 4, X, X2, sc, P, st));
     TPX_TAP(TPX_VAE_STAGE_UP0_RES1, X, 64, C0);
     {   // ConvTranspose3d(k2,s2): 8 independent 1x1 GEMMs, one per output offset (a,b,c); each writes its stride-2 sub-lattice of the
         // 8^3 volume with bulk tensor stores (full 128-B lines; the single N = 8*C0 GEMM with a per-thread scatter epilogue was store-bound)
@@ -254,6 +296,178 @@ int vae_run(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, in
     TPX_TAP(TPX_VAE_STAGE_NORM_OUT, w.sa, 512, C1);
     TPX_RC(conv3(w.sa, h->Wout, h->bout, nullptr, 1.f, out_dtype == TPX_DTYPE_F16 ? static_cast<__half*>(out) : nullptr,
                  out_dtype == TPX_DTYPE_F32 ? static_cast<float*>(out) : nullptr, h->Cout, P, 8, C1, 16, EPI_NCDHW, st));
+#undef TPX_TAP
+#undef TPX_RC
+    return TPX_OK;
+}
+
+// ---- encoder ----------------------------------------------------------------------------------------------------------------
+const char* kEncResPrefix[6] = {"encoder.down_blocks.0.nets.0.", "encoder.down_blocks.0.nets.1.", "encoder.down_blocks.1.nets.0.",
+                                "encoder.down_blocks.1.nets.1.", "encoder.mid_block.nets.0.", "encoder.mid_block.nets.1."};
+
+void carve_enc(tpx_vae_encoder* h, __half* base) {
+    HCarver c{base};
+    const size_t C0 = h->C0, C1 = h->C1;
+    h->Win = c.take(C0 * h->Cin * 27); h->bin = c.take(C0);
+    for (int i = 0; i < 6; ++i) {
+        VaeRes& r = h->res[i];
+        r.cin = i < 3 ? h->C0 : h->C1;
+        r.cout = i < 2 ? h->C0 : h->C1;
+        r.n1g = c.take(r.cin); r.n1b = c.take(r.cin);
+        r.W1 = c.take(static_cast<size_t>(r.cout) * 27 * r.cin); r.b1 = c.take(r.cout);
+        r.n2g = c.take(r.cout); r.n2b = c.take(r.cout);
+        r.W2 = c.take(static_cast<size_t>(r.cout) * 27 * r.cout); r.b2 = c.take(r.cout);
+        if (r.cin != r.cout) { r.Wsc = c.take(static_cast<size_t>(r.cout) * r.cin); r.bsc = c.take(r.cout); }
+        else { r.Wsc = nullptr; r.bsc = nullptr; }
+    }
+    h->Wds = c.take(C0 * 27 * 8 * C0); h->bds = c.take(C0);
+    h->ang = c.take(C1); h->anb = c.take(C1);
+    h->Wqkv = c.take(3 * C1 * C1); h->Wap = c.take(C1 * C1); h->bap = c.take(C1);
+    h->nog = c.take(C1); h->nob = c.take(C1);
+    h->Wout = c.take(16 * 27 * C1); h->bout = c.take(16);
+    h->quant = c.take(8);
+    h->store_halves = c.off;
+}
+
+enum EncSlotKind { EK_PLAIN, EK_CONV3, EK_CONV3_S2D };
+struct ESlot {
+    __half* ptr;
+    EncSlotKind kind;
+    std::vector<int64_t> shape;
+};
+
+bool find_eslot(tpx_vae_encoder* h, const std::string& key, ESlot* s) {
+    const int64_t C0 = h->C0, C1 = h->C1;
+    auto plain = [&](__half* p, std::vector<int64_t> shp) { *s = ESlot{p, EK_PLAIN, shp}; return true; };
+    auto conv = [&](__half* p, std::vector<int64_t> shp) { *s = ESlot{p, EK_CONV3, shp}; return true; };
+    if (key == "encoder.conv_in.weight") return plain(h->Win, {C0, h->Cin, 3, 3, 3});
+    if (key == "encoder.conv_in.bias") return plain(h->bin, {C0});
+    if (key == "encoder.down_blocks.0.downsample.weight") { *s = ESlot{h->Wds, EK_CONV3_S2D, {C0, C0, 3, 3, 3}}; return true; }
+    if (key == "encoder.down_blocks.0.downsample.bias") return plain(h->bds, {C0});
+    if (key == "encoder.norm_out.weight") return plain(h->nog, {C1});
+    if (key == "encoder.norm_out.bias") return plain(h->nob, {C1});
+    if (key == "encoder.conv_out.weight") return conv(h->Wout, {2, C1, 3, 3, 3});   // rows 2..15 stay zero
+    if (key == "encoder.conv_out.bias") return plain(h->bout, {2});
+    if (key == "quant_conv.weight") return plain(h->quant, {2, 2, 1, 1, 1});
+    if (key == "quant_conv.bias") return plain(h->quant + 4, {2});
+    const std::string a = "encoder.mid_block.attns.0.";
+    if (key == a + "norm.weight") return plain(h->ang, {C1});
+    if (key == a + "norm.bias") return plain(h->anb, {C1});
+    if (key == a + "attn.qkv.weight") return plain(h->Wqkv, {3 * C1, C1});
+    if (key == a + "attn.proj.weight") return plain(h->Wap, {C1, C1});
+    if (key == a + "attn.proj.bias") return plain(h->bap, {C1});
+    for (int i = 0; i < 6; ++i) {
+        const std::string p = kEncResPrefix[i];
+        if (key.rfind(p, 0) != 0) continue;
+        VaeRes& r = h->res[i];
+        const std::string t = key.substr(p.size());
+        if (t == "norm1.weight") return plain(r.n1g, {r.cin});
+        if (t == "norm1.bias") return plain(r.n1b, {r.cin});
+        if (t == "norm2.weight") return plain(r.n2g, {r.cout});
+        if (t == "norm2.bias") return plain(r.n2b, {r.cout});
+        if (t == "conv1.weight") return conv(r.W1, {r.cout, r.cin, 3, 3, 3});
+        if (t == "conv1.bias") return plain(r.b1, {r.cout});
+        if (t == "conv2.weight") return conv(r.W2, {r.cout, r.cout, 3, 3, 3});
+        if (t == "conv2.bias") return plain(r.b2, {r.cout});
+        if (r.Wsc != nullptr && t == "shortcut.weight") return plain(r.Wsc, {r.cout, r.cin, 1, 1, 1});
+        if (r.Wsc != nullptr && t == "shortcut.bias") return plain(r.bsc, {r.cout});
+        return false;
+    }
+    return false;
+}
+
+// Scratch: every activation of the encoder is 32 KB per primitive (8^3 x 32 or 4^3 x 256 fp16), so the workspace is eight such buffers.
+struct EncWs {
+    __half *A, *B, *T1, *T2, *Q, *K, *V, *SC;
+    size_t total;
+};
+EncWs carve_ews(int P, uint8_t* base) {
+    EncWs w;
+    size_t off = 0;
+    auto take = [&]() {
+        uint8_t* p = base == nullptr ? nullptr : base + off;
+        off += (static_cast<size_t>(P) * 16384 * 2 + 1023) & ~static_cast<size_t>(1023);
+        return reinterpret_cast<__half*>(p);
+    };
+    w.A = take(); w.B = take(); w.T1 = take(); w.T2 = take(); w.Q = take(); w.K = take(); w.V = take(); w.SC = take();
+    w.total = off;
+    return w;
+}
+
+int check_enc_args(const tpx_vae_encoder* h, const void* x, const void* dst, int P, const void* ws, size_t ws_bytes, const char* what) {
+    TPX_CHECK(h != nullptr && x != nullptr && dst != nullptr && ws != nullptr, TPX_ERR_ARG, "%s: null argument", what);
+    TPX_CHECK(h->finalized, TPX_ERR_STATE, "%s: weights not finalized (load the encoder tensors first)", what);
+    TPX_CHECK(P > 0, TPX_ERR_SHAPE, "%s: empty batch", what);
+    const size_t need = carve_ews(P, nullptr).total;
+    TPX_CHECK(ws_bytes >= need, TPX_ERR_ARG, "%s: workspace too small (%zu < %zu)", what, ws_bytes, need);
+    TPX_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "%s: workspace must be 256-B aligned", what);
+    return TPX_OK;
+}
+
+// The encode schedule (Encoder.forward + quant_conv, vae3d_dib.py:310-327, :431-433).  stop < 0 runs it to the end and writes the
+// moments; stop = TPX_VAE_ENC_STAGE_* ends after that stage and copies its channels-last fp16 activation into `tap`.
+// Launches: conv_in 1, 8^3 block 4 + 4, downsample 2, 32 -> 256 block 5, 256 blocks 4 each, attention 4, norm_out 1, conv_out 1: 34.
+int enc_run(tpx_vae_encoder* h, const void* x, int x_dtype, void* out, int out_dtype, int P, int stop, void* tap, void* ws, cudaStream_t st) {
+    EncWs w = carve_ews(P, static_cast<uint8_t*>(ws));
+    const int C0 = h->C0, C1 = h->C1;
+    const BlockScratch sc{w.T1, w.T2, w.Q, w.K, w.V};
+    int rc;
+#define TPX_RC(call) do { rc = (call); if (rc != TPX_OK) return rc; } while (0)
+#define TPX_TAP(stage, act, S3, C)                                                                                                   \
+    do {                                                                                                                             \
+        if (stop == (stage)) {                                                                                                       \
+            TPX_CUDA(cudaMemcpyAsync(tap, act, static_cast<size_t>(P) * (S3) * (C) * sizeof(__half), cudaMemcpyDeviceToDevice, st)); \
+            return TPX_OK;                                                                                                           \
+        }                                                                                                                            \
+    } while (0)
+    __half *X = w.A, *X2 = w.B;
+    TPX_RC(launch_vae_enc_conv_in(x, x_dtype, h->Win, h->bin, P, X, st));
+    TPX_TAP(TPX_VAE_ENC_STAGE_CONV_IN, X, 512, C0);
+    TPX_RC(resnet_block(h->res[0], 8, X, X2, sc, P, st));
+    TPX_TAP(TPX_VAE_ENC_STAGE_DOWN0_RES0, X, 512, C0);
+    TPX_RC(resnet_block(h->res[1], 8, X, X2, sc, P, st));
+    TPX_TAP(TPX_VAE_ENC_STAGE_DOWN0_RES1, X, 512, C0);
+    // Conv3d(k3, s2, p1) 8^3 -> 4^3 as a stride-1 conv over the space-to-depth volume [P, 4^3, 8*32] (launch_pack_conv3_s2d)
+    TPX_RC(launch_space_to_depth2(X, w.T1, P, C0, st));
+    TPX_RC(conv3(w.T1, h->Wds, h->bds, nullptr, 1.f, X2, nullptr, 0, P, 4, 8 * C0, C0, EPI_STORE, st));
+    std::swap(X, X2);
+    TPX_TAP(TPX_VAE_ENC_STAGE_DOWNSAMPLE, X, 64, C0);
+    {   // ResnetBlock C0 -> C1 at 4^3 with its 1x1 shortcut (a K = 32 GEMM)
+        const VaeRes& r = h->res[2];
+        TPX_RC(launch_groupnorm_silu(X, r.n1g, r.n1b, P, 64, C0, 32, kEps, 1, w.T1, st));
+        TPX_RC(conv3(w.T1, r.W1, r.b1, nullptr, 1.f, w.T2, nullptr, 0, P, 4, C0, C1, EPI_STORE, st));
+        TPX_RC(launch_groupnorm_silu(w.T2, r.n2g, r.n2b, P, 64, C1, 32, kEps, 1, w.T1, st));
+        GemmProblem p{};
+        p.A = X; p.a_mode = AMODE_LINEAR; p.lda = C0; p.W = r.Wsc; p.M = P * 64; p.N = C1; p.K = C0; p.BN = 256; p.epi = EPI_STORE;
+        GemmArgs a{};
+        a.bias = r.bsc; a.post_scale = 1.0f; a.out0 = w.SC; a.ldo = C1;
+        p.args = a;
+        TPX_RC(launch_gemm(p, st));
+        TPX_RC(conv3(w.T1, r.W2, r.b2, w.SC, kSkip, X2, nullptr, 0, P, 4, C1, C1, EPI_RESID_SCALE, st));
+        std::swap(X, X2);
+    }
+    TPX_TAP(TPX_VAE_ENC_STAGE_DOWN1_RES0, X, 64, C1);
+    TPX_RC(resnet_block(h->res[3], 4, X, X2, sc, P, st));
+    TPX_TAP(TPX_VAE_ENC_STAGE_DOWN1_RES1, X, 64, C1);
+    TPX_RC(resnet_block(h->res[4], 4, X, X2, sc, P, st));
+    TPX_TAP(TPX_VAE_ENC_STAGE_MID_RES0, X, 64, C1);
+    TPX_RC(attention_block(VaeAttn{h->ang, h->anb, h->Wqkv, h->Wap, h->bap, h->heads}, X, X2, sc, P, C1, st));
+    TPX_TAP(TPX_VAE_ENC_STAGE_MID_ATTN, X, 64, C1);
+    TPX_RC(resnet_block(h->res[5], 4, X, X2, sc, P, st));
+    TPX_TAP(TPX_VAE_ENC_STAGE_MID_RES1, X, 64, C1);
+    TPX_RC(launch_groupnorm_silu(X, h->nog, h->nob, P, 64, C1, 32, kEps, 1, w.T1, st));
+    TPX_TAP(TPX_VAE_ENC_STAGE_NORM_OUT, w.T1, 64, C1);
+    {   // conv_out 256 -> 2 (16-row tile, rows 2..15 zero) with quant_conv in the epilogue, written NCDHW [P, 2, 4, 4, 4]
+        GemmProblem p{};
+        p.A = w.T1; p.a_mode = AMODE_CONV3; p.conv_S = 4; p.conv_C = C1; p.W = h->Wout;
+        p.M = P * 64; p.N = 16; p.K = 27 * C1; p.BN = 16; p.epi = EPI_MOMENTS;
+        GemmArgs a{};
+        a.bias = h->bout; a.post_scale = 1.0f; a.quant = h->quant; a.S3 = 64;
+        a.out0 = out_dtype == TPX_DTYPE_F16 ? static_cast<__half*>(out) : nullptr;
+        a.out32 = out_dtype == TPX_DTYPE_F32 ? static_cast<float*>(out) : nullptr;
+        p.args = a;
+        TPX_RC(launch_gemm(p, st));
+    }
 #undef TPX_TAP
 #undef TPX_RC
     return TPX_OK;
@@ -363,6 +577,97 @@ int tpx_conv3d_k3(const void* x, const void* W, const void* bias, const void* re
     const bool plain = resid == nullptr && alpha == 1.0f;
     return conv3(static_cast<const __half*>(x), static_cast<const __half*>(W), static_cast<const __half*>(bias), static_cast<const __half*>(resid), alpha,
                  static_cast<__half*>(out), nullptr, 0, P, S, C, Cout, plain ? EPI_STORE : EPI_RESID_SCALE, static_cast<cudaStream_t>(stream));
+}
+
+
+// ---- encoder -------------------------------------------------------------------------------------------------------------------
+int tpx_vae_encoder_create(const tpx_vae_config* c, tpx_vae_encoder** out) {
+    TPX_CHECK(c != nullptr && out != nullptr, TPX_ERR_ARG, "vae_encoder_create: null argument");
+    TPX_CHECK(c->latent_channels == 1 && c->out_channels == 6, TPX_ERR_SHAPE,
+              "vae_encoder_create: latent %d / in_channels %d unsupported (kernel set covers the shipped config: 1 / 6)", c->latent_channels, c->out_channels);
+    TPX_CHECK(c->ch_mid == 256 && c->ch_out == 32, TPX_ERR_SHAPE, "vae_encoder_create: down_channels (%d,%d) unsupported (kernel set covers (32,256))",
+              c->ch_out, c->ch_mid);
+    TPX_CHECK(c->attn_heads > 0 && c->ch_mid % c->attn_heads == 0 && (c->ch_mid / c->attn_heads) == 32, TPX_ERR_SHAPE, "vae_encoder_create: attention head dim must be 32");
+    TPX_DEVICE_GUARD();
+    tpx_vae_encoder* h = new tpx_vae_encoder();
+    h->heads = c->attn_heads;
+    carve_enc(h, nullptr);
+    cudaError_t e = cudaMalloc(&h->store, h->store_halves * 2);
+    if (e != cudaSuccess) { delete h; return cuda_fail(e, "cudaMalloc(vae encoder parameter store)"); }
+    e = cudaMemset(h->store, 0, h->store_halves * 2);
+    if (e != cudaSuccess) { cudaFree(h->store); delete h; return cuda_fail(e, "cudaMemset(vae encoder parameter store)"); }
+    carve_enc(h, h->store);
+    auto& r = h->required;
+    for (const char* k : {"encoder.conv_in.weight", "encoder.conv_in.bias", "encoder.down_blocks.0.downsample.weight", "encoder.down_blocks.0.downsample.bias",
+                          "encoder.mid_block.attns.0.norm.weight", "encoder.mid_block.attns.0.norm.bias", "encoder.mid_block.attns.0.attn.qkv.weight",
+                          "encoder.mid_block.attns.0.attn.proj.weight", "encoder.mid_block.attns.0.attn.proj.bias", "encoder.norm_out.weight",
+                          "encoder.norm_out.bias", "encoder.conv_out.weight", "encoder.conv_out.bias", "quant_conv.weight", "quant_conv.bias"})
+        r.emplace_back(k);
+    for (int i = 0; i < 6; ++i) {
+        for (const char* k : {"norm1.weight", "norm1.bias", "conv1.weight", "conv1.bias", "norm2.weight", "norm2.bias", "conv2.weight", "conv2.bias"})
+            r.emplace_back(std::string(kEncResPrefix[i]) + k);
+        if (h->res[i].Wsc != nullptr) { r.emplace_back(std::string(kEncResPrefix[i]) + "shortcut.weight"); r.emplace_back(std::string(kEncResPrefix[i]) + "shortcut.bias"); }
+    }
+    h->seen.assign(r.size(), 0);
+    *out = h;
+    return TPX_OK;
+}
+
+void tpx_vae_encoder_destroy(tpx_vae_encoder* h) {
+    if (h == nullptr) return;
+    if (h->store != nullptr) cudaFree(h->store);
+    delete h;
+}
+
+int tpx_vae_encoder_set_weight(tpx_vae_encoder* h, const char* ref_key, const void* dev_ptr, int dtype, const int64_t* shape, int ndim, void* stream) {
+    TPX_CHECK(h != nullptr && ref_key != nullptr && dev_ptr != nullptr && shape != nullptr, TPX_ERR_ARG, "vae_encoder_set_weight: null argument");
+    const std::string key(ref_key);
+    if (key.rfind("decoder.", 0) == 0 || key.rfind("post_quant_conv.", 0) == 0) return 1;  // not on the encode path
+    ESlot s;
+    if (!find_eslot(h, key, &s)) { set_error("vae_encoder_set_weight: unexpected key '%s'", ref_key); return TPX_ERR_KEY; }
+    bool ok = ndim == static_cast<int>(s.shape.size());
+    long long n = 1;
+    for (int i = 0; ok && i < ndim; ++i) { ok = shape[i] == s.shape[i]; n *= shape[i]; }
+    TPX_CHECK(ok, TPX_ERR_SHAPE, "vae_encoder_set_weight: size mismatch for %s", ref_key);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int rc = TPX_OK;
+    switch (s.kind) {
+        case EK_PLAIN: rc = launch_to_half(dev_ptr, dtype, s.ptr, n, st); break;
+        case EK_CONV3: rc = launch_pack_conv3(dev_ptr, dtype, s.ptr, static_cast<int>(s.shape[0]), static_cast<int>(s.shape[1]), 0, st); break;
+        case EK_CONV3_S2D: rc = launch_pack_conv3_s2d(dev_ptr, dtype, s.ptr, static_cast<int>(s.shape[0]), static_cast<int>(s.shape[1]), st); break;
+    }
+    if (rc != TPX_OK) return rc;
+    for (size_t i = 0; i < h->required.size(); ++i)
+        if (h->required[i] == key) h->seen[i] = 1;
+    h->finalized = false;
+    return TPX_OK;
+}
+
+int tpx_vae_encoder_finalize(tpx_vae_encoder* h, void* stream) {
+    (void)stream;
+    TPX_CHECK(h != nullptr, TPX_ERR_ARG, "vae_encoder_finalize: null handle");
+    for (size_t i = 0; i < h->required.size(); ++i) TPX_CHECK(h->seen[i], TPX_ERR_STATE, "vae_encoder_finalize: missing key '%s' in state_dict", h->required[i].c_str());
+    h->finalized = true;
+    return TPX_OK;
+}
+
+size_t tpx_vae_encoder_workspace_bytes(const tpx_vae_encoder* h, int P) {
+    if (h == nullptr || P <= 0) return 0;
+    return carve_ews(P, nullptr).total;
+}
+
+int tpx_vae_encode(tpx_vae_encoder* h, const void* x, int x_dtype, void* moments_out, int out_dtype, int P, void* ws, size_t ws_bytes, void* stream) {
+    const int rc = check_enc_args(h, x, moments_out, P, ws, ws_bytes, "vae_encode");
+    if (rc != TPX_OK) return rc;
+    TPX_CHECK(out_dtype == TPX_DTYPE_F32 || out_dtype == TPX_DTYPE_F16, TPX_ERR_ARG, "vae_encode: bad output dtype %d", out_dtype);
+    return enc_run(h, x, x_dtype, moments_out, out_dtype, P, -1, nullptr, ws, static_cast<cudaStream_t>(stream));
+}
+
+int tpx_vae_encode_debug_stage(tpx_vae_encoder* h, const void* x, int x_dtype, int P, int stage, void* tap_f16, void* ws, size_t ws_bytes, void* stream) {
+    const int rc = check_enc_args(h, x, tap_f16, P, ws, ws_bytes, "vae_encode_debug_stage");
+    if (rc != TPX_OK) return rc;
+    TPX_CHECK(stage >= TPX_VAE_ENC_STAGE_CONV_IN && stage <= TPX_VAE_ENC_STAGE_NORM_OUT, TPX_ERR_ARG, "vae_encode_debug_stage: bad stage %d", stage);
+    return enc_run(h, x, x_dtype, nullptr, TPX_DTYPE_F16, P, stage, tap_f16, ws, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

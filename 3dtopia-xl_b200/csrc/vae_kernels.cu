@@ -1,6 +1,8 @@
-// VAE-decoder kernels that are not GEMM shaped: the 1->C input convolution, GroupNorm(+SiLU) on
-// channels-last fp16 volumes, and the weight repacks into the implicit-GEMM [Cout, 27*Cin] layout.
-//   reference: models/vae3d_dib.py:93-145 (ResnetBlock), :344 (conv_in), :366-367 (norm_out / conv_out), :429
+// VAE kernels that are not GEMM shaped: the decoder's 1->C and the encoder's 6->32 input convolutions, the space-to-depth pack
+// of the encoder's stride-2 convolution, GroupNorm(+SiLU) on channels-last fp16 volumes, and the weight repacks into the
+// implicit-GEMM [Cout, 27*Cin] layout.
+//   reference: models/vae3d_dib.py:93-145 (ResnetBlock), :344 (conv_in), :366-367 (norm_out / conv_out), :429,
+//              :284 / :313 (Encoder.conv_in), :168 (DownBlock.downsample)
 #include "kernels.cuh"
 
 namespace tpx {
@@ -45,6 +47,100 @@ int launch_vae_conv_in(const void* z, int z_dtype, const __half* w_pq, const __h
     if (z_dtype == TPX_DTYPE_F32) vae_conv_in_kernel<float><<<P, 256, 0, st>>>(static_cast<const float*>(z), w_pq, b_pq, W, bias, C, out);
     else if (z_dtype == TPX_DTYPE_F16) vae_conv_in_kernel<__half><<<P, 256, 0, st>>>(static_cast<const __half*>(z), w_pq, b_pq, W, bias, C, out);
     else { set_error("vae_conv_in: unsupported latent dtype %d", z_dtype); return TPX_ERR_ARG; }
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Encoder conv_in (3x3x3, pad 1, 6 -> 32): x NCDHW [P,6,8,8,8] fp32 / fp16 -> channels-last fp16 [P,512,32].
+// K = 6*27 = 162 fits neither the 32- nor the 64-channel chunks of the tensor-core paths and the layer is ~5 MFLOP per primitive,
+// so it runs on the FMA pipe: one CTA per primitive, one thread per output voxel holding all 32 output channels; the zero-padded
+// 10^3 x 6 input (rounded to fp16 first: autocast's input cast) and the weights, transposed to [ci*27+tap][32] so one tap's 32
+// output-channel weights are eight broadcast 16-byte loads, live in shared memory.  fp32 accumulation, one fp16 rounding.
+// ---------------------------------------------------------------------------------------------------------
+constexpr int ENC_CIN = 6, ENC_C0 = 32;
+template <typename XT>
+__global__ void __launch_bounds__(512) vae_enc_conv_in_kernel(const XT* __restrict__ x, const __half* __restrict__ W /*[32, 6*27]*/,
+                                                              const __half* __restrict__ bias, __half* __restrict__ out) {
+    __shared__ float s_x[ENC_CIN * 1000];
+    __shared__ __align__(16) float s_w[ENC_CIN * 27 * ENC_C0];
+    const int p = blockIdx.x;
+    for (int i = threadIdx.x; i < ENC_CIN * 1000; i += blockDim.x) s_x[i] = 0.f;
+    for (int i = threadIdx.x; i < ENC_CIN * 27 * ENC_C0; i += blockDim.x) {
+        const int co = i % ENC_C0, k = i / ENC_C0;
+        s_w[i] = __half2float(W[co * (ENC_CIN * 27) + k]);
+    }
+    __syncthreads();
+    const XT* xp = x + static_cast<size_t>(p) * ENC_CIN * 512;
+    for (int i = threadIdx.x; i < ENC_CIN * 512; i += blockDim.x) {
+        const int ci = i >> 9, v = i & 511;
+        s_x[ci * 1000 + (((v >> 6) + 1) * 10 + ((v >> 3) & 7) + 1) * 10 + (v & 7) + 1] = h2f_round(static_cast<float>(xp[i]));
+    }
+    __syncthreads();
+    const int v = threadIdx.x, z = v >> 6, y = (v >> 3) & 7, xx = v & 7;
+    float acc[ENC_C0];
+#pragma unroll
+    for (int c = 0; c < ENC_C0; ++c) acc[c] = __half2float(bias[c]);
+    for (int ci = 0; ci < ENC_CIN; ++ci) {
+#pragma unroll 3
+        for (int t = 0; t < 27; ++t) {
+            const float xv = s_x[ci * 1000 + ((z + t / 9) * 10 + y + (t / 3) % 3) * 10 + xx + t % 3];
+            const float4* wp = reinterpret_cast<const float4*>(s_w + (ci * 27 + t) * ENC_C0);
+#pragma unroll
+            for (int q = 0; q < ENC_C0 / 4; ++q) {
+                const float4 w4 = wp[q];
+                acc[4 * q] = fmaf(w4.x, xv, acc[4 * q]);
+                acc[4 * q + 1] = fmaf(w4.y, xv, acc[4 * q + 1]);
+                acc[4 * q + 2] = fmaf(w4.z, xv, acc[4 * q + 2]);
+                acc[4 * q + 3] = fmaf(w4.w, xv, acc[4 * q + 3]);
+            }
+        }
+    }
+    uint4* op = reinterpret_cast<uint4*>(out + (static_cast<size_t>(p) * 512 + v) * ENC_C0);
+#pragma unroll
+    for (int j = 0; j < ENC_C0 / 8; ++j) {
+        Pack8 o;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) o.h[k] = __float2half_rn(acc[j * 8 + k]);
+        op[j] = o.u;
+    }
+}
+
+int launch_vae_enc_conv_in(const void* x, int x_dtype, const __half* W, const __half* bias, int P, __half* out, cudaStream_t st) {
+    if (P <= 0) return TPX_OK;
+    ProfScope prof(PROF_VAE_MISC, st);
+    if (x_dtype == TPX_DTYPE_F32) vae_enc_conv_in_kernel<float><<<P, 512, 0, st>>>(static_cast<const float*>(x), W, bias, out);
+    else if (x_dtype == TPX_DTYPE_F16) vae_enc_conv_in_kernel<__half><<<P, 512, 0, st>>>(static_cast<const __half*>(x), W, bias, out);
+    else { set_error("vae_enc_conv_in: unsupported input dtype %d", x_dtype); return TPX_ERR_ARG; }
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Space-to-depth: channels-last [P, 8,8,8, C] -> [P, 4,4,4, 8C], out[p, qz,qy,qx, ((az*2+ay)*2+ax)*C + c] = in[p, 2qz+az, 2qy+ay, 2qx+ax, c].
+// With the weight of launch_pack_conv3_s2d, the stride-2 / pad-1 convolution (vae3d_dib.py:168) becomes a stride-1 3x3x3 / pad-1
+// convolution at 4^3 on the implicit-GEMM path: input 2o + d (d = -1, 0, 1) is phase 1 of block o - 1, phase 0 / 1 of block o.
+// One thread per 16-byte channel octet.
+// ---------------------------------------------------------------------------------------------------------
+__global__ void space_to_depth2_kernel(const __half* __restrict__ in, __half* __restrict__ out, int C, long long n_oct) {
+    const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= n_oct) return;
+    const int opv = C;                                   // octets per output voxel: 8C / 8
+    const long long pq = i / opv;                        // (primitive, output voxel)
+    const int r = static_cast<int>(i - pq * opv);
+    const int phase = r / (C >> 3), co8 = r - phase * (C >> 3);
+    const long long p = pq >> 6;
+    const int q = static_cast<int>(pq & 63), qz = q >> 4, qy = (q >> 2) & 3, qx = q & 3;
+    const int z = 2 * qz + (phase >> 2), y = 2 * qy + ((phase >> 1) & 1), x = 2 * qx + (phase & 1);
+    reinterpret_cast<uint4*>(out)[i] = reinterpret_cast<const uint4*>(in + ((p * 512 + (z * 8 + y) * 8 + x) * C))[co8];
+}
+
+int launch_space_to_depth2(const __half* in, __half* out, int P, int C, cudaStream_t st) {
+    TPX_CHECK(C % 8 == 0, TPX_ERR_SHAPE, "space_to_depth: channels %d must be a multiple of 8", C);
+    if (P <= 0) return TPX_OK;
+    ProfScope prof(PROF_VAE_MISC, st);
+    const long long n = static_cast<long long>(P) * 64 * C;   // octets of the output: P * 64 voxels * 8C / 8
+    space_to_depth2_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(in, out, C, n);
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }
@@ -439,6 +535,39 @@ __global__ void pack_convt2_kernel(const T* __restrict__ src, __half* __restrict
     const int row = static_cast<int>(i / Cin), ci = static_cast<int>(i - static_cast<long long>(row) * Cin);
     const int abc = row / Cout, co = row - abc * Cout;
     dst[i] = __float2half_rn(static_cast<float>(src[(static_cast<size_t>(ci) * Cout + co) * 8 + abc]));
+}
+
+// Stride-2 Conv3d weight [Cout,Cin,3,3,3] -> the stride-1 weight over the space-to-depth input, [Cout, 27*8Cin] with
+// k = tap'*8Cin + phase*Cin + ci.  Per axis, block offset k' (0, 1, 2 = block o-1, o, o+1) and phase a pick original tap
+// (k', a) = (0, 1) -> 0, (1, 0) -> 1, (1, 1) -> 2; every other pair (and so every k' = 2 tap) is zero.
+template <typename T>
+__global__ void pack_conv3_s2d_kernel(const T* __restrict__ src, __half* __restrict__ dst, int Cout, int Cin) {
+    const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const int K = 27 * 8 * Cin;
+    if (i >= static_cast<long long>(Cout) * K) return;
+    const int co = static_cast<int>(i / K);
+    const int r = static_cast<int>(i - static_cast<long long>(co) * K);
+    const int tap = r / (8 * Cin), ph = (r / Cin) & 7, ci = r % Cin;
+    const int kk[3] = {tap / 9, (tap / 3) % 3, tap % 3}, aa[3] = {ph >> 2, (ph >> 1) & 1, ph & 1};
+    int orig = 0;
+    bool ok = true;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+        const int t = kk[d] == 0 ? (aa[d] == 1 ? 0 : -1) : (kk[d] == 1 ? 1 + aa[d] : -1);
+        ok = ok && t >= 0;
+        orig = orig * 3 + (t < 0 ? 0 : t);
+    }
+    dst[i] = ok ? __float2half_rn(static_cast<float>(src[(static_cast<size_t>(co) * Cin + ci) * 27 + orig])) : __float2half_rn(0.f);
+}
+
+int launch_pack_conv3_s2d(const void* src, int dtype, __half* dst, int Cout, int Cin, cudaStream_t st) {
+    const long long n = static_cast<long long>(Cout) * 27 * 8 * Cin;
+    const unsigned grid = static_cast<unsigned>((n + 255) / 256);
+    if (dtype == TPX_DTYPE_F32) pack_conv3_s2d_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float*>(src), dst, Cout, Cin);
+    else if (dtype == TPX_DTYPE_F16) pack_conv3_s2d_kernel<__half><<<grid, 256, 0, st>>>(static_cast<const __half*>(src), dst, Cout, Cin);
+    else { set_error("pack_conv3_s2d: unsupported dtype %d", dtype); return TPX_ERR_ARG; }
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
 }
 
 int launch_pack_conv3(const void* src, int dtype, __half* dst, int Cout, int Cin, int transposed, cudaStream_t st) {

@@ -86,6 +86,38 @@ class LatentCodec:
         return out
 
 
+    # ---- the other direction: PrimX volumes -> latents (building a latent dataset, round-trip checks) ----------------------------
+    # The reference ships no encoder-side preprocessing; these are the algebraic inverses of its sampling glue (inference.py:330, :335,
+    # :343-346), a convention of this package.  Elementwise torch ops on the inputs' device.
+    def unpack(self, recon_param: torch.Tensor):
+        """Inverse of ``pack``: recon_param [B, P, 4 + 6*512] -> srt [B, P, 4] fp32, feats [B*P, 6, 8, 8, 8] fp32 with the sdf channel
+        times 5 and the other five channels mapped back by x * 2 - 1 (and, without per-channel statistics, srt scale (s - 0.05) * 10)."""
+        if recon_param.dim() != 3 or recon_param.shape[-1] != 4 + 6 * VOX:
+            raise ValueError(f"recon_param must be [B, P, {4 + 6 * VOX}], got {tuple(recon_param.shape)}")
+        B, P = recon_param.shape[:2]
+        rp = recon_param.to(torch.float32)
+        srt = rp[..., 0:4].clone()
+        if not self.perchannel_norm:
+            srt[..., 0:1] = (srt[..., 0:1] - 0.05) * 10
+        feats = rp[..., 4:].reshape(B * P, 6, 8, 8, 8).clone()
+        feats[:, 0:1] *= 5.0
+        feats[:, 1:] = feats[:, 1:] * 2.0 - 1.0
+        return srt, feats
+
+    def merge(self, srt: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
+        """Inverse of ``split``: srt [B, P, 4] + z [B*P, 1, 4, 4, 4] (or [B, P, 64]) -> sample [B, P, 68] fp32 in the DiT's normalised
+        latent space: (p - latent_mean) / latent_std * latent_nf with per-channel statistics, else (srt, z * latent_nf)."""
+        B, P = srt.shape[:2]
+        if z.numel() != B * P * 64:
+            raise ValueError(f"z must hold {B * P} latents of 64 values, got {tuple(z.shape)}")
+        p = torch.cat([srt.to(torch.float32), z.reshape(B, P, 64).to(torch.float32)], dim=-1)
+        if self.perchannel_norm:
+            mean, std = (self._mean.to(p.device), self._std.to(p.device))
+            return (p - mean) / std * self.latent_nf
+        p[..., 4:] = p[..., 4:] * self.latent_nf
+        return p
+
+
 class PrimXPipeline:
     """DDIM/DDPM sampling + VAE decode of image-conditioned PrimX latents (config #2 / #3 / #5 of BASELINE.json).
 
@@ -117,6 +149,17 @@ class PrimXPipeline:
         P = self.num_prims
         decoded = torch.cat([self.vae.decode(z[b * P:(b + 1) * P]) for b in range(sample.shape[0])], dim=0) if sample.shape[0] > 1 else self.vae.decode(z)
         return self.codec.pack(srt, decoded)
+
+    def encode_primvolume(self, recon_param: torch.Tensor, sample: bool = False) -> torch.Tensor:
+        """PrimX volumes -> DiT latents, the inverse of ``decode_latents``: recon_param [B, P, 3076] -> [B, P, 68] (``LatentCodec.unpack``,
+        VAE.encode, the posterior's mode or a sample, ``LatentCodec.merge``).  One asset at a time, like decoding."""
+        srt, feats = self.codec.unpack(recon_param)
+        B, P = srt.shape[:2]
+        zs = []
+        for b in range(B):
+            post = self.vae.encode(feats[b * P:(b + 1) * P])
+            zs.append(post.sample() if sample else post.mode())
+        return self.codec.merge(srt, torch.cat(zs, dim=0))
 
     def _model_kwargs(self, y):
         kw = dict(y=y, precision_dtype=self.precision_dtype, enable_amp=self.amp)

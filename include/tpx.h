@@ -182,6 +182,34 @@ enum {
 int tpx_vae_debug_stage(tpx_vae* h, const void* z_dev, int z_dtype, int P, int stage, void* tap_f16_dev, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * VAE encoder — models/vae3d_dib.py:431-435 (VAE.encode), :270-327 (Encoder), :147-184 (DownBlock), :428 (quant_conv).
+ * A handle of its own, so the decoder handle's keys, return codes and workspace are untouched.  The config is tpx_vae_config with
+ * out_channels = the encoder's in_channels (6), ch_out / ch_mid = down_channels (32 / 256), latent_channels 1, attn_heads 8.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct tpx_vae_encoder tpx_vae_encoder;
+int tpx_vae_encoder_create(const tpx_vae_config* cfg, tpx_vae_encoder** out);
+void tpx_vae_encoder_destroy(tpx_vae_encoder* h);
+/* encoder.* / quant_conv.* keys are consumed (the stride-2 downsample weight is repacked for its space-to-depth input);
+ * decoder.* / post_quant_conv.* keys are accepted and ignored (return 1). */
+int tpx_vae_encoder_set_weight(tpx_vae_encoder* h, const char* ref_key, const void* dev_ptr, int dtype, const int64_t* shape, int ndim, void* stream);
+int tpx_vae_encoder_finalize(tpx_vae_encoder* h, void* stream);
+size_t tpx_vae_encoder_workspace_bytes(const tpx_vae_encoder* h, int P);
+/* VAE.encode up to the posterior's parameters (vae3d_dib.py:431-433): x device [P,6,8,8,8] (dtype x_dtype) -> moments device
+ * [P,2,4,4,4] (dtype out_dtype) = quant_conv(encoder(x)); channel 0 is the mean, 1 the (unclamped) log-variance. */
+int tpx_vae_encode(tpx_vae_encoder* h, const void* x_dev, int x_dtype, void* moments_dev, int out_dtype, int P, void* ws, size_t ws_bytes, void* stream);
+/* Debug / parity: run the encode schedule through `stage` and copy that stage's channels-last fp16 activation [P, S^3, C] into
+ * tap_f16_dev.  Stages (Encoder.forward, vae3d_dib.py:310-327): 0 conv_in, 1 / 2 down_blocks.0 res 0 / 1 [P,512,32];
+ * 3 down_blocks.0 downsample [P,64,32]; 4 / 5 down_blocks.1 res 0 (with its 1x1 shortcut) / 1, 6 mid_block res 0, 7 its attention,
+ * 8 mid_block res 1, 9 norm_out + SiLU [P,64,256].  conv_out + quant_conv after stage 9 give tpx_vae_encode's output. */
+enum {
+    TPX_VAE_ENC_STAGE_CONV_IN = 0, TPX_VAE_ENC_STAGE_DOWN0_RES0 = 1, TPX_VAE_ENC_STAGE_DOWN0_RES1 = 2, TPX_VAE_ENC_STAGE_DOWNSAMPLE = 3,
+    TPX_VAE_ENC_STAGE_DOWN1_RES0 = 4, TPX_VAE_ENC_STAGE_DOWN1_RES1 = 5, TPX_VAE_ENC_STAGE_MID_RES0 = 6, TPX_VAE_ENC_STAGE_MID_ATTN = 7,
+    TPX_VAE_ENC_STAGE_MID_RES1 = 8, TPX_VAE_ENC_STAGE_NORM_OUT = 9
+};
+int tpx_vae_encode_debug_stage(tpx_vae_encoder* h, const void* x_dev, int x_dtype, int P, int stage, void* tap_f16_dev, void* ws, size_t ws_bytes,
+                               void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Per-kernel entry points (unit parity tests; each is one launch of one hot-path kernel)
  * ---------------------------------------------------------------------------------------------------------- */
 /* out[M,N] fp16 = act(A[M,K] W[N,K]^T + bias) ; act: 0 none (optionally * post_scale, re-rounded), 1 GELU-tanh.  tile_n: 0 = auto. */
