@@ -13,6 +13,14 @@
 //     (strictly-inside test in the primitive's frame, trilinear channels-last sample, alpha faded by exp(-fadescale * sum |y|^fadeexp)
 //     with the fast-math intrinsics the reference is compiled with), additive alpha with saturation at 1.
 // The first 96 listed primitives' transforms live in shared memory (the march re-reads them at every step).
+// The same kernel, instantiated with GRAD, is the backward (raymarch_subset_backward_kernel, mvpraymarch_subset_kernel.h:103-217, with
+// forwarddir = true): it rebuilds the hit list, re-marches from the same first step through the SAME device code (so every inside test,
+// saturation and step count is the forward's), and per listed primitive and step applies PrimAccumAdditive::forwardbackward_prim
+// (primaccum.h:81-98), PrimSamplerTW<false>::backward (primsampler.h:68-91) and PrimTransfSRT::backward (primtransf.h:155-179):
+//   * the template gradient is a trilinear scatter, one sm_90 vector reduction (atomicAdd(float4*) -> RED.E.ADD.F32x4) per corner;
+//   * the 15 transform partials are summed over the warp with shuffles (all 32 lanes visit the same primitive at the same step) and
+//     lanes 0..14 each issue one reduction.
+// Subsampled rays (ray_subsample_factor > 1): output pixel (j, i) traces the ray through image pixel (x0 + stride j, y0 + stride i).
 #include "kernels.cuh"
 
 namespace tpx {
@@ -32,9 +40,17 @@ struct RayMarchArgs {
     const float* camrot;     // [N, 3, 3]
     const float* focal;      // [N, 2]
     const float* princpt;    // [N, 2]
-    float* out;              // [N, H, W, 4]
-    int N, K, S, H, W;
+    float* out;              // [N, H, W, 4]  (forward)
+    int N, K, S, H, W;       // H, W: the marched (subsampled) image
     float volradius, stepsize, fadescale, fadeexp;
+    int stride;              // image pixel = offset + stride * output pixel
+    const int* offsets;      // [N, 2] (x0, y0), or null for (0, 0)
+    float* raysat;           // forward: [N, H, W, 3] colour of the saturating sample, (-1,-1,-1) if none; may be null.  backward: read
+    const float* grad_out;   // backward: [N, H, W, 4]
+    float* grad_tpl;         // backward, accumulated: [N, K, S, S, S, 4]
+    float* grad_pos;         // [N, K, 3]
+    float* grad_rot;         // [N, K, 3, 3]
+    float* grad_scale;       // [N, K, 3]
 };
 
 struct Prim {
@@ -59,7 +75,8 @@ __device__ __forceinline__ Prim load_prim(const RayMarchArgs& a, int n, int k) {
     return p;
 }
 
-__global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_preview_kernel(const RayMarchArgs a) {
+template <bool GRAD>
+__global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchArgs a) {
     __shared__ int s_list[4][RM_MAXHIT];
     __shared__ float s_prim[4][RM_CACHE][16];
     const int lin = threadIdx.y * RM_BX + threadIdx.x;
@@ -73,8 +90,9 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_preview_kernel(const R
     // ---- ray (compute_raydirs_forward_kernel) ----
     float3 raypos = ld3(a.campos + n * 3);
     raypos = make_float3(raypos.x / a.volradius, raypos.y / a.volradius, raypos.z / a.volradius);
-    const float px = (static_cast<float>(w) - a.princpt[n * 2]) / a.focal[n * 2];
-    const float py = (static_cast<float>(h) - a.princpt[n * 2 + 1]) / a.focal[n * 2 + 1];
+    const int ox = a.offsets ? a.offsets[n * 2] : 0, oy = a.offsets ? a.offsets[n * 2 + 1] : 0;
+    const float px = (static_cast<float>(ox + a.stride * w) - a.princpt[n * 2]) / a.focal[n * 2];
+    const float py = (static_cast<float>(oy + a.stride * h) - a.princpt[n * 2 + 1]) / a.focal[n * 2 + 1];
     float3 raydir = ld3(a.camrot + n * 9) * px + ld3(a.camrot + n * 9 + 3) * py + ld3(a.camrot + n * 9 + 6);
     raydir = raydir * rsqrtf(dot3(raydir, raydir));
     float2 tminmax;
@@ -166,6 +184,14 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_preview_kernel(const R
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     const int S = a.S;
     const float hs = static_cast<float>(S - 1);
+    const size_t pix = (static_cast<size_t>(n) * a.H + h) * a.W + w;
+    float3 satrgb = make_float3(-1.f, -1.f, -1.f);   // forward: PrimAccumAdditive's raysat; backward: read back
+    float4 dL = make_float4(0.f, 0.f, 0.f, 0.f);     // backward: upstream gradient of this ray (zero for the border duplicates)
+    if (GRAD) {
+        satrgb = ld3(a.raysat + pix * 3);
+        if (live) dL = *reinterpret_cast<const float4*>(a.grad_out + pix * 4);
+    }
+    const bool rsat = satrgb.x > -1.f;               // the ray saturates somewhere (the reference's test, primaccum.h:92)
     while (!__all_sync(0xffffffffu, done || t > rtmax + 1e-5f)) {
         const bool active = !done && t < rtmax + 1e-5f;
         for (int ks = 0; ks < nhit; ++ks) {
@@ -181,7 +207,13 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_preview_kernel(const R
             const float3 xmt = pos - p.t;
             const float3 y = (p.r0 * xmt.x + p.r1 * xmt.y + p.r2 * xmt.z) * p.s;
             const bool inside = y.x > -1.f && y.x < 1.f && y.y > -1.f && y.y < 1.f && y.z > -1.f && y.z < 1.f;
-            if (inside && active && !done) {
+            const bool eval = inside && active && !done;
+            float gs[15];                                // backward: d/dscale (3), d/drot (9, row-major), d/dpos (3) of this sample
+            if (GRAD) {
+#pragma unroll
+                for (int i = 0; i < 15; ++i) gs[i] = 0.f;
+            }
+            if (eval) {
                 // trilinear channels-last sample (grid_sample_chlast_forward; strictly inside, so all eight corners exist)
                 const float ix = (y.x + 1.f) * 0.5f * hs, iy = (y.y + 1.f) * 0.5f * hs, iz = (y.z + 1.f) * 0.5f * hs;
                 const int x0 = min(static_cast<int>(floorf(ix)), S - 2), y0 = min(static_cast<int>(floorf(iy)), S - 2), z0 = min(static_cast<int>(floorf(iz)), S - 2);
@@ -200,14 +232,93 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_preview_kernel(const R
                 // PrimAccumAdditive::forward_prim
                 const float newalpha = acc.w + alpha * a.stepsize;
                 const float contrib = fminf(newalpha, 1.f) - acc.w;
+                if (GRAD) {
+                    // PrimAccumAdditive::forwardbackward_prim: this sample saturates iff the forward's newalpha >= 1 (same operands)
+                    const bool sat = newalpha >= 1.f;
+                    const float wgt_rgb = sat ? 1.f - acc.w : __fmul_rn(alpha, a.stepsize);
+                    const float dla = sat ? 0.f
+                                          : a.stepsize * ((smp.x - (rsat ? satrgb.x : 0.f)) * dL.x + (smp.y - (rsat ? satrgb.y : 0.f)) * dL.y +
+                                                          (smp.z - (rsat ? satrgb.z : 0.f)) * dL.z + (rsat ? 0.f : dL.w));
+                    // PrimSamplerTW<false>::backward: fade, then the trilinear scatter and its position gradient
+                    const float cf = -(a.fadescale * a.fadeexp) * alpha * dla;
+                    const float fe1 = a.fadeexp - 1.f;
+                    float3 dy = make_float3(cf * __powf(fabsf(y.x), fe1) * (y.x > 0.f ? 1.f : -1.f), cf * __powf(fabsf(y.y), fe1) * (y.y > 0.f ? 1.f : -1.f),
+                                            cf * __powf(fabsf(y.z), fe1) * (y.z > 0.f ? 1.f : -1.f));
+                    const float4 g = make_float4(wgt_rgb * dL.x, wgt_rgb * dL.y, wgt_rgb * dL.z, dla * fade);
+                    float4* gtp = reinterpret_cast<float4*>(a.grad_tpl) + (static_cast<size_t>(n) * a.K + k) * S * S * S + (z0 * S + y0) * S + x0;
+                    float gx = 0.f, gy = 0.f, gz = 0.f;
+#pragma unroll
+                    for (int c = 0; c < 8; ++c) {
+                        const int dz = c >> 2, dy_ = (c >> 1) & 1, dx = c & 1;
+                        const float wx = dx ? ax : 1.f - ax, wy = dy_ ? ay : 1.f - ay, wz = dz ? az : 1.f - az;
+                        const float4 v = __ldg(tp + (dz * S + dy_) * S + dx);
+                        const float gv = v.x * g.x + v.y * g.y + v.z * g.z + v.w * g.w;
+                        gx += (dx ? gv : -gv) * wy * wz;
+                        gy += (dy_ ? gv : -gv) * wx * wz;
+                        gz += (dz ? gv : -gv) * wx * wy;
+                        const float wgt = wx * wy * wz;
+                        if (live) atomicAdd(gtp + (dz * S + dy_) * S + dx, make_float4(g.x * wgt, g.y * wgt, g.z * wgt, g.w * wgt));
+                    }
+                    dy.x += gx * (0.5f * hs); dy.y += gy * (0.5f * hs); dy.z += gz * (0.5f * hs);
+                    // PrimTransfSRT::backward
+                    const float3 rx = p.r0 * xmt.x + p.r1 * xmt.y + p.r2 * xmt.z;
+                    gs[0] = rx.x * dy.x; gs[1] = rx.y * dy.y; gs[2] = rx.z * dy.z;
+                    dy = dy * p.s;
+                    gs[3] = xmt.x * dy.x; gs[4] = xmt.x * dy.y; gs[5] = xmt.x * dy.z;
+                    gs[6] = xmt.y * dy.x; gs[7] = xmt.y * dy.y; gs[8] = xmt.y * dy.z;
+                    gs[9] = xmt.z * dy.x; gs[10] = xmt.z * dy.y; gs[11] = xmt.z * dy.z;
+                    gs[12] = -dot3(p.r0, dy); gs[13] = -dot3(p.r1, dy); gs[14] = -dot3(p.r2, dy);
+                }
                 acc.x = fmaf(smp.x, contrib, acc.x); acc.y = fmaf(smp.y, contrib, acc.y); acc.z = fmaf(smp.z, contrib, acc.z); acc.w += contrib;
-                if (newalpha >= 1.f) done = true;
+                if (newalpha >= 1.f) {
+                    if (!GRAD) satrgb = make_float3(smp.x, smp.y, smp.z);
+                    done = true;
+                }
+            }
+            if (GRAD && __any_sync(0xffffffffu, eval)) {
+                // one warp-wide sum per partial; lane i < 15 then holds partial i and issues its reduction
+                float mine = 0.f;
+#pragma unroll
+                for (int i = 0; i < 15; ++i) {
+                    float v = gs[i];
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+                    if (lane == i) mine = v;
+                }
+                const size_t o = static_cast<size_t>(n) * a.K + k;
+                float* dst = lane < 3 ? a.grad_scale + o * 3 + lane : lane < 12 ? a.grad_rot + o * 9 + (lane - 3) : a.grad_pos + o * 3 + (lane - 12);
+                if (lane < 15 && mine != 0.f) atomicAdd(dst, mine);
             }
         }
         t += a.stepsize;
         pos = pos + raydir * a.stepsize;
     }
-    if (live) *reinterpret_cast<float4*>(a.out + ((static_cast<size_t>(n) * a.H + h) * a.W + w) * 4) = acc;
+    if (!GRAD && live) {
+        *reinterpret_cast<float4*>(a.out + pix * 4) = acc;
+        if (a.raysat) { a.raysat[pix * 3] = satrgb.x; a.raysat[pix * 3 + 1] = satrgb.y; a.raysat[pix * 3 + 2] = satrgb.z; }
+    }
+}
+
+int raymarch_check(const RayMarchArgs& a, int H, int W) {
+    TPX_CHECK(a.tpl != nullptr && a.primpos != nullptr && a.primrot != nullptr && a.primscale != nullptr && a.campos != nullptr && a.camrot != nullptr &&
+                  a.focal != nullptr && a.princpt != nullptr,
+              TPX_ERR_ARG, "raymarch: null argument");
+    TPX_CHECK(a.N > 0 && a.K > 0 && a.S >= 2 && a.S <= 64 && H > 0 && W > 0 && a.N <= 65535, TPX_ERR_SHAPE, "raymarch: bad geometry (N %d K %d S %d %d x %d)", a.N,
+              a.K, a.S, H, W);
+    TPX_CHECK(a.stride >= 1 && a.H >= 1 && a.W >= 1, TPX_ERR_SHAPE, "raymarch: stride %d leaves a %d x %d image of %d x %d", a.stride, a.H, a.W, H, W);
+    TPX_CHECK(a.stepsize > 0.f && a.volradius > 0.f, TPX_ERR_ARG, "raymarch: step size and volume radius must be positive");
+    TPX_CHECK((reinterpret_cast<uintptr_t>(a.tpl) & 15) == 0, TPX_ERR_ARG, "raymarch: template must be 16-B aligned");
+    return TPX_OK;
+}
+
+template <bool GRAD>
+int raymarch_launch(const RayMarchArgs& a, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ProfScope prof(PROF_VAE_MISC, st);
+    const dim3 grid((a.W + RM_BX - 1) / RM_BX, (a.H + RM_BY - 1) / RM_BY, a.N), block(RM_BX, RM_BY);
+    raymarch_kernel<GRAD><<<grid, block, 0, st>>>(a);
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
 }
 
 }  // namespace
@@ -219,18 +330,35 @@ using namespace tpx;
 extern "C" int tpx_raymarch_preview(const float* tpl, const float* primpos, const float* primrot, const float* primscale, const float* campos,
                                     const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius,
                                     float stepsize, float fadescale, float fadeexp, float* out, void* stream) {
-    TPX_CHECK(tpl != nullptr && primpos != nullptr && primrot != nullptr && primscale != nullptr && campos != nullptr && camrot != nullptr && focal != nullptr &&
-                  princpt != nullptr && out != nullptr,
-              TPX_ERR_ARG, "raymarch_preview: null argument");
-    TPX_CHECK(N > 0 && K > 0 && S >= 2 && S <= 64 && H > 0 && W > 0 && N <= 65535, TPX_ERR_SHAPE, "raymarch: bad geometry (N %d K %d S %d %d x %d)", N, K, S, H, W);
-    TPX_CHECK(stepsize > 0.f && volradius > 0.f, TPX_ERR_ARG, "raymarch: step size and volume radius must be positive");
-    TPX_CHECK((reinterpret_cast<uintptr_t>(tpl) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, TPX_ERR_ARG, "raymarch: template / output must be 16-B aligned");
+    return tpx_raymarch_forward(tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, N, K, S, H, W, volradius, stepsize, fadescale, fadeexp, 1,
+                                nullptr, out, nullptr, stream);
+}
+
+extern "C" int tpx_raymarch_forward(const float* tpl, const float* primpos, const float* primrot, const float* primscale, const float* campos,
+                                    const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius,
+                                    float stepsize, float fadescale, float fadeexp, int stride, const int* offsets, float* out, float* raysat_out, void* stream) {
+    const int h = stride >= 1 ? H / stride : 0, w = stride >= 1 ? W / stride : 0;
+    const RayMarchArgs a{tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, out, N, K, S, h, w, volradius, stepsize, fadescale, fadeexp,
+                         stride, offsets, raysat_out, nullptr, nullptr, nullptr, nullptr, nullptr};
+    TPX_CHECK(out != nullptr, TPX_ERR_ARG, "raymarch: null argument");
+    if (const int rc = raymarch_check(a, H, W)) return rc;
+    TPX_CHECK((reinterpret_cast<uintptr_t>(out) & 15) == 0, TPX_ERR_ARG, "raymarch: output must be 16-B aligned");
     TPX_DEVICE_GUARD();
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    ProfScope prof(PROF_VAE_MISC, st);
-    RayMarchArgs a{tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, out, N, K, S, H, W, volradius, stepsize, fadescale, fadeexp};
-    const dim3 grid((W + RM_BX - 1) / RM_BX, (H + RM_BY - 1) / RM_BY, N), block(RM_BX, RM_BY);
-    raymarch_preview_kernel<<<grid, block, 0, st>>>(a);
-    TPX_LAUNCH_CHECK();
-    return TPX_OK;
+    return raymarch_launch<false>(a, stream);
+}
+
+extern "C" int tpx_raymarch_backward(const float* tpl, const float* primpos, const float* primrot, const float* primscale, const float* campos,
+                                     const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius,
+                                     float stepsize, float fadescale, float fadeexp, int stride, const int* offsets, const float* raysat,
+                                     const float* grad_rgba, float* grad_tpl, float* grad_primpos, float* grad_primrot, float* grad_primscale, void* stream) {
+    const int h = stride >= 1 ? H / stride : 0, w = stride >= 1 ? W / stride : 0;
+    const RayMarchArgs a{tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, nullptr, N, K, S, h, w, volradius, stepsize, fadescale, fadeexp,
+                         stride, offsets, const_cast<float*>(raysat), grad_rgba, grad_tpl, grad_primpos, grad_primrot, grad_primscale};
+    TPX_CHECK(raysat != nullptr && grad_rgba != nullptr && grad_tpl != nullptr && grad_primpos != nullptr && grad_primrot != nullptr && grad_primscale != nullptr,
+              TPX_ERR_ARG, "raymarch: null argument");
+    if (const int rc = raymarch_check(a, H, W)) return rc;
+    TPX_CHECK((reinterpret_cast<uintptr_t>(grad_rgba) & 15) == 0 && (reinterpret_cast<uintptr_t>(grad_tpl) & 15) == 0, TPX_ERR_ARG,
+              "raymarch: output gradient / template gradient must be 16-B aligned");
+    TPX_DEVICE_GUARD();
+    return raymarch_launch<true>(a, stream);
 }

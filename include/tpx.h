@@ -284,6 +284,34 @@ int tpx_primsdf_sdf_grid(const float* coords_dev, int R, const float* srt_dev, c
 int tpx_raymarch_preview(const float* template_chlast, const float* primpos, const float* primrot, const float* primscale, const float* campos,
                          const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius, float stepsize,
                          float fadescale, float fadeexp, float* rgba_out, void* stream);
+/* The same march, saving what the backward needs (MVPRaymarch.forward with gradmode, dva/mvp/extensions/mvpraymarch/mvpraymarch.py:
+ * 74-150), with subsampled rays (dva/ray_marcher.py:33-73,174-190).  Arguments as tpx_raymarch_preview, plus:
+ *   stride >= 1 (ray_subsample_factor): rgba_out is [N,h,w,4] with h = H / stride, w = W / stride (h, w >= 1), and output pixel (j,i)
+ *   traces the ray through image pixel (x0 + stride j, y0 + stride i) -- the pixel_coords that subsample_pixel_coords /
+ *   resize_pixel_coords hand to compute_raydirs; the hit list is per warp of 8 x 4 OUTPUT pixels, as the reference's;
+ *   offsets: device int32 [N,2] per-image (x0, y0), each in [0, stride) (read by the kernel, not checked here), or NULL for (0, 0);
+ *   raysat_out: device fp32 [N,h,w,3] or NULL: PrimAccumAdditive's saturation colour (primaccum.h:63-79), the rgb of the first sample
+ *   whose accumulated alpha reaches 1, or (-1,-1,-1) if the ray never saturates.
+ * With stride 1, offsets NULL and raysat_out NULL the image is tpx_raymarch_preview's, bit for bit. */
+int tpx_raymarch_forward(const float* template_chlast, const float* primpos, const float* primrot, const float* primscale, const float* campos,
+                         const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius, float stepsize,
+                         float fadescale, float fadeexp, int stride, const int* offsets, float* rgba_out, float* raysat_out, void* stream);
+/* Backward of tpx_raymarch_forward (MVPRaymarch.backward, mvpraymarch.py:152-213 -> raymarch_subset_backward_kernel with forwarddir,
+ * mvpraymarch_subset_kernel.h:103-217, primaccum.h:81-98, primsampler.h:68-91, primtransf.h:155-179).  Inputs: the forward's, its
+ * raysat [N,h,w,3] and grad_rgba [N,h,w,4] (16-B aligned).  ADDS into caller-zeroed grad_template (channels-last [N,K,S,S,S,4], 16-B
+ * aligned), grad_primpos [N,K,3] (per unit of primpos / volradius, the units the march sees), grad_primrot [N,K,3,3] and
+ * grad_primscale [N,K,3].  The ray's march is repeated from the same first step through the same device code, so every inside test,
+ * saturation and step count is the forward's.  Per listed primitive and step, with acc the alpha accumulated before the sample:
+ *   sat = acc + a dt >= 1; dL_rgb = (sat ? 1 - acc : a dt) dL.rgb; dL_a = sat ? 0 : dt ((rgb,1) - (raysat valid ? (raysat,1) : 0)) . dL;
+ *   dL_y += -fadescale fadeexp |y|^(fadeexp-1) sign(y) a dL_a; the template gets the trilinear scatter of (dL_rgb, fade dL_a) and
+ *   dL_y the trilinear weights' derivative x (S-1)/2; grad_scale += (R^T (x - t)) * dL_y; dL_y *= s; grad_rot[r] += (x - t)[r] dL_y;
+ *   grad_pos -= R dL_y.
+ * Camera gradients are not computed (the reference returns None for them).  Floating-point atomics: the summation order, and so the
+ * last bits of the gradients, vary from run to run. */
+int tpx_raymarch_backward(const float* template_chlast, const float* primpos, const float* primrot, const float* primscale, const float* campos,
+                          const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius, float stepsize,
+                          float fadescale, float fadeexp, int stride, const int* offsets, const float* raysat, const float* grad_rgba,
+                          float* grad_template, float* grad_primpos, float* grad_primrot, float* grad_primscale, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Marching cubes — the `mcubes.marching_cubes(grid, 0.0)` call of extract_texmesh (inference.py:106-124), which copies the SDF grid
