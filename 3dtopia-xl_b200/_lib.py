@@ -83,6 +83,7 @@ SIGNATURES = {
     "tpx_primsdf_grid_bytes": (_sz, [_i64]),
     "tpx_primsdf_grid_build": (_i, [_vp, _i, _vp, _sz, _vp]),
     "tpx_primsdf_query_grid": (_i, [_vp, _vp, _vp, _vp, _sz, _i64, _i, _i, _i, _i, _vp, _vp]),
+    "tpx_primsdf_query_backward": (_i, [_vp, _vp, _vp, _vp, _sz, _i64, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "tpx_primsdf_sdf_grid": (_i, [_vp, _i, _vp, _vp, _vp, _sz, _i, _i, _i, _i, _vp, _vp]),
     "tpx_raymarch_preview": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _f, _vp, _vp]),
     "tpx_raymarch_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _f, _i, _vp, _vp, _vp, _vp]),

@@ -23,39 +23,86 @@ struct PointAcc {
     float wsum;
 };
 
-// visit primitive k for the point (px,py,pz): box weight, and — if it covers the point — its trilinear sample
-template <int NC, int DF>
-__device__ __forceinline__ void visit_prim(PointAcc<NC>& a, float px, float py, float pz, const float4 v /* scale, tx, ty, tz */, int k,
-                                           const float* __restrict__ feat, int S, int S3, float half_span) {
+// box weight w = 1 - |l|_inf of primitive v (scale, tx, ty, tz) at the point, and the local position l = (x - pos) / scale it was
+// decided on.  The point and the backward decide coverage (w > 0) here and nowhere else.
+__device__ __forceinline__ float prim_box(float px, float py, float pz, const float4 v, float& lx, float& ly, float& lz) {
     const float inv = 1.0f / v.x;
     const float dx = px - v.y, dy = py - v.z, dz = pz - v.w;
-    float lx = __fmul_rn(dx, inv), ly = __fmul_rn(dy, inv), lz = __fmul_rn(dz, inv);
+    lx = __fmul_rn(dx, inv); ly = __fmul_rn(dy, inv); lz = __fmul_rn(dz, inv);
     float w = 1.0f - fmaxf(fabsf(lx), fmaxf(fabsf(ly), fabsf(lz)));
     if (fabsf(w) < 1e-5f) {   // on the box boundary: decide with the reference's exact division, not the reciprocal
         lx = dx / v.x; ly = dy / v.x; lz = dz / v.x;
         w = 1.0f - fmaxf(fabsf(lx), fmaxf(fabsf(ly), fabsf(lz)));
     }
+    return w;
+}
+
+// trilinear cell of a covered local position in feat[k] viewed as [DF, D(z), H(y), W(x)], align_corners=True; |l| < 1 so no
+// padding case.  off is the flat offset of the (x0, y0, z0) corner, a = the fractions along x, y, z.
+struct TriCell {
+    int off;
+    float ax, ay, az;
+};
+__device__ __forceinline__ TriCell tri_cell(float lx, float ly, float lz, int S, float half_span) {
+    const float fx = (lx + 1.0f) * half_span, fy = (ly + 1.0f) * half_span, fz = (lz + 1.0f) * half_span;
+    const int x0 = min(static_cast<int>(fx), S - 2), y0 = min(static_cast<int>(fy), S - 2), z0 = min(static_cast<int>(fz), S - 2);
+    return TriCell{(z0 * S + y0) * S + x0, fx - x0, fy - y0, fz - z0};
+}
+
+// Every product is rounded or fused as written (no compiler contraction), so the sdf channel comes out bit-identical whether one
+// channel (the SDF grid) or all six (the point query) are accumulated: u (1 - t) + v t = fma(1 - t, u, t v).
+__device__ __forceinline__ float tri_sample(const float* __restrict__ fc, const TriCell& t, int S) {
+    const float bx = 1.f - t.ax, by = 1.f - t.ay, bz = 1.f - t.az;
+    const float c00 = __fmaf_rn(bx, fc[0], __fmul_rn(t.ax, fc[1]));
+    const float c01 = __fmaf_rn(bx, fc[S], __fmul_rn(t.ax, fc[S + 1]));
+    const float c10 = __fmaf_rn(bx, fc[S * S], __fmul_rn(t.ax, fc[S * S + 1]));
+    const float c11 = __fmaf_rn(bx, fc[S * S + S], __fmul_rn(t.ax, fc[S * S + S + 1]));
+    return __fmaf_rn(bz, __fmaf_rn(by, c00, __fmul_rn(t.ay, c01)), __fmul_rn(t.az, __fmaf_rn(by, c10, __fmul_rn(t.ay, c11))));
+}
+
+// visit primitive k for the point (px,py,pz): box weight, and — if it covers the point — its trilinear sample
+template <int NC, int DF>
+__device__ __forceinline__ void visit_prim(PointAcc<NC>& a, float px, float py, float pz, const float4 v /* scale, tx, ty, tz */, int k,
+                                           const float* __restrict__ feat, int S, int S3, float half_span) {
+    float lx, ly, lz;
+    const float w = prim_box(px, py, pz, v, lx, ly, lz);
     if (w > 0.f) {
         a.wsum += w;
-        // trilinear sample of feat[k] viewed as [DF, D(z), H(y), W(x)], align_corners=True; |l| < 1 so no padding case
-        const float fx = (lx + 1.0f) * half_span, fy = (ly + 1.0f) * half_span, fz = (lz + 1.0f) * half_span;
-        const int x0 = min(static_cast<int>(fx), S - 2), y0 = min(static_cast<int>(fy), S - 2), z0 = min(static_cast<int>(fz), S - 2);
-        const float ax = fx - x0, ay = fy - y0, az = fz - z0;
-        const float bx = 1.f - ax, by = 1.f - ay, bz = 1.f - az;
-        const float* f = feat + static_cast<size_t>(k) * DF * S3 + (z0 * S + y0) * S + x0;
-        // Every product is rounded or fused as written (no compiler contraction), so the sdf channel comes out bit-identical
-        // whether one channel (the SDF grid) or all six (the point query) are accumulated: u (1 - t) + v t = fma(1 - t, u, t v).
+        const TriCell t = tri_cell(lx, ly, lz, S, half_span);
+        const float* f = feat + static_cast<size_t>(k) * DF * S3 + t.off;
 #pragma unroll
-        for (int c = 0; c < NC; ++c) {
-            const float* fc = f + c * S3;
-            const float c00 = __fmaf_rn(bx, fc[0], __fmul_rn(ax, fc[1]));
-            const float c01 = __fmaf_rn(bx, fc[S], __fmul_rn(ax, fc[S + 1]));
-            const float c10 = __fmaf_rn(bx, fc[S * S], __fmul_rn(ax, fc[S * S + 1]));
-            const float c11 = __fmaf_rn(bx, fc[S * S + S], __fmul_rn(ax, fc[S * S + S + 1]));
-            const float val = __fmaf_rn(bz, __fmaf_rn(by, c00, __fmul_rn(ay, c01)), __fmul_rn(az, __fmaf_rn(by, c10, __fmul_rn(ay, c11))));
-            a.acc[c] = fmaf(w, val, a.acc[c]);
-        }
+        for (int c = 0; c < NC; ++c) a.acc[c] = fmaf(w, tri_sample(f + c * S3, t, S), a.acc[c]);
     }
+}
+
+// Nearest voxel of primitive v to an uncovered point (inference).  It is one of the 2x2x2 lattice neighbours of the (clamped) local
+// position.  They are ranked the way the reference ranks all S^3 candidates (primsdf.py:93-96): fp32 L2 distance to pos + scale *
+// linspace grid, first flat index wins a tie — a far point often has two candidates whose fp32 distances coincide.  e = x - voxel.
+struct NearVoxel {
+    int xi, yi, zi;
+    float dist, ex, ey, ez;
+};
+__device__ __forceinline__ float lin_coord(int i, int S) {   // torch.linspace(-1, 1, S)[i]
+    const float step = 2.0f / static_cast<float>(S - 1);
+    return i < S / 2 ? -1.f + step * static_cast<float>(i) : 1.f - step * static_cast<float>(S - 1 - i);
+}
+__device__ __forceinline__ NearVoxel nearest_voxel(float px, float py, float pz, const float4 v, int S, float half_span) {
+    const float sc = v.x;
+    const float lx = (px - v.y) / sc, ly = (py - v.z) / sc, lz = (pz - v.w) / sc;
+    const int x0 = min(max(static_cast<int>(floorf((lx + 1.f) * half_span)), 0), S - 2);
+    const int y0 = min(max(static_cast<int>(floorf((ly + 1.f) * half_span)), 0), S - 2);
+    const int z0 = min(max(static_cast<int>(floorf((lz + 1.f) * half_span)), 0), S - 2);
+    NearVoxel r{x0, y0, z0, INFINITY, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        const int cz = z0 + (c >> 2), cy = y0 + ((c >> 1) & 1), cx = x0 + (c & 1);
+        const float ex = px - __fadd_rn(v.y, __fmul_rn(sc, lin_coord(cx, S)));
+        const float ey = py - __fadd_rn(v.z, __fmul_rn(sc, lin_coord(cy, S)));
+        const float ez = pz - __fadd_rn(v.w, __fmul_rn(sc, lin_coord(cz, S)));
+        const float d = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez)));
+        if (d < r.dist) r = NearVoxel{cx, cy, cz, d, ex, ey, ez};
+    }
+    return r;
 }
 
 template <int NC, int DF>
@@ -73,30 +120,10 @@ __device__ __forceinline__ void finish_point(const PointAcc<NC>& a, float px, fl
     if (inference && K > 0) {
         // SDF of an uncovered point: nearest voxel of the nearest primitive, same sign, plus the L2 distance to it
         const float4 v = *reinterpret_cast<const float4*>(srt + 4 * static_cast<size_t>(best_k));
-        const float sc = v.x;
-        const float lx = (px - v.y) / sc, ly = (py - v.z) / sc, lz = (pz - v.w) / sc;
-        // The nearest voxel is one of the 2x2x2 lattice neighbours of the (clamped) local position.  They are ranked the
-        // way the reference ranks all S^3 candidates (primsdf.py:93-96): fp32 L2 distance to pos + scale * linspace
-        // grid, first flat index wins a tie — a far point often has two candidates whose fp32 distances coincide.
-        const int x0 = min(max(static_cast<int>(floorf((lx + 1.f) * half_span)), 0), S - 2);
-        const int y0 = min(max(static_cast<int>(floorf((ly + 1.f) * half_span)), 0), S - 2);
-        const int z0 = min(max(static_cast<int>(floorf((lz + 1.f) * half_span)), 0), S - 2);
-        const float step = 2.0f / static_cast<float>(S - 1);
-        auto lin = [&](int i) { return i < S / 2 ? -1.f + step * static_cast<float>(i) : 1.f - step * static_cast<float>(S - 1 - i); };  // torch.linspace
-        float dist = INFINITY;
-        int xi = x0, yi = y0, zi = z0;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-            const int cz = z0 + (c >> 2), cy = y0 + ((c >> 1) & 1), cx = x0 + (c & 1);
-            const float ex = px - __fadd_rn(v.y, __fmul_rn(sc, lin(cx)));
-            const float ey = py - __fadd_rn(v.z, __fmul_rn(sc, lin(cy)));
-            const float ez = pz - __fadd_rn(v.w, __fmul_rn(sc, lin(cz)));
-            const float d = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez)));
-            if (d < dist) { dist = d; xi = cx; yi = cy; zi = cz; }
-        }
-        const float sdf = feat[static_cast<size_t>(best_k) * DF * S3 + (zi * S + yi) * S + xi];
+        const NearVoxel nv = nearest_voxel(px, py, pz, v, S, half_span);
+        const float sdf = feat[static_cast<size_t>(best_k) * DF * S3 + (nv.zi * S + nv.yi) * S + nv.xi];
         const float sgn = sdf > 0.f ? 1.f : (sdf < 0.f ? -1.f : 0.f);
-        o[0] = sdf + dist * sgn;
+        o[0] = sdf + nv.dist * sgn;
     }
 }
 
@@ -261,19 +288,16 @@ __global__ void __launch_bounds__(1024) grid_scan_kernel(const int* __restrict__
     }
 }
 
-// one point of the binned query; hdr == nullptr (no grid) takes the exhaustive loop
-template <int NC, int DF>
-__device__ __forceinline__ void query_point_binned(float px, float py, float pz, const float* __restrict__ srt, const float* __restrict__ feat,
-                                                   const GridHdr* __restrict__ hdr, const int* __restrict__ offsets, const int* __restrict__ entries, int K,
-                                                   int S, int inference, float* __restrict__ o) {
-    PointAcc<NC> a;
-#pragma unroll
-    for (int c = 0; c < NC; ++c) a.acc[c] = 0.f;
-    a.wsum = 0.f;
+// The walk of one point: every primitive (no grid, a point outside it or an over-full grid) or the cover list of the point's cell,
+// in ascending k, calling visit(k, srt[k]) on each; then, only on a cell walk where covered() is false and `nearest` is set, the
+// cell's near list.  Returns the nearest centre (strict <, ascending k: the first of equals) over the primitives scanned for it.
+// The query and its backward both walk through here, so a (point, primitive) pair counts in both or in neither.
+template <class Visit, class Covered>
+__device__ __forceinline__ int walk_point(float px, float py, float pz, const float* __restrict__ srt, const GridHdr* __restrict__ hdr,
+                                          const int* __restrict__ offsets, const int* __restrict__ entries, int K, bool nearest, Visit&& visit,
+                                          Covered&& covered) {
     float best_d2 = INFINITY;
     int best_k = 0;
-    const int S3 = S * S * S;
-    const float half_span = 0.5f * static_cast<float>(S - 1);
     bool inside = false;
     int cell = 0;
     if (hdr != nullptr) {
@@ -288,16 +312,16 @@ __device__ __forceinline__ void query_point_binned(float px, float py, float pz,
             const float dx = px - p.y, dy = py - p.z, dz = pz - p.w;
             const float d2 = dx * dx + dy * dy + dz * dz;
             if (d2 < best_d2) { best_d2 = d2; best_k = k; }
-            visit_prim<NC, DF>(a, px, py, pz, p, k, feat, S, S3, half_span);
+            visit(k, p);
         }
     } else {
         const int c0 = offsets[cell], c1 = offsets[cell + 1];
         for (int e = c0; e < c1; ++e) {
             const int k = entries[e];
             const float4 p = __ldg(reinterpret_cast<const float4*>(srt + 4 * static_cast<size_t>(k)));
-            visit_prim<NC, DF>(a, px, py, pz, p, k, feat, S, S3, half_span);
+            visit(k, p);
         }
-        if (!(a.wsum > 0.f) && inference) {
+        if (!covered() && nearest) {
             const int n0 = offsets[PG_CELLS + cell], n1 = offsets[PG_CELLS + cell + 1];
             for (int e = n0; e < n1; ++e) {
                 const int k = entries[e];
@@ -308,6 +332,23 @@ __device__ __forceinline__ void query_point_binned(float px, float py, float pz,
             }
         }
     }
+    return best_k;
+}
+
+// one point of the binned query; hdr == nullptr (no grid) takes the exhaustive loop
+template <int NC, int DF>
+__device__ __forceinline__ void query_point_binned(float px, float py, float pz, const float* __restrict__ srt, const float* __restrict__ feat,
+                                                   const GridHdr* __restrict__ hdr, const int* __restrict__ offsets, const int* __restrict__ entries, int K,
+                                                   int S, int inference, float* __restrict__ o) {
+    PointAcc<NC> a;
+#pragma unroll
+    for (int c = 0; c < NC; ++c) a.acc[c] = 0.f;
+    a.wsum = 0.f;
+    const int S3 = S * S * S;
+    const float half_span = 0.5f * static_cast<float>(S - 1);
+    const int best_k = walk_point(
+        px, py, pz, srt, hdr, offsets, entries, K, inference != 0,
+        [&](int k, const float4 p) { visit_prim<NC, DF>(a, px, py, pz, p, k, feat, S, S3, half_span); }, [&] { return a.wsum > 0.f; });
     finish_point<NC, DF>(a, px, py, pz, best_k, srt, feat, K, S, S3, half_span, inference, o);
 }
 
@@ -319,6 +360,120 @@ __global__ void __launch_bounds__(PS_THREADS) primsdf_query_grid_kernel(const fl
     const long long i = static_cast<long long>(blockIdx.x) * PS_THREADS + threadIdx.x;
     if (i >= n) return;
     query_point_binned<DF, DF>(x[3 * i], x[3 * i + 1], x[3 * i + 2], srt, feat, hdr, offsets, entries, K, S, inference, out + static_cast<size_t>(i) * DF);
+}
+
+// =====================================================================================================================
+// Backward of the point query (models/primsdf.py:52-109 under autograd; the loss of dva/losses.py:102-148 fits through it).
+// One thread per point, walking exactly the primitives the forward walked (walk_point, prim_box, nearest_voxel):
+//   pass 1: the forward's wsum, raw normalised output o_c and nearest-primitive choice, with its arithmetic;
+//   the upstream gradient g of channels 1..5 is zeroed where o_c lies outside [0, 1] (torch.clip passes the bounds);
+//   pass 2: the covering primitives again, emitting with W = wsum + 1e-6:
+//     dL/dv_jc = g_c w_j / W, scattered to the 8 trilinear corners of channel c of feat[j];
+//     dL/dw_j = sum_c g_c (v_jc - o_c) / W;
+//     dL/dl_j = sum_c (g_c w_j / W) dv_jc/dl - dL/dw_j sign(l_jd) [|l_jd| = max] / (tied axes);
+//     dL/dx += dL/dl_j / s_j, dL/dpos_j -= dL/dl_j / s_j, dL/ds_j -= (dL/dl_j . l_j) / s_j.
+//   An uncovered point at inference (sdf = f + d sign(f), d = |x - c|, c the nearest voxel, u = (x - c) / d, 0 at d = 0):
+//     dL/dfeat_geo[k,v] += g_0, dL/dx += g_0 sign(f) u, dL/dpos_k -= g_0 sign(f) u, dL/ds_k -= g_0 sign(f) (u . grid_v).
+// grad_x is owned by the point's thread; grad_srt / grad_feat are fp32 reductions (RED.E.ADD.F32), so their last bits depend on
+// the order in which points arrive.  Any of the three may be null.  Two blocks per SM cap the registers at 128 without spills.
+// =====================================================================================================================
+template <int DF>
+__global__ void __launch_bounds__(PS_THREADS, 2) primsdf_backward_kernel(const float* __restrict__ x, const float* __restrict__ srt, const float* __restrict__ feat,
+                                                                      const GridHdr* __restrict__ hdr, const int* __restrict__ offsets,
+                                                                      const int* __restrict__ entries, long long n, int K, int S, int inference,
+                                                                      const float* __restrict__ grad_out, float* __restrict__ grad_x,
+                                                                      float* __restrict__ grad_srt, float* __restrict__ grad_feat) {
+    const long long i = static_cast<long long>(blockIdx.x) * PS_THREADS + threadIdx.x;
+    if (i >= n) return;
+    const float px = x[3 * i], py = x[3 * i + 1], pz = x[3 * i + 2];
+    const int S3 = S * S * S;
+    const float half_span = 0.5f * static_cast<float>(S - 1);
+    PointAcc<DF> a;
+#pragma unroll
+    for (int c = 0; c < DF; ++c) a.acc[c] = 0.f;
+    a.wsum = 0.f;
+    const int best_k = walk_point(
+        px, py, pz, srt, hdr, offsets, entries, K, inference != 0,
+        [&](int k, const float4 p) { visit_prim<DF, DF>(a, px, py, pz, p, k, feat, S, S3, half_span); }, [&] { return a.wsum > 0.f; });
+    float g[DF];
+#pragma unroll
+    for (int c = 0; c < DF; ++c) g[c] = grad_out[static_cast<size_t>(i) * DF + c];
+    float gpx = 0.f, gpy = 0.f, gpz = 0.f;
+    if (a.wsum > 0.f) {
+        const float inv = 1.0f / (a.wsum + 1e-6f);
+        float o[DF];
+#pragma unroll
+        for (int c = 0; c < DF; ++c) {
+            o[c] = a.acc[c] * inv;
+            if (c > 0 && !(o[c] >= 0.f && o[c] <= 1.f)) g[c] = 0.f;
+        }
+        walk_point(
+            px, py, pz, srt, hdr, offsets, entries, K, false,
+            [&](int k, const float4 p) {
+                float lx, ly, lz;
+                const float w = prim_box(px, py, pz, p, lx, ly, lz);
+                if (!(w > 0.f)) return;
+                const TriCell t = tri_cell(lx, ly, lz, S, half_span);
+                const float bx = 1.f - t.ax, by = 1.f - t.ay, bz = 1.f - t.az;
+                const size_t base = static_cast<size_t>(k) * DF * S3 + t.off;
+                const float wn = w * inv;
+                float gw = 0.f, dax = 0.f, day = 0.f, daz = 0.f;   // dL/dw_j * W and dL/d(ax, ay, az)
+#pragma unroll
+                for (int c = 0; c < DF; ++c) {
+                    const float* fc = feat + base + static_cast<size_t>(c) * S3;
+                    const float f000 = fc[0], f001 = fc[1], f010 = fc[S], f011 = fc[S + 1];
+                    const float f100 = fc[S * S], f101 = fc[S * S + 1], f110 = fc[S * S + S], f111 = fc[S * S + S + 1];
+                    const float c00 = bx * f000 + t.ax * f001, c01 = bx * f010 + t.ax * f011;
+                    const float c10 = bx * f100 + t.ax * f101, c11 = bx * f110 + t.ax * f111;
+                    const float e0 = by * c00 + t.ay * c01, e1 = by * c10 + t.ay * c11;
+                    gw += g[c] * ((bz * e0 + t.az * e1) - o[c]);
+                    const float gv = g[c] * wn;
+                    if (gv == 0.f) continue;
+                    dax += gv * (bz * (by * (f001 - f000) + t.ay * (f011 - f010)) + t.az * (by * (f101 - f100) + t.ay * (f111 - f110)));
+                    day += gv * (bz * (c01 - c00) + t.az * (c11 - c10));
+                    daz += gv * (e1 - e0);
+                    if (grad_feat != nullptr) {
+                        float* gf = grad_feat + base + static_cast<size_t>(c) * S3;
+                        atomicAdd(gf, gv * bz * by * bx);                 atomicAdd(gf + 1, gv * bz * by * t.ax);
+                        atomicAdd(gf + S, gv * bz * t.ay * bx);           atomicAdd(gf + S + 1, gv * bz * t.ay * t.ax);
+                        atomicAdd(gf + S * S, gv * t.az * by * bx);       atomicAdd(gf + S * S + 1, gv * t.az * by * t.ax);
+                        atomicAdd(gf + S * S + S, gv * t.az * t.ay * bx); atomicAdd(gf + S * S + S + 1, gv * t.az * t.ay * t.ax);
+                    }
+                }
+                // the inf-norm's derivative splits a tie evenly between the tied axes; at the centre (l = 0) it is 0
+                const float m = fmaxf(fabsf(lx), fmaxf(fabsf(ly), fabsf(lz)));
+                const bool tx = fabsf(lx) == m, ty = fabsf(ly) == m, tz = fabsf(lz) == m;
+                const float q = gw * inv / static_cast<float>(static_cast<int>(tx) + static_cast<int>(ty) + static_cast<int>(tz));
+                const float is = 1.0f / p.x;
+                const float glx = (dax * half_span - (tx && lx != 0.f ? (lx > 0.f ? q : -q) : 0.f)) * is;
+                const float gly = (day * half_span - (ty && ly != 0.f ? (ly > 0.f ? q : -q) : 0.f)) * is;
+                const float glz = (daz * half_span - (tz && lz != 0.f ? (lz > 0.f ? q : -q) : 0.f)) * is;
+                gpx += glx; gpy += gly; gpz += glz;
+                if (grad_srt != nullptr) {
+                    float* gs = grad_srt + 4 * static_cast<size_t>(k);
+                    atomicAdd(gs, -(glx * lx + gly * ly + glz * lz));
+                    atomicAdd(gs + 1, -glx); atomicAdd(gs + 2, -gly); atomicAdd(gs + 3, -glz);
+                }
+            },
+            [] { return true; });
+    } else if (inference && K > 0) {
+        const float4 v = *reinterpret_cast<const float4*>(srt + 4 * static_cast<size_t>(best_k));
+        const NearVoxel nv = nearest_voxel(px, py, pz, v, S, half_span);
+        const size_t vi = static_cast<size_t>(best_k) * DF * S3 + (nv.zi * S + nv.yi) * S + nv.xi;
+        const float f = feat[vi];
+        if (grad_feat != nullptr && g[0] != 0.f) atomicAdd(grad_feat + vi, g[0]);
+        const float h = (f > 0.f ? g[0] : (f < 0.f ? -g[0] : 0.f)) / nv.dist;       // g_0 sign(f) / d
+        if (nv.dist > 0.f && h != 0.f) {
+            const float ux = h * nv.ex, uy = h * nv.ey, uz = h * nv.ez;
+            gpx = ux; gpy = uy; gpz = uz;
+            if (grad_srt != nullptr) {
+                float* gs = grad_srt + 4 * static_cast<size_t>(best_k);
+                atomicAdd(gs, -(ux * lin_coord(nv.xi, S) + uy * lin_coord(nv.yi, S) + uz * lin_coord(nv.zi, S)));
+                atomicAdd(gs + 1, -ux); atomicAdd(gs + 2, -uy); atomicAdd(gs + 3, -uz);
+            }
+        }
+    }
+    if (grad_x != nullptr) { grad_x[3 * i] += gpx; grad_x[3 * i + 1] += gpy; grad_x[3 * i + 2] += gpz; }
 }
 
 // sdf channel of the query on the R^3 lattice (coords[i], coords[j], coords[k]); grid[(i R + j) R + k] (inference.py:108-116:
@@ -448,6 +603,27 @@ int tpx_primsdf_query_grid(const float* x, const float* srt, const float* feat, 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     ProfScope prof(PROF_VAE_MISC, st);
     primsdf_query_grid_kernel<6><<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(x, srt, feat, g.hdr, g.offsets, g.entries, n, K, S, inference, out);
+    TPX_LAUNCH_CHECK();
+    return TPX_OK;
+}
+
+int tpx_primsdf_query_backward(const float* x, const float* srt, const float* feat, const void* grid_ws, size_t grid_bytes, int64_t n, int K, int S,
+                               int dim_feat, int inference, const float* grad_out, float* grad_x, float* grad_srt, float* grad_feat, void* stream) {
+    if (n == 0) return TPX_OK;
+    TPX_CHECK(n > 0 && x != nullptr && srt != nullptr && feat != nullptr && grad_out != nullptr, TPX_ERR_ARG,
+              "primsdf_query_backward: null argument or negative n");
+    TPX_CHECK(dim_feat == 6, TPX_ERR_SHAPE, "primsdf_query_backward: dim_feat %d (kernel covers the released 6-channel layout)", dim_feat);
+    TPX_CHECK(S >= 2 && S <= 32 && K >= 0 && (K > 0 || grid_ws == nullptr), TPX_ERR_SHAPE, "primsdf_query_backward: bad primitive geometry (S %d, K %d)", S, K);
+    TPX_CHECK((reinterpret_cast<uintptr_t>(srt) & 15) == 0, TPX_ERR_ARG, "primsdf_query_backward: srt must be 16-B aligned");
+    const long long blocks = (n + PS_THREADS - 1) / PS_THREADS;
+    TPX_CHECK(blocks < (1LL << 31), TPX_ERR_SHAPE, "primsdf_query_backward: too many points");
+    TPX_DEVICE_GUARD();
+    if (grad_x == nullptr && grad_srt == nullptr && grad_feat == nullptr) return TPX_OK;
+    const GridPtrs g = grid_carve(grid_ws, grid_bytes);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ProfScope prof(PROF_VAE_MISC, st);
+    primsdf_backward_kernel<6><<<static_cast<unsigned>(blocks), PS_THREADS, 0, st>>>(x, srt, feat, g.hdr, g.offsets, g.entries, n, K, S, inference, grad_out,
+                                                                                     grad_x, grad_srt, grad_feat);
     TPX_LAUNCH_CHECK();
     return TPX_OK;
 }

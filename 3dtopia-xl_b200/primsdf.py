@@ -6,6 +6,12 @@ kwargs (configs/inference_dit.yml:22-30), the same two parameters ``srt_param [K
 ``forward(x[n,3]) -> {"sdf","tex","mat"}``.  The reference evaluates a dense [points x prims] weight matrix per 8192-point
 chunk; the kernel visits every primitive per point in registers and samples only the covering ones.
 Mesh-based initialisation (``_init_param``) is training-time and absent, as in the released reference (it is ``pass``).
+
+Gradients: with ``differentiable=True``, autograd on, and any of ``x`` / ``srt_param`` / ``feat_param`` requiring grad, ``forward`` runs
+as a ``torch.autograd.Function`` over the same query kernel and ``tpx_primsdf_query_backward``, so ``PrimSDFLoss``-style fitting
+(dva/losses.py:102-148) and ``d sdf / d x`` (the field's normal) work through it.  Its outputs are bit-identical to the no-grad path's.
+The backward is once-differentiable: a second derivative (``PrimSDFLoss``'s ``grad_l2`` term) raises.  Without ``differentiable``, every
+call returns detached outputs, as before.  ``sdf_grid``, ``bake_texture`` and the ``extract_*`` methods carry no gradient.
 """
 from __future__ import annotations
 
@@ -13,14 +19,53 @@ import math
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib, bake, mesh, unwrap
 
 
+class _PrimSDFFunction(torch.autograd.Function):
+    """PrimSDF.forward (models/primsdf.py:52-109) under autograd: x [n,3], srt [K,4], feat [K, 6 S^3] in any float dtype -> fp32
+    [n,6] = (sdf, rgb, roughness, metallic), with ``module`` supplying prim_shape, training (the uncovered-point fill) and the
+    grid cache.  The backward walks the workspace the forward used (kept on ctx: the module may rebuild its grid before backward runs)."""
+
+    @staticmethod
+    def forward(ctx, x, srt_param, feat_param, module):
+        xx, srt, feat = (t.detach().float().contiguous() for t in (x, srt_param, feat_param))
+        out, ws = module._query(xx, srt, feat)
+        ctx.save_for_backward(x, srt_param, feat_param)
+        ctx.ws, ctx.S, ctx.dim_feat, ctx.inference = ws, module.prim_shape, module.dim_feat, 0 if module.training else 1
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        if torch.is_grad_enabled():       # create_graph=True: a graph of the gradient was asked for
+            raise RuntimeError("PrimSDF's backward is once_differentiable: a second derivative (create_graph=True, e.g. a loss on "
+                               "d sdf / d x) is not supported")
+        return _PrimSDFFunction._backward(ctx, grad_out)
+
+    @staticmethod
+    @once_differentiable
+    def _backward(ctx, grad_out):
+        x, srt_param, feat_param = ctx.saved_tensors
+        xx, srt, feat = (t.detach().float().contiguous() for t in (x, srt_param, feat_param))
+        need = ctx.needs_input_grad[:3]
+        gx, gs, gf = (torch.zeros_like(t) if nd else None for t, nd in zip((xx, srt, feat), need))
+        g = grad_out.float().contiguous()
+        ws = ctx.ws
+        with torch.cuda.device(xx.device):
+            _lib.check(_lib.lib().tpx_primsdf_query_backward(xx.data_ptr(), srt.data_ptr(), feat.data_ptr(), _lib.ptr(ws), 0 if ws is None else ws.numel(),
+                                                             xx.shape[0], srt.shape[0], ctx.S, ctx.dim_feat, ctx.inference, g.data_ptr(), _lib.ptr(gx),
+                                                             _lib.ptr(gs), _lib.ptr(gf), _lib.stream_ptr()), "tpx_primsdf_query_backward")
+        return (None if gx is None else gx.to(x.dtype), None if gs is None else gs.to(srt_param.dtype),
+                None if gf is None else gf.to(feat_param.dtype), None)
+
+
 class PrimSDF(nn.Module):
     def __init__(self, mesh_obj=None, f_sdf=None, geo_fn=None, asset_list=None, num_prims=1024, dim_feat=6, prim_shape=8, init_scale=0.05,
-                 sdf2alpha_var=0.005, auto_scale_init=True, init_sampling="uniform", **_unused):
+                 sdf2alpha_var=0.005, auto_scale_init=True, init_sampling="uniform", differentiable=False, **_unused):
         super().__init__()
+        self.differentiable = differentiable   # forward records a graph (see _PrimSDFFunction) only when this is set
         self.num_prims, self.dim_feat, self.prim_shape = num_prims, dim_feat, prim_shape
         self.sdf2alpha_var = sdf2alpha_var
         self.auto_scale_init, self.init_sampling = auto_scale_init, init_sampling
@@ -39,12 +84,19 @@ class PrimSDF(nn.Module):
             raise ValueError(f"x must be [n,3], got {tuple(x.shape)}")
         if not x.is_cuda or not self.srt_param.is_cuda:
             raise _lib.TpxError("PrimSDF query runs on CUDA only (no CPU path): move the module and the points to the GPU")
+        if self.differentiable and torch.is_grad_enabled() and any(t.requires_grad for t in (x, self.srt_param, self.feat_param)):
+            out = _PrimSDFFunction.apply(x, self.srt_param, self.feat_param, self)
+        else:
+            out, _ = self._query(x.detach().float().contiguous(), self.srt_param.detach().float().contiguous(),
+                                 self.feat_param.detach().float().contiguous())
+        return {"sdf": out[:, 0:1], "tex": out[:, 1:4], "mat": out[:, 4:6]}
+
+    def _query(self, xx: torch.Tensor, srt: torch.Tensor, feat: torch.Tensor):
+        """fp32 [n, dim_feat] query of the fp32 contiguous points, and the grid workspace it walked (None: exhaustive kernel)."""
         lib = _lib.lib()
-        xx = x.detach().float().contiguous()
-        srt = self.srt_param.detach().float().contiguous()
-        feat = self.feat_param.detach().float().contiguous()
         n, K = xx.shape[0], srt.shape[0]
         out = torch.empty(n, self.dim_feat, dtype=torch.float32, device=xx.device)
+        ws = None
         with torch.cuda.device(xx.device):
             if K < 1 or K > 4096:      # outside the grid builder's range: exhaustive kernel
                 _lib.check(lib.tpx_primsdf_query(xx.data_ptr(), srt.data_ptr(), feat.data_ptr(), n, K, self.prim_shape, self.dim_feat,
@@ -53,7 +105,7 @@ class PrimSDF(nn.Module):
                 ws = self._grid_workspace(srt, K, xx.device)
                 _lib.check(lib.tpx_primsdf_query_grid(xx.data_ptr(), srt.data_ptr(), feat.data_ptr(), ws.data_ptr(), ws.numel(), n, K, self.prim_shape,
                                                       self.dim_feat, 0 if self.training else 1, out.data_ptr(), _lib.stream_ptr()), "tpx_primsdf_query_grid")
-        return {"sdf": out[:, 0:1], "tex": out[:, 1:4], "mat": out[:, 4:6]}
+        return out, ws
 
     def _grid_workspace(self, srt: torch.Tensor, K: int, device) -> torch.Tensor:
         """The binned lists of the current srt_param (tpx_primsdf_grid_build), rebuilt only when srt_param changes."""

@@ -263,6 +263,23 @@ size_t tpx_primsdf_grid_bytes(int64_t cap_entries);
 int tpx_primsdf_grid_build(const float* srt_dev, int K, void* grid_ws, size_t grid_bytes, void* stream);
 int tpx_primsdf_query_grid(const float* x_dev, const float* srt_dev, const float* feat_dev, const void* grid_ws, size_t grid_bytes, int64_t n, int K, int S,
                            int dim_feat, int inference, float* out_dev, void* stream);
+/* Backward of the point query: models/primsdf.py:52-109 under autograd, what PrimSDFLoss (dva/losses.py:102-148: SDF L1 in the
+ * shape phase, tex / mat L1 in the texture phase) fits primitives through.  Inputs as tpx_primsdf_query_grid, with grid_ws the
+ * workspace the forward used, or NULL for the exhaustive walk (the forward of K > 4096 primitives, tpx_primsdf_query);
+ * grad_out device fp32 [n,6], the upstream gradient of (sdf, rgb, roughness, metallic).  ADDS into caller-zeroed grad_x [n,3],
+ * grad_srt [K,4] and grad_feat [K,6*S^3]; each may be NULL when that gradient is not needed.  Every point walks the primitives the
+ * forward walked, through the same device code (cover test, boundary re-decision, nearest primitive and voxel).  With
+ * l = (x - pos)/s, w_j = 1 - |l_j|_inf over the covering j, W = sum w_j + 1e-6, v_jc the trilinear sample, o_c = sum w_j v_jc / W and
+ * g_c = 0 for c >= 1 where o_c is outside [0,1]:
+ *   dL/dv_jc = g_c w_j / W (scattered to the 8 corners of channel c of feat[j]); dL/dw_j = sum_c g_c (v_jc - o_c) / W;
+ *   dL/dl_j = sum_c (g_c w_j / W) dv_jc/dl - dL/dw_j sign(l_jd) [|l_jd| = max] / (tied axes);
+ *   dL/dx += dL/dl_j / s_j, dL/dpos_j -= dL/dl_j / s_j, dL/ds_j -= (dL/dl_j . l_j) / s_j.
+ * Uncovered points: nothing when inference == 0; at inference (sdf = f + d sign(f), d = |x - c|, c = pos_k + s_k grid_v,
+ * u = (x - c)/d, 0 at d = 0): dL/dfeat[k, v] += g_0, dL/dx += g_0 sign(f) u, dL/dpos_k -= g_0 sign(f) u, dL/ds_k -= g_0 sign(f) u . grid_v.
+ * grad_srt / grad_feat are fp32 atomic reductions: their last bits vary from run to run. */
+int tpx_primsdf_query_backward(const float* x_dev, const float* srt_dev, const float* feat_dev, const void* grid_ws, size_t grid_bytes, int64_t n, int K,
+                               int S, int dim_feat, int inference, const float* grad_out_dev, float* grad_x_dev, float* grad_srt_dev, float* grad_feat_dev,
+                               void* stream);
 /* The sdf column of the same query on the R x R x R lattice (coords[i], coords[j], coords[k]) that extract_texmesh evaluates
  * (inference.py:106-116: linspace / meshgrid(indexing='ij') points in 8192-point chunks, reshape(R,R,R)), without materialising the
  * points: grid_out device fp32 [R,R,R], grid_out[i,j,k] = sdf at (x, y, z) = (coords[i], coords[j], coords[k]); coords device fp32 [R]
