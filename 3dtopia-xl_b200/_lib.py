@@ -177,3 +177,22 @@ def dtype_tag(t: torch.Tensor) -> int:
     if t.dtype == torch.float16:
         return DTYPE_F16
     raise TpxError(f"unsupported tensor dtype {t.dtype} (fp32 / fp16 only)")
+
+
+def upload(handle, set_weight, finalize, tensors, dev: torch.device) -> None:
+    """Load (key, tensor) pairs into a parameter handle on `dev` through its tpx_*_set_weight and tpx_*_finalize.  Each tensor is
+    staged as a contiguous fp16 / fp32 copy on the device; the stream is synchronised before the staged copies are dropped, since
+    the repack kernels read them."""
+    with torch.cuda.device(dev):
+        st = stream_ptr()
+        keep = []
+        for k, v in tensors:
+            t = v.detach()
+            if t.dtype not in (torch.float16, torch.float32):
+                t = t.float()
+            t = t.to(dev, non_blocking=True).contiguous()
+            keep.append(t)
+            shape = (C.c_int64 * t.dim())(*t.shape)
+            check(set_weight(handle, k.encode(), t.data_ptr(), dtype_tag(t), shape, t.dim(), st), f"{set_weight.__name__}({k})")
+        check(finalize(handle, st), finalize.__name__)
+        torch.cuda.current_stream().synchronize()

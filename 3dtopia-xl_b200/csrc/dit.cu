@@ -2,10 +2,7 @@
 // conditioning hoist, and the per-step forward schedule (one stream, ~12 launches per block, no host sync).
 //   reference: models/dit_crossattn.py:111-213, models/attention.py, models/utils.py
 #include <cstdlib>
-#include <string>
-#include <vector>
 
-#include "../../include/tpx.h"
 #include "kernels.cuh"
 
 using namespace tpx;
@@ -16,16 +13,12 @@ struct DitLayer {
 
 struct tpx_dit {
     int N, Cin, Cout, Dc, D, L, H, Dm, Dh, DhP, Ltot;
-    __half* store = nullptr;
-    size_t store_halves = 0;
+    ParamStore params;
     std::vector<DitLayer> layers;
     __half *Wada, *bada;                  // [L*9D + 2D, D], [L*9D + 2D]
     __half *null16, *Wx, *bx, *Wt0, *bt0, *Wt2, *bt2, *Wfl, *bfl;
     __half *uconst;                       // [L, D] : proj(to_v(null)) per block
     __half *tmp_v;                        // [D]
-    std::vector<uint8_t> seen;            // per required key
-    std::vector<std::string> required;
-    bool finalized = false;
     bool has_null = false;                // null_cond_embedding given (cond_drop_prob > 0 models only; dit_crossattn.py:143-146)
     // conditioning store
     __half *ck = nullptr, *cv = nullptr, *y16 = nullptr;
@@ -36,108 +29,40 @@ struct tpx_dit {
     std::vector<long long> ts_values;
 };
 
-static size_t al8(size_t n) { return (n + 7) & ~static_cast<size_t>(7); }
-
 namespace {
-struct Carver {
-    __half* base;
-    size_t off = 0;
-    __half* take(size_t n) {
-        __half* p = base == nullptr ? nullptr : base + off;
-        off += al8(n);
-        return p;
-    }
-};
-
-void carve_store(tpx_dit* h, __half* base) {
-    Carver c{base};
-    const size_t D = h->D, Dc = h->Dc, Dm = h->Dm;
+// The parameter store, keyed by the reference's state_dict names.  Optional: null_cond_embedding (only models with cond_drop_prob > 0
+// have it) and the attention biases (absent with attn_proj_bias = False; the rest stay zero).
+void declare_params(tpx_dit* h, ParamStore& s) {
+    const int64_t D = h->D, Dc = h->Dc, Dm = h->Dm;
+    const auto prefix = [h](int i) { return i < h->L ? "blocks." + std::to_string(i) + "." : std::string("final_layer."); };
     h->layers.resize(h->L);
     for (int i = 0; i < h->L; ++i) {
         DitLayer& l = h->layers[i];
-        l.Wq = c.take(D * D);       l.bq = c.take(D);
-        l.Wkv = c.take(2 * D * Dc); l.bkv = c.take(2 * D);
-        l.Wcp = c.take(D * D);      l.bcp = c.take(D);
-        l.Wqkv = c.take(3 * D * D); l.bqkv = c.take(3 * D);
-        l.Wsp = c.take(D * D);      l.bsp = c.take(D);
-        l.W1 = c.take(Dm * D);      l.b1 = c.take(Dm);
-        l.W2 = c.take(D * Dm);      l.b2 = c.take(D);
+        const std::string p = prefix(i);
+        s.weight_bias(p + "crossattn.to_q", l.Wq, l.bq, {D, D}, PK_PLAIN, false);
+        l.Wkv = s.take(2 * D * Dc);       // to_k rows, then to_v rows: one GEMM computes both
+        l.bkv = s.take(2 * D);
+        s.weight_bias_at(p + "crossattn.to_k", l.Wkv, l.bkv, {D, Dc}, PK_PLAIN, false);
+        s.weight_bias_at(p + "crossattn.to_v", l.Wkv + D * Dc, l.bkv + D, {D, Dc}, PK_PLAIN, false);
+        s.weight_bias(p + "crossattn.proj", l.Wcp, l.bcp, {D, D}, PK_PLAIN, false);
+        s.weight_bias(p + "attn.qkv", l.Wqkv, l.bqkv, {3 * D, D}, PK_PLAIN, false);
+        s.weight_bias(p + "attn.proj", l.Wsp, l.bsp, {D, D}, PK_PLAIN, false);
+        s.weight_bias(p + "mlp.fc1", l.W1, l.b1, {Dm, D});
+        s.weight_bias(p + "mlp.fc2", l.W2, l.b2, {D, Dm});
     }
-    h->Wada = c.take(static_cast<size_t>(h->Ltot) * D);
-    h->bada = c.take(h->Ltot);
-    h->null16 = c.take(Dc);
-    h->Wx = c.take(D * h->Cin);  h->bx = c.take(D);
-    h->Wt0 = c.take(D * 256);    h->bt0 = c.take(D);
-    h->Wt2 = c.take(D * D);      h->bt2 = c.take(D);
-    h->Wfl = c.take(static_cast<size_t>(h->Cout) * D);  h->bfl = c.take(h->Cout);
-    h->uconst = c.take(static_cast<size_t>(h->L) * D);
-    h->tmp_v = c.take(D);
-    h->store_halves = c.off;
-}
-
-struct Slot {
-    __half* ptr;
-    int64_t d0, d1;  // expected shape (d1 == 0 -> 1-D)
-    bool optional;
-};
-
-// Map a reference state_dict key to its slot.  Returns false for an unknown key.
-bool find_slot(tpx_dit* h, const std::string& key, Slot* s) {
-    const int64_t D = h->D, Dc = h->Dc, Dm = h->Dm;
-    auto set = [&](__half* p, int64_t a, int64_t b, bool opt = false) { *s = Slot{p, a, b, opt}; return true; };
-    if (key == "null_cond_embedding") return set(h->null16, Dc, 0);
-    if (key == "x_embedder.weight") return set(h->Wx, D, h->Cin);
-    if (key == "x_embedder.bias") return set(h->bx, D, 0);
-    if (key == "t_embedder.mlp.0.weight") return set(h->Wt0, D, 256);
-    if (key == "t_embedder.mlp.0.bias") return set(h->bt0, D, 0);
-    if (key == "t_embedder.mlp.2.weight") return set(h->Wt2, D, D);
-    if (key == "t_embedder.mlp.2.bias") return set(h->bt2, D, 0);
-    if (key == "final_layer.linear.weight") return set(h->Wfl, h->Cout, D);
-    if (key == "final_layer.linear.bias") return set(h->bfl, h->Cout, 0);
-    if (key == "final_layer.adaLN_modulation.1.weight") return set(h->Wada + static_cast<size_t>(h->L) * 9 * D * D, 2 * D, D);
-    if (key == "final_layer.adaLN_modulation.1.bias") return set(h->bada + static_cast<size_t>(h->L) * 9 * D, 2 * D, 0);
-    if (key.rfind("blocks.", 0) != 0) return false;
-    const size_t dot = key.find('.', 7);
-    if (dot == std::string::npos) return false;
-    char* endp = nullptr;
-    const long i = strtol(key.c_str() + 7, &endp, 10);
-    if (endp != key.c_str() + dot || i < 0 || i >= h->L) return false;
-    const std::string r = key.substr(dot + 1);
-    DitLayer& l = h->layers[i];
-    if (r == "crossattn.to_q.weight") return set(l.Wq, D, D);
-    if (r == "crossattn.to_q.bias") return set(l.bq, D, 0, true);
-    if (r == "crossattn.to_k.weight") return set(l.Wkv, D, Dc);
-    if (r == "crossattn.to_k.bias") return set(l.bkv, D, 0, true);
-    if (r == "crossattn.to_v.weight") return set(l.Wkv + D * Dc, D, Dc);
-    if (r == "crossattn.to_v.bias") return set(l.bkv + D, D, 0, true);
-    if (r == "crossattn.proj.weight") return set(l.Wcp, D, D);
-    if (r == "crossattn.proj.bias") return set(l.bcp, D, 0, true);
-    if (r == "attn.qkv.weight") return set(l.Wqkv, 3 * D, D);
-    if (r == "attn.qkv.bias") return set(l.bqkv, 3 * D, 0, true);
-    if (r == "attn.proj.weight") return set(l.Wsp, D, D);
-    if (r == "attn.proj.bias") return set(l.bsp, D, 0, true);
-    if (r == "mlp.fc1.weight") return set(l.W1, Dm, D);
-    if (r == "mlp.fc1.bias") return set(l.b1, Dm, 0);
-    if (r == "mlp.fc2.weight") return set(l.W2, D, Dm);
-    if (r == "mlp.fc2.bias") return set(l.b2, D, 0);
-    if (r == "adaLN_modulation.1.weight") return set(h->Wada + static_cast<size_t>(i) * 9 * D * D, 9 * D, D);
-    if (r == "adaLN_modulation.1.bias") return set(h->bada + static_cast<size_t>(i) * 9 * D, 9 * D, 0);
-    return false;
-}
-
-void build_required(tpx_dit* h) {
-    auto& r = h->required;
-    // null_cond_embedding is optional: the reference only creates it when cond_drop_prob > 0 (dit_crossattn.py:143-146)
-    for (const char* k : {"x_embedder.weight", "x_embedder.bias", "t_embedder.mlp.0.weight", "t_embedder.mlp.0.bias",
-                          "t_embedder.mlp.2.weight", "t_embedder.mlp.2.bias", "final_layer.linear.weight", "final_layer.linear.bias",
-                          "final_layer.adaLN_modulation.1.weight", "final_layer.adaLN_modulation.1.bias"})
-        r.emplace_back(k);
-    for (int i = 0; i < h->L; ++i)
-        for (const char* k : {"crossattn.to_q.weight", "crossattn.to_k.weight", "crossattn.to_v.weight", "crossattn.proj.weight", "attn.qkv.weight",
-                              "attn.proj.weight", "mlp.fc1.weight", "mlp.fc1.bias", "mlp.fc2.weight", "mlp.fc2.bias", "adaLN_modulation.1.weight",
-                              "adaLN_modulation.1.bias"})
-            r.emplace_back("blocks." + std::to_string(i) + "." + k);
-    h->seen.assign(r.size(), 0);
+    // every block's adaLN rows (9D each), then the final layer's 2D: one GEMV computes all modulations of a step
+    h->Wada = s.take(static_cast<size_t>(h->Ltot) * D);
+    h->bada = s.take(h->Ltot);
+    for (int i = 0; i <= h->L; ++i)
+        s.weight_bias_at(prefix(i) + "adaLN_modulation.1", h->Wada + static_cast<size_t>(i) * 9 * D * D, h->bada + static_cast<size_t>(i) * 9 * D,
+                         {i < h->L ? 9 * D : 2 * D, D});
+    h->null16 = s.param("null_cond_embedding", {Dc}, PK_PLAIN, false);
+    s.weight_bias("x_embedder", h->Wx, h->bx, {D, h->Cin});
+    s.weight_bias("t_embedder.mlp.0", h->Wt0, h->bt0, {D, 256});
+    s.weight_bias("t_embedder.mlp.2", h->Wt2, h->bt2, {D, D});
+    s.weight_bias("final_layer.linear", h->Wfl, h->bfl, {h->Cout, D});
+    h->uconst = s.take(static_cast<size_t>(h->L) * D);
+    h->tmp_v = s.take(D);
 }
 
 struct DitWs {
@@ -147,25 +72,43 @@ struct DitWs {
     size_t total;
 };
 
-DitWs carve_ws(const tpx_dit* h, int S, uint8_t* base) {
+DitWs carve_ws(const tpx_dit* h, int S, void* base) {
+    Carve c{static_cast<uint8_t*>(base)};
     DitWs w;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { uint8_t* p = base == nullptr ? nullptr : base + off; off += (bytes + 255) & ~static_cast<size_t>(255); return p; };
     const size_t T = static_cast<size_t>(S) * h->N;
-    w.xres = reinterpret_cast<float*>(take(T * h->D * 4));
-    w.h16 = reinterpret_cast<__half*>(take(T * h->D * 2));
-    const size_t hb = static_cast<size_t>(S) * h->H * h->N * h->DhP * 2;
-    w.q = reinterpret_cast<__half*>(take(hb));
-    w.k = reinterpret_cast<__half*>(take(hb));
-    w.v = reinterpret_cast<__half*>(take(hb));
-    w.ao = reinterpret_cast<__half*>(take(T * h->D * 2));
-    w.hid = reinterpret_cast<__half*>(take(T * h->Dm * 2));
-    w.mod = reinterpret_cast<__half*>(take(static_cast<size_t>(S) * h->Ltot * 2));
-    w.ts16 = reinterpret_cast<__half*>(take(static_cast<size_t>(S) * h->D * 2));
-    w.fin = reinterpret_cast<__half*>(take(T * h->Cout * 2));
-    w.th1 = reinterpret_cast<float*>(take(static_cast<size_t>(S) * h->D * 4));
-    w.temb = reinterpret_cast<float*>(take(static_cast<size_t>(S) * h->D * 4));
-    w.total = off;
+    w.xres = c.take<float>(T * h->D);
+    w.h16 = c.take<__half>(T * h->D);
+    const size_t hb = static_cast<size_t>(S) * h->H * h->N * h->DhP;
+    w.q = c.take<__half>(hb);
+    w.k = c.take<__half>(hb);
+    w.v = c.take<__half>(hb);
+    w.ao = c.take<__half>(T * h->D);
+    w.hid = c.take<__half>(T * h->Dm);
+    w.mod = c.take<__half>(static_cast<size_t>(S) * h->Ltot);
+    w.ts16 = c.take<__half>(static_cast<size_t>(S) * h->D);
+    w.fin = c.take<__half>(T * h->Cout);
+    w.th1 = c.take<float>(static_cast<size_t>(S) * h->D);
+    w.temb = c.take<float>(static_cast<size_t>(S) * h->D);
+    w.total = c.off;
+    return w;
+}
+
+// Conditioning store: K and V of every block's cross-attention, then the fp16 conditioning
+struct CondWs {
+    __half *ck, *cv, *y16;
+    int MP;                        // key count padded for the transposed V (TMA row pitch must be a multiple of 16 B)
+    size_t total;
+};
+
+CondWs carve_cond(const tpx_dit* h, int n_cross, int M, void* base) {
+    Carve c{static_cast<uint8_t*>(base)};
+    CondWs w;
+    w.MP = (M + 7) & ~7;
+    const size_t kv = static_cast<size_t>(h->L) * n_cross * h->H * w.MP * h->DhP;
+    w.ck = c.take<__half>(kv);
+    w.cv = c.take<__half>(kv);
+    w.y16 = c.take<__half>(static_cast<size_t>(n_cross) * M * h->Dc);
+    w.total = c.off;
     return w;
 }
 
@@ -180,16 +123,15 @@ struct TsWs {
     size_t total;
 };
 
-TsWs carve_ts(const tpx_dit* h, int K, uint8_t* base) {
+TsWs carve_ts(const tpx_dit* h, int K, void* base) {
+    Carve c{static_cast<uint8_t*>(base)};
     TsWs w;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { uint8_t* p = base == nullptr ? nullptr : base + off; off += (bytes + 255) & ~static_cast<size_t>(255); return p; };
-    w.table = reinterpret_cast<__half*>(take(static_cast<size_t>(K) * h->Ltot * 2));
-    w.t_dev = reinterpret_cast<long long*>(take(static_cast<size_t>(K) * 8));
-    w.th1 = reinterpret_cast<float*>(take(static_cast<size_t>(TS_CHUNK) * h->D * 4));
-    w.temb = reinterpret_cast<float*>(take(static_cast<size_t>(TS_CHUNK) * h->D * 4));
-    w.ts16 = reinterpret_cast<__half*>(take(static_cast<size_t>(TS_CHUNK) * h->D * 2));
-    w.total = off;
+    w.table = c.take<__half>(static_cast<size_t>(K) * h->Ltot);
+    w.t_dev = c.take<long long>(K);
+    w.th1 = c.take<float>(static_cast<size_t>(TS_CHUNK) * h->D);
+    w.temb = c.take<float>(static_cast<size_t>(TS_CHUNK) * h->D);
+    w.ts16 = c.take<__half>(static_cast<size_t>(TS_CHUNK) * h->D);
+    w.total = c.off;
     return w;
 }
 
@@ -214,75 +156,51 @@ int tpx_dit_create(const tpx_dit_config* c, tpx_dit** out) {
     h->DhP = Dh <= 16 ? 16 : (Dh <= 32 ? 32 : (Dh <= 64 ? 64 : (Dh <= 80 ? 80 : 128)));
     h->Ltot = h->L * 9 * h->D + 2 * h->D;
     h->tc_attn = (h->Dh == 72 && h->N % 8 == 0);   // the wgmma kernel's 80-wide tiles
-    carve_store(h, nullptr);
-    cudaError_t e = cudaMalloc(&h->store, h->store_halves * 2);
-    if (e != cudaSuccess) { delete h; return cuda_fail(e, "cudaMalloc(parameter store)"); }
-    e = cudaMemset(h->store, 0, h->store_halves * 2);
-    if (e != cudaSuccess) { cudaFree(h->store); delete h; return cuda_fail(e, "cudaMemset(parameter store)"); }
-    carve_store(h, h->store);
-    build_required(h);
+    const int rc = h->params.create(16, [h](ParamStore& s) { declare_params(h, s); });
+    if (rc != TPX_OK) { delete h; return rc; }
     *out = h;
     return TPX_OK;
 }
 
-void tpx_dit_destroy(tpx_dit* h) {
-    if (h == nullptr) return;
-    if (h->store != nullptr) cudaFree(h->store);
-    delete h;
-}
+void tpx_dit_destroy(tpx_dit* h) { delete h; }
 
 int tpx_dit_set_weight(tpx_dit* h, const char* ref_key, const void* dev_ptr, int dtype, const int64_t* shape, int ndim, void* stream) {
-    TPX_CHECK(h != nullptr && ref_key != nullptr && dev_ptr != nullptr && shape != nullptr, TPX_ERR_ARG, "dit_set_weight: null argument");
-    Slot s;
-    const std::string key(ref_key);
-    if (!find_slot(h, key, &s)) { set_error("dit_set_weight: unexpected key '%s'", ref_key); return TPX_ERR_KEY; }
-    const bool ok = s.d1 == 0 ? (ndim == 1 && shape[0] == s.d0) : (ndim == 2 && shape[0] == s.d0 && shape[1] == s.d1);
-    TPX_CHECK(ok, TPX_ERR_SHAPE, "dit_set_weight: size mismatch for %s: expected [%lld%s%lld], got %d-d [%lld,...]", ref_key, (long long)s.d0,
-              s.d1 ? "," : "", (long long)s.d1, ndim, (long long)shape[0]);
-    const long long n = s.d1 == 0 ? s.d0 : s.d0 * s.d1;
-    int rc = launch_to_half(dev_ptr, dtype, s.ptr, n, static_cast<cudaStream_t>(stream));
+    TPX_CHECK(h != nullptr, TPX_ERR_ARG, "dit_set_weight: null argument");
+    const int rc = h->params.set("dit_set_weight", ref_key, dev_ptr, dtype, shape, ndim, static_cast<cudaStream_t>(stream));
     if (rc != TPX_OK) return rc;
-    for (size_t i = 0; i < h->required.size(); ++i)
-        if (h->required[i] == key) h->seen[i] = 1;
-    if (key == "null_cond_embedding") h->has_null = true;
-    h->finalized = false;
+    h->has_null = h->params.seen(h->null16);
     h->ts_values.clear();       // a timestep table derived from the previous weights is stale
     h->ts_table = nullptr;
     return TPX_OK;
 }
 
 int tpx_dit_get_weight(tpx_dit* h, const char* ref_key, void* dst_dev, int dtype, void* stream) {
-    TPX_CHECK(h != nullptr && ref_key != nullptr && dst_dev != nullptr, TPX_ERR_ARG, "dit_get_weight: null argument");
-    Slot s;
-    if (!find_slot(h, std::string(ref_key), &s)) { set_error("dit_get_weight: unexpected key '%s'", ref_key); return TPX_ERR_KEY; }
-    return launch_from_half(s.ptr, dst_dev, dtype, s.d1 == 0 ? s.d0 : s.d0 * s.d1, static_cast<cudaStream_t>(stream));
+    TPX_CHECK(h != nullptr, TPX_ERR_ARG, "dit_get_weight: null argument");
+    return h->params.get("dit_get_weight", ref_key, dst_dev, dtype, static_cast<cudaStream_t>(stream));
 }
 
 int tpx_dit_finalize(tpx_dit* h, void* stream) {
     TPX_CHECK(h != nullptr, TPX_ERR_ARG, "dit_finalize: null handle");
-    for (size_t i = 0; i < h->required.size(); ++i)
-        TPX_CHECK(h->seen[i], TPX_ERR_STATE, "dit_finalize: missing key '%s' in state_dict", h->required[i].c_str());
+    int rc = h->params.complete("dit_finalize");
+    if (rc != TPX_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // per-block constant of cross-attention against an all-null context: h(Wp . h(Wv . null + bv) + bp)
     for (int i = 0; h->has_null && i < h->L; ++i) {
         const DitLayer& l = h->layers[i];
-        int rc = launch_gemv(GEMV_IN_F16, GEMV_OUT_F16, l.Wkv + static_cast<size_t>(h->D) * h->Dc, l.bkv + h->D, h->null16, nullptr, 1, h->D, h->Dc,
-                             h->tmp_v, nullptr, h->D, st);
+        rc = launch_gemv(GEMV_IN_F16, GEMV_OUT_F16, l.Wkv + static_cast<size_t>(h->D) * h->Dc, l.bkv + h->D, h->null16, nullptr, 1, h->D, h->Dc,
+                         h->tmp_v, nullptr, h->D, st);
         if (rc != TPX_OK) return rc;
         rc = launch_gemv(GEMV_IN_F16, GEMV_OUT_F16, l.Wcp, l.bcp, h->tmp_v, nullptr, 1, h->D, h->D, h->uconst + static_cast<size_t>(i) * h->D, nullptr,
                          h->D, st);
         if (rc != TPX_OK) return rc;
     }
-    h->finalized = true;
+    h->params.finalized = true;
     return TPX_OK;
 }
 
 size_t tpx_dit_cond_bytes(const tpx_dit* h, int n_cross, int M) {
     if (h == nullptr || n_cross <= 0 || M <= 0) return 0;
-    const int MP = (M + 7) & ~7;   // key count padded for the transposed V (TMA row pitch must be a multiple of 16 B)
-    const size_t kv = static_cast<size_t>(h->L) * n_cross * h->H * MP * h->DhP * 2;
-    const size_t y = (static_cast<size_t>(n_cross) * M * h->Dc * 2 + 255) & ~static_cast<size_t>(255);
-    return 2 * ((kv + 255) & ~static_cast<size_t>(255)) + y;
+    return carve_cond(h, n_cross, M, nullptr).total;
 }
 
 size_t tpx_dit_workspace_bytes(const tpx_dit* h, int n_seq) {
@@ -292,26 +210,25 @@ size_t tpx_dit_workspace_bytes(const tpx_dit* h, int n_seq) {
 
 int tpx_dit_set_cond(tpx_dit* h, const float* y, int n_cross, int M, void* cond_ws, size_t cond_bytes, void* stream) {
     TPX_CHECK(h != nullptr && y != nullptr && cond_ws != nullptr, TPX_ERR_ARG, "dit_set_cond: null argument");
-    TPX_CHECK(h->finalized, TPX_ERR_STATE, "dit_set_cond: weights not finalized (load_state_dict first)");
+    TPX_CHECK(h->params.finalized, TPX_ERR_STATE, "dit_set_cond: weights not finalized (load_state_dict first)");
     TPX_CHECK(n_cross > 0 && M > 0, TPX_ERR_SHAPE, "dit_set_cond: empty conditioning (%d x %d)", n_cross, M);
     TPX_CHECK(cond_bytes >= tpx_dit_cond_bytes(h, n_cross, M), TPX_ERR_ARG, "dit_set_cond: conditioning store too small (%zu < %zu)", cond_bytes,
               tpx_dit_cond_bytes(h, n_cross, M));
     TPX_CHECK((reinterpret_cast<uintptr_t>(cond_ws) & 255) == 0, TPX_ERR_ARG, "dit_set_cond: store must be 256-B aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int MP = (M + 7) & ~7;
-    const size_t kv = (static_cast<size_t>(h->L) * n_cross * h->H * MP * h->DhP * 2 + 255) & ~static_cast<size_t>(255);
-    uint8_t* base = static_cast<uint8_t*>(cond_ws);
-    h->ck = reinterpret_cast<__half*>(base);
-    h->cv = reinterpret_cast<__half*>(base + kv);
-    h->y16 = reinterpret_cast<__half*>(base + 2 * kv);
+    const CondWs w = carve_cond(h, n_cross, M, cond_ws);
+    h->ck = w.ck;
+    h->cv = w.cv;
+    h->y16 = w.y16;
     h->cond_n = n_cross;
     h->cond_M = M;
-    h->cond_MP = MP;
-    if (h->tc_attn) TPX_CUDA(cudaMemsetAsync(h->cv, 0, kv, st));   // key columns [M, MP) of the transposed V must be finite
+    h->cond_MP = w.MP;
+    // key columns [M, MP) of the transposed V must be finite
+    if (h->tc_attn) TPX_CUDA(cudaMemsetAsync(h->cv, 0, reinterpret_cast<uint8_t*>(h->y16) - reinterpret_cast<uint8_t*>(h->cv), st));
     int rc = launch_to_half(y, TPX_DTYPE_F32, h->y16, static_cast<long long>(n_cross) * M * h->Dc, st);
     if (rc != TPX_OK) return rc;
     const size_t per_layer = static_cast<size_t>(n_cross) * h->H * M * h->DhP;
-    const size_t per_layer_v = h->tc_attn ? static_cast<size_t>(n_cross) * h->H * MP * h->DhP : per_layer;
+    const size_t per_layer_v = h->tc_attn ? static_cast<size_t>(n_cross) * h->H * h->cond_MP * h->DhP : per_layer;
     for (int i = 0; i < h->L; ++i) {
         GemmArgs a{};
         a.bias = h->layers[i].bkv;
@@ -319,7 +236,7 @@ int tpx_dit_set_cond(tpx_dit* h, const float* y, int n_cross, int M, void* cond_
         a.out0 = h->ck + i * per_layer;
         a.out1 = h->cv + i * per_layer_v;
         a.split_cols = h->D; a.Dh = h->Dh; a.DhP = h->DhP; a.H = h->H; a.Nseq = M;
-        if (h->tc_attn) { a.vt_which_plus1 = 2; a.vt_ld = MP; }
+        if (h->tc_attn) { a.vt_which_plus1 = 2; a.vt_ld = h->cond_MP; }
         rc = gemm_linear(h->y16, h->Dc, h->layers[i].Wkv, n_cross * M, 2 * h->D, h->Dc, EPI_HEADS, a, 0, st);
         if (rc != TPX_OK) return rc;
     }
@@ -334,7 +251,7 @@ static int dit_forward_impl(tpx_dit* h, const float* x, const int64_t* t, const 
                             size_t ws_bytes, void* stream, int stop_block = -1, int stop_stage = -1) {
     TPX_CHECK(h != nullptr && x != nullptr && (t != nullptr || mod_rows != nullptr) && (out != nullptr || stop_stage >= 0) && ws != nullptr, TPX_ERR_ARG,
               "dit_forward: null argument");
-    TPX_CHECK(h->finalized, TPX_ERR_STATE, "dit_forward: weights not finalized");
+    TPX_CHECK(h->params.finalized, TPX_ERR_STATE, "dit_forward: weights not finalized");
     TPX_CHECK(B >= 1 && B <= 8, TPX_ERR_SHAPE, "dit_forward: batch %d must be in [1,8]", B);
     TPX_CHECK(use_cfg >= 0 && use_cfg <= 2, TPX_ERR_ARG, "dit_forward: use_cfg %d", use_cfg);
     TPX_CHECK(use_cfg == 0 || h->has_null, TPX_ERR_STATE, "dit_forward: classifier-free guidance needs null_cond_embedding (model built with cond_drop_prob = 0)");
@@ -346,7 +263,7 @@ static int dit_forward_impl(tpx_dit* h, const float* x, const int64_t* t, const 
               tpx_dit_workspace_bytes(h, S));
     TPX_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "dit_forward: workspace must be 256-B aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const DitWs w = carve_ws(h, S, static_cast<uint8_t*>(ws));
+    const DitWs w = carve_ws(h, S, ws);
     const int N = h->N, D = h->D, Ltot = h->Ltot, M = h->cond_M;
     const float qscale = 1.0f / sqrtf(static_cast<float>(h->Dh));
     int rc;
@@ -465,13 +382,13 @@ size_t tpx_dit_timesteps_bytes(const tpx_dit* h, int K) {
 
 int tpx_dit_set_timesteps(tpx_dit* h, const int64_t* t_host, int K, void* ts_ws, size_t ts_bytes, void* stream) {
     TPX_CHECK(h != nullptr && t_host != nullptr && ts_ws != nullptr, TPX_ERR_ARG, "dit_set_timesteps: null argument");
-    TPX_CHECK(h->finalized, TPX_ERR_STATE, "dit_set_timesteps: weights not finalized (load_state_dict first)");
+    TPX_CHECK(h->params.finalized, TPX_ERR_STATE, "dit_set_timesteps: weights not finalized (load_state_dict first)");
     TPX_CHECK(K >= 1 && K <= TS_MAX, TPX_ERR_SHAPE, "dit_set_timesteps: %d timesteps (1..%d)", K, TS_MAX);
     TPX_CHECK(ts_bytes >= tpx_dit_timesteps_bytes(h, K), TPX_ERR_ARG, "dit_set_timesteps: table store too small (%zu < %zu)", ts_bytes,
               tpx_dit_timesteps_bytes(h, K));
     TPX_CHECK((reinterpret_cast<uintptr_t>(ts_ws) & 255) == 0, TPX_ERR_ARG, "dit_set_timesteps: store must be 256-B aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const TsWs w = carve_ts(h, K, static_cast<uint8_t*>(ts_ws));
+    const TsWs w = carve_ts(h, K, ts_ws);
     h->ts_values.clear();
     h->ts_table = nullptr;
     // pageable source: the driver stages the values before the call returns, so t_host need not outlive it
@@ -514,7 +431,7 @@ int tpx_dit_debug_tap(const tpx_dit* h, const void* ws, int n_seq, int which, in
     TPX_CHECK(which >= TPX_DIT_TAP_RESIDUAL && which <= TPX_DIT_TAP_PRE_CFG, TPX_ERR_ARG, "dit_debug_tap: bad tap %d", which);
     TPX_CHECK(n_seq >= 1 && count >= 1 && count <= n_seq, TPX_ERR_ARG, "dit_debug_tap: count %d must be in [1, n_seq = %d]", count, n_seq);
     TPX_CHECK(h != nullptr && ws != nullptr && dst != nullptr, TPX_ERR_ARG, "dit_debug_tap: null argument");
-    const DitWs w = carve_ws(h, n_seq, static_cast<uint8_t*>(const_cast<void*>(ws)));
+    const DitWs w = carve_ws(h, n_seq, const_cast<void*>(ws));
     const size_t T = static_cast<size_t>(count) * h->N;
     const void* src = which == TPX_DIT_TAP_RESIDUAL ? static_cast<const void*>(w.xres)
                       : which == TPX_DIT_TAP_ATTN_OUT ? static_cast<const void*>(w.ao)

@@ -29,32 +29,21 @@ struct McPtrs {
     int* blk_f;
     long long* off_v;
     long long* off_f;
+    size_t total;
 };
 
-size_t align256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
-
 McPtrs mc_carve(void* ws, long long N, long long nb) {
-    uint8_t* b = static_cast<uint8_t*>(ws);
+    Carve c{static_cast<uint8_t*>(ws)};
     McPtrs p;
-    p.hdr = reinterpret_cast<McHdr*>(b);
-    b += 256;
-    p.code = reinterpret_cast<uint16_t*>(b);
-    b += align256(static_cast<size_t>(N) * 2);
-    p.vbase = reinterpret_cast<int*>(b);
-    b += align256(static_cast<size_t>(N) * 4);
-    p.blk_v = reinterpret_cast<int*>(b);
-    b += align256(static_cast<size_t>(nb) * 4);
-    p.blk_f = reinterpret_cast<int*>(b);
-    b += align256(static_cast<size_t>(nb) * 4);
-    p.off_v = reinterpret_cast<long long*>(b);
-    b += align256(static_cast<size_t>(nb) * 8);
-    p.off_f = reinterpret_cast<long long*>(b);
+    p.hdr = c.take<McHdr>(1);
+    p.code = c.take<uint16_t>(N);
+    p.vbase = c.take<int>(N);
+    p.blk_v = c.take<int>(nb);
+    p.blk_f = c.take<int>(nb);
+    p.off_v = c.take<long long>(nb);
+    p.off_f = c.take<long long>(nb);
+    p.total = c.off;
     return p;
-}
-
-size_t mc_bytes(long long N, long long nb) {
-    return 256 + align256(static_cast<size_t>(N) * 2) + align256(static_cast<size_t>(N) * 4) + 2 * align256(static_cast<size_t>(nb) * 4) +
-           2 * align256(static_cast<size_t>(nb) * 8);
 }
 
 // exclusive block-wide prefix sum of v (MC_THREADS threads); *total receives the block's sum
@@ -233,7 +222,8 @@ int mc_check(const float* vol, long long X, long long Y, long long Z, const void
     *N = X * Y * Z;
     *nb = (*N + MC_THREADS - 1) / MC_THREADS;
     TPX_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "marching_cubes: workspace must be 256-B aligned");
-    TPX_CHECK(ws_bytes >= mc_bytes(*N, *nb), TPX_ERR_ARG, "marching_cubes: workspace of %zu bytes, %zu needed", ws_bytes, mc_bytes(*N, *nb));
+    const size_t need = mc_carve(nullptr, *N, *nb).total;
+    TPX_CHECK(ws_bytes >= need, TPX_ERR_ARG, "marching_cubes: workspace of %zu bytes, %zu needed", ws_bytes, need);
     return TPX_OK;
 }
 }  // namespace
@@ -248,7 +238,7 @@ size_t tpx_mc_workspace_bytes(int64_t X, int64_t Y, int64_t Z) {
     if (X < 2 || Y < 2 || Z < 2 || X >= MC_INDEX_LIMIT || Y >= MC_INDEX_LIMIT || Z >= MC_INDEX_LIMIT || X * Y >= MC_INDEX_LIMIT || X * Y * Z >= MC_INDEX_LIMIT)
         return 0;
     const long long N = X * Y * Z;
-    return mc_bytes(N, (N + MC_THREADS - 1) / MC_THREADS);
+    return mc_carve(nullptr, N, (N + MC_THREADS - 1) / MC_THREADS).total;
 }
 
 int tpx_mc_count(const float* vol, int64_t X, int64_t Y, int64_t Z, float iso, void* ws, size_t ws_bytes, int64_t* counts, void* stream) {

@@ -1,6 +1,5 @@
-// Pieces shared by the mesh clean-up / decimation (mesh_simplify.cu) and the isotropic remesher (mesh_remesh.cu): the workspace
-// carver, face input and output kernels, corner keys and the vertex CSR, the frozen-vertex state, the star flip test, the two-ring
-// minimum acceptance, face remap / compaction, the host-side argument checks and the CUB helpers.  Everything sits in an anonymous
+// Pieces shared by the mesh clean-up / decimation (mesh_simplify.cu) and the isotropic remesher (mesh_remesh.cu): face input and
+// output kernels, corner keys and the vertex CSR, the frozen-vertex state, the star flip test, the two-ring minimum acceptance, face remap / compaction, the host-side argument checks and the CUB helpers.  Everything sits in an anonymous
 // namespace, so each translation unit that includes this gets its own copy; both are compiled with -fmad=false (build.py).
 #pragma once
 #include <cub/cub.cuh>
@@ -16,22 +15,8 @@ constexpr long long MS_INDEX_LIMIT = 1LL << 31;
 constexpr u64 KEY_NONE = ~0ull;
 constexpr double SINGULAR_REL = 1e-10;
 
-size_t align256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
-
-// bump allocator over the caller's workspace; with base == nullptr it only counts bytes (the *_workspace_bytes queries)
-struct Carve {
-    uint8_t* base;
-    size_t off = 0;
-    template <class T>
-    T* take(long long n) {
-        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-        off += align256(static_cast<size_t>(n) * sizeof(T));
-        return p;
-    }
-};
-
 // CUB scratch: the onesweep radix sort needs a lookback table of a few bytes per key; the launch checks the real need against this
-size_t cub_reserve(long long n3) { return align256(static_cast<size_t>(n3) * 8 + (16u << 20)); }
+size_t cub_reserve(long long n3) { return align_up(static_cast<size_t>(n3) * 8 + (16u << 20), 256); }
 
 unsigned blocks(long long n) { return static_cast<unsigned>((n + MS_THREADS - 1) / MS_THREADS); }
 int key_bits(long long V) {

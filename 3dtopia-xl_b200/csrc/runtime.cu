@@ -1,11 +1,12 @@
-// Library-wide runtime of libtpx_b200: the thread-local error message, the device check, the launch counter and the optional
-// per-kernel-class event profiling, with their C entry points.
+// Library-wide runtime of libtpx_b200: the thread-local error message, the device check, the launch counter, the optional
+// per-kernel-class event profiling with their C entry points, and the parameter store of the model handles.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <cstring>
 #include <vector>
 
-#include "tpx_common.cuh"
+#include "kernels.cuh"
 
 namespace tpx {
 
@@ -56,6 +57,104 @@ int gemm_num_sms() {
         if (n <= 0) n = 132;
     }
     return n;
+}
+
+// ---- parameter store ------------------------------------------------------------------------------------
+static long long numel(const std::vector<int64_t>& shape) {
+    long long n = 1;
+    for (int64_t d : shape) n *= d;
+    return n;
+}
+
+ParamStore::~ParamStore() {
+    if (dev_ != nullptr) cudaFree(dev_);
+}
+
+int ParamStore::create(size_t align, const std::function<void(ParamStore&)>& layout) {
+    carve_ = Carve{nullptr, align};
+    layout(*this);
+    const size_t bytes = carve_.off;
+    TPX_CUDA(cudaMalloc(&dev_, bytes));
+    TPX_CUDA(cudaMemset(dev_, 0, bytes));
+    entries_.clear();
+    carve_ = Carve{reinterpret_cast<uint8_t*>(dev_), align};
+    layout(*this);
+    return TPX_OK;
+}
+
+__half* ParamStore::param_at(__half* slot, const std::string& key, std::vector<int64_t> shape, int kind, bool required) {
+    entries_.push_back(Entry{key, slot, std::move(shape), kind, required, false});
+    return slot;
+}
+
+__half* ParamStore::param(const std::string& key, std::vector<int64_t> shape, int kind, bool required) {
+    __half* slot = take(numel(shape));
+    return param_at(slot, key, std::move(shape), kind, required);
+}
+
+void ParamStore::weight_bias_at(const std::string& name, __half* W, __half* b, std::vector<int64_t> w_shape, int kind, bool bias_required) {
+    const int64_t rows = w_shape[0];
+    param_at(W, name + ".weight", std::move(w_shape), kind);
+    param_at(b, name + ".bias", {rows}, PK_PLAIN, bias_required);
+}
+
+void ParamStore::weight_bias(const std::string& name, __half*& W, __half*& b, std::vector<int64_t> w_shape, int kind, bool bias_required) {
+    W = take(numel(w_shape));
+    b = take(w_shape[0]);
+    weight_bias_at(name, W, b, std::move(w_shape), kind, bias_required);
+}
+
+ParamStore::Entry* ParamStore::find(const char* key) {
+    for (Entry& e : entries_)
+        if (e.key == key) return &e;
+    return nullptr;
+}
+
+int ParamStore::set(const char* what, const char* key, const void* src, int dtype, const int64_t* shape, int ndim, cudaStream_t st) {
+    TPX_CHECK(key != nullptr && src != nullptr && shape != nullptr, TPX_ERR_ARG, "%s: null argument", what);
+    for (const std::string& p : ignored)
+        if (strncmp(key, p.c_str(), p.size()) == 0) return 1;
+    Entry* e = find(key);
+    TPX_CHECK(e != nullptr, TPX_ERR_KEY, "%s: unexpected key '%s'", what, key);
+    bool ok = ndim == static_cast<int>(e->shape.size());
+    for (int i = 0; ok && i < ndim; ++i) ok = shape[i] == e->shape[i];
+    std::string want;
+    for (int64_t d : e->shape) want += (want.empty() ? "" : ",") + std::to_string(d);
+    TPX_CHECK(ok, TPX_ERR_SHAPE, "%s: size mismatch for %s: expected [%s], got %d-d", what, key, want.c_str(), ndim);
+    const int64_t* s = e->shape.data();
+    int rc = TPX_OK;
+    switch (e->kind) {
+        case PK_PLAIN: rc = launch_to_half(src, dtype, e->ptr, numel(e->shape), st); break;
+        case PK_CONV3: rc = launch_pack_conv3(src, dtype, e->ptr, static_cast<int>(s[0]), static_cast<int>(s[1]), 0, st); break;
+        case PK_CONV3_T: rc = launch_pack_conv3(src, dtype, e->ptr, static_cast<int>(s[1]), static_cast<int>(s[0]), 1, st); break;
+        case PK_CONVT2: rc = launch_pack_convt2(src, dtype, e->ptr, static_cast<int>(s[0]), static_cast<int>(s[1]), st); break;
+        case PK_CONV3_S2D: rc = launch_pack_conv3_s2d(src, dtype, e->ptr, static_cast<int>(s[0]), static_cast<int>(s[1]), st); break;
+        case PK_BIAS_REP8:
+            for (int j = 0; j < 8 && rc == TPX_OK; ++j) rc = launch_to_half(src, dtype, e->ptr + j * s[0], s[0], st);
+            break;
+    }
+    if (rc != TPX_OK) return rc;
+    e->seen = true;
+    finalized = false;
+    return TPX_OK;
+}
+
+int ParamStore::get(const char* what, const char* key, void* dst, int dtype, cudaStream_t st) {
+    TPX_CHECK(key != nullptr && dst != nullptr, TPX_ERR_ARG, "%s: null argument", what);
+    const Entry* e = find(key);
+    TPX_CHECK(e != nullptr, TPX_ERR_KEY, "%s: unexpected key '%s'", what, key);
+    return launch_from_half(e->ptr, dst, dtype, numel(e->shape), st);
+}
+
+bool ParamStore::seen(const __half* slot) const {
+    for (const Entry& e : entries_)
+        if (e.ptr == slot) return e.seen;
+    return false;
+}
+
+int ParamStore::complete(const char* what) const {
+    for (const Entry& e : entries_) TPX_CHECK(e.seen || !e.required, TPX_ERR_STATE, "%s: missing key '%s' in state_dict", what, e.key.c_str());
+    return TPX_OK;
 }
 
 }  // namespace tpx

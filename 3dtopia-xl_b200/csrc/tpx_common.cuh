@@ -1,5 +1,5 @@
-// Common device helpers for the sm_90a kernels: mbarrier, TMA and wgmma PTX wrappers.
-// Everything here is inline PTX for CUDA 12.x / sm_90a; no CUTLASS dependency.
+// Common helpers of libtpx_b200.  Host: error plumbing, buffer carving and the model handles' parameter store.  Device: mbarrier,
+// TMA and wgmma PTX wrappers, inline PTX for CUDA 12.x / sm_90a; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -7,6 +7,10 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
+
+#include <functional>
+#include <string>
+#include <vector>
 
 #include "../../include/tpx.h"
 
@@ -53,6 +57,73 @@ struct ProfScope {
 
 // SM count of the current device (cached on first use): the grid of the persistent kernels.
 int gemm_num_sms();
+
+// ------------------------------------------------------------------------------------------------
+// buffer carving and parameter stores (host)
+// ------------------------------------------------------------------------------------------------
+inline size_t align_up(size_t bytes, size_t align) { return (bytes + align - 1) / align * align; }
+
+// Bump allocator over one buffer: take<T>(n) hands out the next n elements and moves on by n * sizeof(T) rounded up to `align`
+// bytes.  With a null base it hands out nulls and only counts, so a *_bytes query and the call it sizes share one layout.
+struct Carve {
+    uint8_t* base;
+    size_t align = 256;
+    size_t off = 0;
+    template <class T>
+    T* take(size_t n) {
+        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+        off += align_up(n * sizeof(T), align);
+        return p;
+    }
+};
+
+// How a reference tensor is repacked into its fp16 slot (vae_kernels.cu): as it is; a Conv3d k3 weight [Cout, Cin, 3,3,3] as
+// [Cout, 27 Cin]; a ConvTranspose3d k3 weight [Cin, Cout, 3,3,3] the same way (rows >= Cout stay zero); a ConvTranspose3d k2 weight
+// as 8 [Cout, Cin] matrices; a bias copied 8 times (one per k2 output offset); a stride-2 Conv3d k3 weight for the space-to-depth input.
+enum ParamKind { PK_PLAIN, PK_CONV3, PK_CONV3_T, PK_CONVT2, PK_BIAS_REP8, PK_CONV3_S2D };
+
+// The fp16 parameters of a model handle, keyed by the reference's state_dict names: one zero-filled device allocation carved
+// into slots, and one declaration per key (slot, expected shape, repack, required).  `what` names the entry point in messages.
+class ParamStore {
+public:
+    bool finalized = false;                  // cleared by every successful set()
+    std::vector<std::string> ignored;        // key prefixes of the checkpoint's other half: set() returns 1 and records nothing
+
+    ParamStore() = default;
+    ParamStore(const ParamStore&) = delete;
+    ParamStore& operator=(const ParamStore&) = delete;
+    ~ParamStore();
+
+    // Runs `layout` once to size the store (slots `align` bytes apart), allocates and zero-fills it, then runs `layout` again on it.
+    // Zero-fill is part of the contract: padded rows and optional tensors that are never given read as 0.
+    int create(size_t align, const std::function<void(ParamStore&)>& layout);
+    // for `layout`: a slot that is no key, and the declaration of a key in a slot (which it returns)
+    __half* take(size_t n) { return carve_.take<__half>(n); }
+    __half* param_at(__half* slot, const std::string& key, std::vector<int64_t> shape, int kind = PK_PLAIN, bool required = true);
+    __half* param(const std::string& key, std::vector<int64_t> shape, int kind = PK_PLAIN, bool required = true);
+    // `name`.weight of shape w_shape and `name`.bias of shape [w_shape[0]], in the slots given or in two new ones
+    void weight_bias_at(const std::string& name, __half* W, __half* b, std::vector<int64_t> w_shape, int kind = PK_PLAIN, bool bias_required = true);
+    void weight_bias(const std::string& name, __half*& W, __half*& b, std::vector<int64_t> w_shape, int kind = PK_PLAIN, bool bias_required = true);
+
+    // null check, ignored prefixes, lookup (TPX_ERR_KEY), shape check (TPX_ERR_SHAPE), repack on `st`, then mark seen
+    int set(const char* what, const char* key, const void* src, int dtype, const int64_t* shape, int ndim, cudaStream_t st);
+    int get(const char* what, const char* key, void* dst, int dtype, cudaStream_t st);
+    bool seen(const __half* slot) const;
+    int complete(const char* what) const;    // TPX_ERR_STATE naming the first required key not set yet
+
+private:
+    struct Entry {
+        std::string key;
+        __half* ptr;
+        std::vector<int64_t> shape;
+        int kind;
+        bool required, seen;
+    };
+    Entry* find(const char* key);
+    __half* dev_ = nullptr;
+    Carve carve_{nullptr};
+    std::vector<Entry> entries_;
+};
 
 #ifdef __CUDACC__
 // Launch with the programmatic-stream-serialization attribute (PDL).  The kernel MUST call pdl_wait() before its

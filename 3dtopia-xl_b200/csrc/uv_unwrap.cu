@@ -24,19 +24,6 @@ constexpr int UW_RED_THREADS = 1024;
 constexpr long long UW_FACE_LIMIT = (1LL << 31) / 3;
 constexpr int UW_NTAPS = 6;
 
-size_t align256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
-
-struct Carve {
-    uint8_t* base;
-    size_t off = 0;
-    template <class T>
-    T* take(long long n) {
-        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-        off += align256(static_cast<size_t>(n) * sizeof(T));
-        return p;
-    }
-};
-
 unsigned blocks(long long n) { return static_cast<unsigned>((n + UW_THREADS - 1) / UW_THREADS); }
 int bits_for(long long n) {
     int b = 1;
@@ -103,7 +90,7 @@ size_t cub_need(long long V, long long F, int G) {
         need = b > need ? b : need;
     if (cub::DeviceScan::InclusiveSum(nullptr, b, static_cast<const int*>(nullptr), static_cast<int*>(nullptr), static_cast<int>(n3)) == cudaSuccess)
         need = b > need ? b : need;
-    return align256(need + 4096);
+    return align_up(need + 4096, 256);
 }
 
 Ws carve(void* base, long long V, long long F, int G, size_t cub_bytes, size_t* total) {
@@ -743,7 +730,7 @@ int uw_setup(void* ws, size_t ws_bytes, long long V, long long F, Ws* out) {
     size_t total = 0;
     carve(nullptr, V, F, G, 0, &total);
     const size_t cb = cub_need(V, F, G);
-    TPX_CHECK(ws_bytes >= total + align256(cb), TPX_ERR_ARG, "uv unwrap: workspace of %zu bytes, need %zu", ws_bytes, total + align256(cb));
+    TPX_CHECK(ws_bytes >= total + align_up(cb, 256), TPX_ERR_ARG, "uv unwrap: workspace of %zu bytes, need %zu", ws_bytes, total + align_up(cb, 256));
     TPX_CHECK(ws != nullptr && (reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "uv unwrap: workspace must be 256-B aligned");
     *out = carve(ws, V, F, G, cb, &total);
     return TPX_OK;
@@ -758,7 +745,7 @@ size_t tpx_uv_unwrap_workspace_bytes(int64_t V, int64_t F) {
     size_t total = 0;
     const int G = grid_side(F);
     carve(nullptr, V, F, G, 0, &total);
-    return total + align256(cub_need(V, F, G));
+    return total + align_up(cub_need(V, F, G), 256);
 }
 
 int tpx_vertex_normals(const float* verts_dev, int64_t V, const int32_t* faces_dev, int64_t F, void* ws, size_t ws_bytes, float* normals_dev, void* stream) {

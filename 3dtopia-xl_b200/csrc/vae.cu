@@ -5,9 +5,6 @@
 // Activations are channels-last fp16 [P, S^3, C]; every primitive is independent (GroupNorm statistics are
 // per primitive), so the whole decoder is a batch of P tiny volumes.
 #include <cmath>
-#include <cstring>
-#include <string>
-#include <vector>
 
 #include "kernels.cuh"
 
@@ -17,19 +14,19 @@ struct VaeRes {
     int cin, cout;
     __half *n1g, *n1b, *W1, *b1, *n2g, *n2b, *W2, *b2, *Wsc, *bsc;  // Wsc null when cin == cout
 };
+struct VaeAttn {
+    __half *ng, *nb, *Wqkv, *Wproj, *bproj;
+    int heads;
+};
 
 struct tpx_vae {
-    int C0, C1, Cout, heads;
-    __half* store = nullptr;
-    size_t store_halves = 0;
+    int C0, C1, Cout;
+    ParamStore params;
     __half *w_pq, *b_pq, *Win, *bin;
     VaeRes res[6];                           // mid0, mid1, up0.0, up0.1, up1.0, up1.1
-    __half *ang, *anb, *Wqkv, *Wap, *bap;    // mid attention
+    VaeAttn attn;                            // mid attention
     __half *Wup, *bup;                       // [8*C0, C0], [8*C0]
     __half *nog, *nob, *Wout, *bout;         // norm_out, conv_out (padded to 16 rows)
-    std::vector<std::string> required;
-    std::vector<uint8_t> seen;
-    bool finalized = false;
 };
 
 
@@ -37,123 +34,67 @@ struct tpx_vae {
 // ResnetBlocks, the stride-2 downsample to 4^3, a 32 -> 256 block with its 1x1 shortcut, a 256 block, the mid block (res, attention,
 // res), norm_out + SiLU and conv_out 256 -> 2 with quant_conv in its epilogue.
 struct tpx_vae_encoder {
-    int Cin = 6, C0 = 32, C1 = 256, heads = 8;
-    __half* store = nullptr;
-    size_t store_halves = 0;
+    int Cin = 6, C0 = 32, C1 = 256;
+    ParamStore params;
     __half *Win, *bin;                       // conv_in [32, 6*27] (the reference's own layout), bias
     VaeRes res[6];                           // down0.0, down0.1 (32, 8^3), down1.0 (32 -> 256), down1.1, mid0, mid1 (256, 4^3)
     __half *Wds, *bds;                       // downsample, repacked for the space-to-depth input: [32, 27*256]
-    __half *ang, *anb, *Wqkv, *Wap, *bap;    // mid attention
+    VaeAttn attn;                            // mid attention
     __half *nog, *nob, *Wout, *bout;         // norm_out, conv_out (padded to 16 rows)
     __half* quant;                           // quant_conv [w00, w01, w10, w11, b0, b1]
-    std::vector<std::string> required;
-    std::vector<uint8_t> seen;
-    bool finalized = false;
 };
 
 namespace {
-const char* kResPrefix[6] = {"decoder.mid_block.nets.0.", "decoder.mid_block.nets.1.", "decoder.up_blocks.0.nets.0.", "decoder.up_blocks.0.nets.1.",
-                             "decoder.up_blocks.1.nets.0.", "decoder.up_blocks.1.nets.1."};
+// Parameter slots are 128 B apart (TMA operands need 16-B alignment)
+constexpr size_t kSlotAlign = 128;
 
-struct HCarver {
-    __half* base;
-    size_t off = 0;
-    __half* take(size_t n) {
-        __half* p = base == nullptr ? nullptr : base + off;
-        off += (n + 63) & ~static_cast<size_t>(63);   // 128-B slots (TMA operands need 16-B alignment)
-        return p;
-    }
-};
-
-void carve(tpx_vae* h, __half* base) {
-    HCarver c{base};
-    const size_t C0 = h->C0, C1 = h->C1;
-    h->w_pq = c.take(8); h->b_pq = c.take(8);
-    h->Win = c.take(C0 * 27); h->bin = c.take(C0);
-    for (int i = 0; i < 6; ++i) {
-        VaeRes& r = h->res[i];
-        r.cin = i < 4 ? h->C0 : (i == 4 ? h->C0 : h->C1);
-        r.cout = i < 4 ? h->C0 : h->C1;
-        r.n1g = c.take(r.cin); r.n1b = c.take(r.cin);
-        r.W1 = c.take(static_cast<size_t>(r.cout) * 27 * r.cin); r.b1 = c.take(r.cout);
-        r.n2g = c.take(r.cout); r.n2b = c.take(r.cout);
-        r.W2 = c.take(static_cast<size_t>(r.cout) * 27 * r.cout); r.b2 = c.take(r.cout);
-        if (r.cin != r.cout) { r.Wsc = c.take(static_cast<size_t>(r.cout) * r.cin); r.bsc = c.take(r.cout); }
-        else { r.Wsc = nullptr; r.bsc = nullptr; }
-    }
-    h->ang = c.take(C0); h->anb = c.take(C0);
-    h->Wqkv = c.take(3 * C0 * C0); h->Wap = c.take(C0 * C0); h->bap = c.take(C0);
-    h->Wup = c.take(8 * C0 * C0); h->bup = c.take(8 * C0);
-    h->nog = c.take(C1); h->nob = c.take(C1);
-    h->Wout = c.take(16 * 27 * C1); h->bout = c.take(16);
-    h->store_halves = c.off;
+// ResnetBlock (vae3d_dib.py:128-145) and VolumeAttention (:34-48) keys under `p`, the same in the decoder and the encoder
+void res_params(ParamStore& s, const std::string& p, VaeRes& r, int cin, int cout) {
+    r.cin = cin;
+    r.cout = cout;
+    s.weight_bias(p + "norm1", r.n1g, r.n1b, {cin});
+    s.weight_bias(p + "conv1", r.W1, r.b1, {cout, cin, 3, 3, 3}, PK_CONV3);
+    s.weight_bias(p + "norm2", r.n2g, r.n2b, {cout});
+    s.weight_bias(p + "conv2", r.W2, r.b2, {cout, cout, 3, 3, 3}, PK_CONV3);
+    r.Wsc = r.bsc = nullptr;
+    if (cin != cout) s.weight_bias(p + "shortcut", r.Wsc, r.bsc, {cout, cin, 1, 1, 1});
 }
 
-enum SlotKind { SK_PLAIN, SK_CONV3, SK_CONV3_T, SK_CONVT2, SK_BIAS_REP8 };
-struct VSlot {
-    __half* ptr;
-    SlotKind kind;
-    std::vector<int64_t> shape;
-    int a, b;  // conv dims (Cout, Cin) or (Cin, Cout)
-};
+void attn_params(ParamStore& s, const std::string& p, VaeAttn& at, int C, int heads) {
+    at.heads = heads;
+    s.weight_bias(p + "norm", at.ng, at.nb, {C});
+    at.Wqkv = s.param(p + "attn.qkv.weight", {3 * C, C});
+    s.weight_bias(p + "attn.proj", at.Wproj, at.bproj, {C, C});
+}
 
-bool find_vslot(tpx_vae* h, const std::string& key, VSlot* s) {
+void declare_decoder(tpx_vae* h, ParamStore& s, int heads) {
     const int64_t C0 = h->C0, C1 = h->C1;
-    auto plain = [&](__half* p, std::vector<int64_t> shp) { *s = VSlot{p, SK_PLAIN, shp, 0, 0}; return true; };
-    if (key == "post_quant_conv.weight") return plain(h->w_pq, {1, 1, 1, 1, 1});
-    if (key == "post_quant_conv.bias") return plain(h->b_pq, {1});
-    if (key == "decoder.conv_in.weight") return plain(h->Win, {C0, 1, 3, 3, 3});
-    if (key == "decoder.conv_in.bias") return plain(h->bin, {C0});
-    if (key == "decoder.norm_out.weight") return plain(h->nog, {C1});
-    if (key == "decoder.norm_out.bias") return plain(h->nob, {C1});
-    if (key == "decoder.conv_out.weight") { *s = VSlot{h->Wout, SK_CONV3_T, {C1, h->Cout, 3, 3, 3}, h->Cout, static_cast<int>(C1)}; return true; }
-    if (key == "decoder.conv_out.bias") return plain(h->bout, {h->Cout});
-    if (key == "decoder.up_blocks.0.upsample.weight") { *s = VSlot{h->Wup, SK_CONVT2, {C0, C0, 2, 2, 2}, static_cast<int>(C0), static_cast<int>(C0)}; return true; }
-    if (key == "decoder.up_blocks.0.upsample.bias") { *s = VSlot{h->bup, SK_BIAS_REP8, {C0}, static_cast<int>(C0), 0}; return true; }
-    const std::string a = "decoder.mid_block.attns.0.";
-    if (key == a + "norm.weight") return plain(h->ang, {C0});
-    if (key == a + "norm.bias") return plain(h->anb, {C0});
-    if (key == a + "attn.qkv.weight") return plain(h->Wqkv, {3 * C0, C0});
-    if (key == a + "attn.proj.weight") return plain(h->Wap, {C0, C0});
-    if (key == a + "attn.proj.bias") return plain(h->bap, {C0});
-    for (int i = 0; i < 6; ++i) {
-        const std::string p = kResPrefix[i];
-        if (key.rfind(p, 0) != 0) continue;
-        VaeRes& r = h->res[i];
-        const std::string t = key.substr(p.size());
-        if (t == "norm1.weight") return plain(r.n1g, {r.cin});
-        if (t == "norm1.bias") return plain(r.n1b, {r.cin});
-        if (t == "norm2.weight") return plain(r.n2g, {r.cout});
-        if (t == "norm2.bias") return plain(r.n2b, {r.cout});
-        if (t == "conv1.weight") { *s = VSlot{r.W1, SK_CONV3, {r.cout, r.cin, 3, 3, 3}, r.cout, r.cin}; return true; }
-        if (t == "conv1.bias") return plain(r.b1, {r.cout});
-        if (t == "conv2.weight") { *s = VSlot{r.W2, SK_CONV3, {r.cout, r.cout, 3, 3, 3}, r.cout, r.cout}; return true; }
-        if (t == "conv2.bias") return plain(r.b2, {r.cout});
-        if (r.Wsc != nullptr && t == "shortcut.weight") return plain(r.Wsc, {r.cout, r.cin, 1, 1, 1});
-        if (r.Wsc != nullptr && t == "shortcut.bias") return plain(r.bsc, {r.cout});
-        return false;
-    }
-    return false;
-}
-
-__global__ void rep8_kernel(const __half* __restrict__ src, __half* __restrict__ dst, int C) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < 8 * C) dst[i] = src[i % C];
+    s.weight_bias("post_quant_conv", h->w_pq, h->b_pq, {1, 1, 1, 1, 1});
+    s.weight_bias("decoder.conv_in", h->Win, h->bin, {C0, 1, 3, 3, 3});
+    const char* res[6] = {"mid_block.nets.0.", "mid_block.nets.1.", "up_blocks.0.nets.0.", "up_blocks.0.nets.1.", "up_blocks.1.nets.0.",
+                          "up_blocks.1.nets.1."};
+    for (int i = 0; i < 6; ++i) res_params(s, std::string("decoder.") + res[i], h->res[i], i < 5 ? h->C0 : h->C1, i < 4 ? h->C0 : h->C1);
+    attn_params(s, "decoder.mid_block.attns.0.", h->attn, h->C0, heads);
+    h->Wup = s.param("decoder.up_blocks.0.upsample.weight", {C0, C0, 2, 2, 2}, PK_CONVT2);
+    h->bup = s.param_at(s.take(8 * C0), "decoder.up_blocks.0.upsample.bias", {C0}, PK_BIAS_REP8);
+    s.weight_bias("decoder.norm_out", h->nog, h->nob, {C1});
+    h->Wout = s.param_at(s.take(16 * 27 * C1), "decoder.conv_out.weight", {C1, h->Cout, 3, 3, 3}, PK_CONV3_T);   // rows >= Cout stay zero
+    h->bout = s.param_at(s.take(16), "decoder.conv_out.bias", {h->Cout});
 }
 
 struct VaeWs {
     __half *X, *T1, *T2, *X2, *Q, *K, *V, *U, *G, *sa, *sb, *sc, *sd;
     size_t total;
 };
-VaeWs carve_vws(const tpx_vae* h, int P, uint8_t* base) {
+VaeWs carve_vws(const tpx_vae* h, int P, void* base) {
+    Carve c{static_cast<uint8_t*>(base), 1024};
     VaeWs w;
-    size_t off = 0;
-    auto take = [&](size_t halves) { uint8_t* p = base == nullptr ? nullptr : base + off; off += (halves * 2 + 1023) & ~static_cast<size_t>(1023); return reinterpret_cast<__half*>(p); };
     const size_t S4 = static_cast<size_t>(P) * 64 * h->C0, S8 = static_cast<size_t>(P) * 512 * h->C0, s8 = static_cast<size_t>(P) * 512 * h->C1;
-    w.X = take(S4); w.T1 = take(S4); w.T2 = take(S4); w.X2 = take(S4); w.Q = take(S4); w.K = take(S4); w.V = take(S4);
-    w.U = take(S8); w.G = take(S8);
-    w.sa = take(s8); w.sb = take(s8); w.sc = take(s8); w.sd = take(s8);
-    w.total = off;
+    w.X = c.take<__half>(S4); w.T1 = c.take<__half>(S4); w.T2 = c.take<__half>(S4); w.X2 = c.take<__half>(S4); w.Q = c.take<__half>(S4);
+    w.K = c.take<__half>(S4); w.V = c.take<__half>(S4);
+    w.U = c.take<__half>(S8); w.G = c.take<__half>(S8);
+    w.sa = c.take<__half>(s8); w.sb = c.take<__half>(s8); w.sc = c.take<__half>(s8); w.sd = c.take<__half>(s8);
+    w.total = c.off;
     return w;
 }
 
@@ -172,10 +113,6 @@ int conv3(const __half* x, const __half* W, const __half* bias, const __half* re
 }
 
 // ---- blocks both schedules run (weights come as structs, scratch as pointers: no handle) ------------------------------------
-struct VaeAttn {
-    __half *ng, *nb, *Wqkv, *Wproj, *bproj;
-    int heads;
-};
 struct BlockScratch {
     __half *T1, *T2, *Q, *K, *V;   // [P, S^3, C] each
 };
@@ -217,23 +154,20 @@ int attention_block(const VaeAttn& at, __half*& X, __half*& X2, const BlockScrat
     return TPX_OK;
 }
 
-int check_run_args(const tpx_vae* h, const void* z, const void* dst, int P, const void* ws, size_t ws_bytes, const char* what) {
-    TPX_CHECK(h != nullptr && z != nullptr && dst != nullptr && ws != nullptr, TPX_ERR_ARG, "%s: null argument", what);
-    TPX_CHECK(h->finalized, TPX_ERR_STATE, "%s: weights not finalized (load_state_dict first)", what);
+// Argument checks of the decode and encode entry points; ws_bytes_fn is the handle's *_workspace_bytes.
+template <class H>
+int check_run_args(const H* h, size_t (*ws_bytes_fn)(const H*, int), const void* in, const void* dst, int P, const void* ws, size_t ws_bytes,
+                   const char* what) {
+    TPX_CHECK(h != nullptr && in != nullptr && dst != nullptr && ws != nullptr, TPX_ERR_ARG, "%s: null argument", what);
+    TPX_CHECK(h->params.finalized, TPX_ERR_STATE, "%s: weights not finalized (load_state_dict first)", what);
     TPX_CHECK(P > 0, TPX_ERR_SHAPE, "%s: empty batch", what);
-    TPX_CHECK(ws_bytes >= tpx_vae_workspace_bytes(h, P), TPX_ERR_ARG, "%s: workspace too small (%zu < %zu)", what, ws_bytes, tpx_vae_workspace_bytes(h, P));
+    const size_t need = ws_bytes_fn(h, P);
+    TPX_CHECK(ws_bytes >= need, TPX_ERR_ARG, "%s: workspace too small (%zu < %zu)", what, ws_bytes, need);
     TPX_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "%s: workspace must be 256-B aligned", what);
     return TPX_OK;
 }
 
-// The decode schedule.  stop < 0 runs it to the end and writes `out`; stop = TPX_VAE_STAGE_* ends after that stage and copies its
-// channels-last fp16 activation into `tap` (tpx_vae_debug_stage).  Both run the same launches up to the stop.
-int vae_run(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, int P, int stop, void* tap, void* ws, cudaStream_t st) {
-    VaeWs w = carve_vws(h, P, static_cast<uint8_t*>(ws));
-    const int C0 = h->C0, C1 = h->C1;
-    const float skip = kSkip;
-    const float eps = kEps;
-    int rc;
+// The schedules' launch check and debug tap: stop = the stage to end after (< 0: none), whose activation is copied into `tap`
 #define TPX_RC(call) do { rc = (call); if (rc != TPX_OK) return rc; } while (0)
 #define TPX_TAP(stage, act, S3, C)                                                                                                   \
     do {                                                                                                                             \
@@ -242,13 +176,22 @@ int vae_run(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, in
             return TPX_OK;                                                                                                           \
         }                                                                                                                            \
     } while (0)
+
+// The decode schedule.  stop < 0 runs it to the end and writes `out`; stop = TPX_VAE_STAGE_* ends after that stage and copies its
+// channels-last fp16 activation into `tap` (tpx_vae_debug_stage).  Both run the same launches up to the stop.
+int vae_run(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, int P, int stop, void* tap, void* ws, cudaStream_t st) {
+    VaeWs w = carve_vws(h, P, ws);
+    const int C0 = h->C0, C1 = h->C1;
+    const float skip = kSkip;
+    const float eps = kEps;
+    int rc;
     TPX_RC(launch_vae_conv_in(z, z_dtype, h->w_pq, h->b_pq, h->Win, h->bin, P, C0, w.X, st));
     __half *X = w.X, *X2 = w.X2;
     const BlockScratch sc{w.T1, w.T2, w.Q, w.K, w.V};
     TPX_TAP(TPX_VAE_STAGE_CONV_IN, X, 64, C0);
     TPX_RC(resnet_block(h->res[0], 4, X, X2, sc, P, st));
     TPX_TAP(TPX_VAE_STAGE_MID_RES0, X, 64, C0);
-    TPX_RC(attention_block(VaeAttn{h->ang, h->anb, h->Wqkv, h->Wap, h->bap, h->heads}, X, X2, sc, P, C0, st));
+    TPX_RC(attention_block(h->attn, X, X2, sc, P, C0, st));
     TPX_TAP(TPX_VAE_STAGE_MID_ATTN, X, 64, C0);
     TPX_RC(resnet_block(h->res[1], 4, X, X2, sc, P, st));
     TPX_TAP(TPX_VAE_STAGE_MID_RES1, X, 64, C0);
@@ -296,84 +239,26 @@ int vae_run(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, in
     TPX_TAP(TPX_VAE_STAGE_NORM_OUT, w.sa, 512, C1);
     TPX_RC(conv3(w.sa, h->Wout, h->bout, nullptr, 1.f, out_dtype == TPX_DTYPE_F16 ? static_cast<__half*>(out) : nullptr,
                  out_dtype == TPX_DTYPE_F32 ? static_cast<float*>(out) : nullptr, h->Cout, P, 8, C1, 16, EPI_NCDHW, st));
-#undef TPX_TAP
-#undef TPX_RC
     return TPX_OK;
 }
 
 // ---- encoder ----------------------------------------------------------------------------------------------------------------
-const char* kEncResPrefix[6] = {"encoder.down_blocks.0.nets.0.", "encoder.down_blocks.0.nets.1.", "encoder.down_blocks.1.nets.0.",
-                                "encoder.down_blocks.1.nets.1.", "encoder.mid_block.nets.0.", "encoder.mid_block.nets.1."};
-
-void carve_enc(tpx_vae_encoder* h, __half* base) {
-    HCarver c{base};
-    const size_t C0 = h->C0, C1 = h->C1;
-    h->Win = c.take(C0 * h->Cin * 27); h->bin = c.take(C0);
-    for (int i = 0; i < 6; ++i) {
-        VaeRes& r = h->res[i];
-        r.cin = i < 3 ? h->C0 : h->C1;
-        r.cout = i < 2 ? h->C0 : h->C1;
-        r.n1g = c.take(r.cin); r.n1b = c.take(r.cin);
-        r.W1 = c.take(static_cast<size_t>(r.cout) * 27 * r.cin); r.b1 = c.take(r.cout);
-        r.n2g = c.take(r.cout); r.n2b = c.take(r.cout);
-        r.W2 = c.take(static_cast<size_t>(r.cout) * 27 * r.cout); r.b2 = c.take(r.cout);
-        if (r.cin != r.cout) { r.Wsc = c.take(static_cast<size_t>(r.cout) * r.cin); r.bsc = c.take(r.cout); }
-        else { r.Wsc = nullptr; r.bsc = nullptr; }
-    }
-    h->Wds = c.take(C0 * 27 * 8 * C0); h->bds = c.take(C0);
-    h->ang = c.take(C1); h->anb = c.take(C1);
-    h->Wqkv = c.take(3 * C1 * C1); h->Wap = c.take(C1 * C1); h->bap = c.take(C1);
-    h->nog = c.take(C1); h->nob = c.take(C1);
-    h->Wout = c.take(16 * 27 * C1); h->bout = c.take(16);
-    h->quant = c.take(8);
-    h->store_halves = c.off;
-}
-
-enum EncSlotKind { EK_PLAIN, EK_CONV3, EK_CONV3_S2D };
-struct ESlot {
-    __half* ptr;
-    EncSlotKind kind;
-    std::vector<int64_t> shape;
-};
-
-bool find_eslot(tpx_vae_encoder* h, const std::string& key, ESlot* s) {
+void declare_encoder(tpx_vae_encoder* h, ParamStore& s, int heads) {
     const int64_t C0 = h->C0, C1 = h->C1;
-    auto plain = [&](__half* p, std::vector<int64_t> shp) { *s = ESlot{p, EK_PLAIN, shp}; return true; };
-    auto conv = [&](__half* p, std::vector<int64_t> shp) { *s = ESlot{p, EK_CONV3, shp}; return true; };
-    if (key == "encoder.conv_in.weight") return plain(h->Win, {C0, h->Cin, 3, 3, 3});
-    if (key == "encoder.conv_in.bias") return plain(h->bin, {C0});
-    if (key == "encoder.down_blocks.0.downsample.weight") { *s = ESlot{h->Wds, EK_CONV3_S2D, {C0, C0, 3, 3, 3}}; return true; }
-    if (key == "encoder.down_blocks.0.downsample.bias") return plain(h->bds, {C0});
-    if (key == "encoder.norm_out.weight") return plain(h->nog, {C1});
-    if (key == "encoder.norm_out.bias") return plain(h->nob, {C1});
-    if (key == "encoder.conv_out.weight") return conv(h->Wout, {2, C1, 3, 3, 3});   // rows 2..15 stay zero
-    if (key == "encoder.conv_out.bias") return plain(h->bout, {2});
-    if (key == "quant_conv.weight") return plain(h->quant, {2, 2, 1, 1, 1});
-    if (key == "quant_conv.bias") return plain(h->quant + 4, {2});
-    const std::string a = "encoder.mid_block.attns.0.";
-    if (key == a + "norm.weight") return plain(h->ang, {C1});
-    if (key == a + "norm.bias") return plain(h->anb, {C1});
-    if (key == a + "attn.qkv.weight") return plain(h->Wqkv, {3 * C1, C1});
-    if (key == a + "attn.proj.weight") return plain(h->Wap, {C1, C1});
-    if (key == a + "attn.proj.bias") return plain(h->bap, {C1});
-    for (int i = 0; i < 6; ++i) {
-        const std::string p = kEncResPrefix[i];
-        if (key.rfind(p, 0) != 0) continue;
-        VaeRes& r = h->res[i];
-        const std::string t = key.substr(p.size());
-        if (t == "norm1.weight") return plain(r.n1g, {r.cin});
-        if (t == "norm1.bias") return plain(r.n1b, {r.cin});
-        if (t == "norm2.weight") return plain(r.n2g, {r.cout});
-        if (t == "norm2.bias") return plain(r.n2b, {r.cout});
-        if (t == "conv1.weight") return conv(r.W1, {r.cout, r.cin, 3, 3, 3});
-        if (t == "conv1.bias") return plain(r.b1, {r.cout});
-        if (t == "conv2.weight") return conv(r.W2, {r.cout, r.cout, 3, 3, 3});
-        if (t == "conv2.bias") return plain(r.b2, {r.cout});
-        if (r.Wsc != nullptr && t == "shortcut.weight") return plain(r.Wsc, {r.cout, r.cin, 1, 1, 1});
-        if (r.Wsc != nullptr && t == "shortcut.bias") return plain(r.bsc, {r.cout});
-        return false;
-    }
-    return false;
+    s.weight_bias("encoder.conv_in", h->Win, h->bin, {C0, h->Cin, 3, 3, 3});
+    const char* res[6] = {"down_blocks.0.nets.0.", "down_blocks.0.nets.1.", "down_blocks.1.nets.0.", "down_blocks.1.nets.1.", "mid_block.nets.0.",
+                          "mid_block.nets.1."};
+    for (int i = 0; i < 6; ++i) res_params(s, std::string("encoder.") + res[i], h->res[i], i < 3 ? h->C0 : h->C1, i < 2 ? h->C0 : h->C1);
+    h->Wds = s.take(C0 * 27 * 8 * C0);
+    h->bds = s.take(C0);
+    s.weight_bias_at("encoder.down_blocks.0.downsample", h->Wds, h->bds, {C0, C0, 3, 3, 3}, PK_CONV3_S2D);
+    attn_params(s, "encoder.mid_block.attns.0.", h->attn, h->C1, heads);
+    s.weight_bias("encoder.norm_out", h->nog, h->nob, {C1});
+    h->Wout = s.take(16 * 27 * C1);   // rows 2..15 stay zero
+    h->bout = s.take(16);
+    s.weight_bias_at("encoder.conv_out", h->Wout, h->bout, {2, C1, 3, 3, 3}, PK_CONV3);
+    h->quant = s.take(8);
+    s.weight_bias_at("quant_conv", h->quant, h->quant + 4, {2, 2, 1, 1, 1});
 }
 
 // Scratch: every activation of the encoder is 32 KB per primitive (8^3 x 32 or 4^3 x 256 fp16), so the workspace is eight such buffers.
@@ -381,45 +266,24 @@ struct EncWs {
     __half *A, *B, *T1, *T2, *Q, *K, *V, *SC;
     size_t total;
 };
-EncWs carve_ews(int P, uint8_t* base) {
+EncWs carve_ews(int P, void* base) {
+    Carve c{static_cast<uint8_t*>(base), 1024};
     EncWs w;
-    size_t off = 0;
-    auto take = [&]() {
-        uint8_t* p = base == nullptr ? nullptr : base + off;
-        off += (static_cast<size_t>(P) * 16384 * 2 + 1023) & ~static_cast<size_t>(1023);
-        return reinterpret_cast<__half*>(p);
-    };
-    w.A = take(); w.B = take(); w.T1 = take(); w.T2 = take(); w.Q = take(); w.K = take(); w.V = take(); w.SC = take();
-    w.total = off;
+    const size_t n = static_cast<size_t>(P) * 16384;
+    w.A = c.take<__half>(n); w.B = c.take<__half>(n); w.T1 = c.take<__half>(n); w.T2 = c.take<__half>(n);
+    w.Q = c.take<__half>(n); w.K = c.take<__half>(n); w.V = c.take<__half>(n); w.SC = c.take<__half>(n);
+    w.total = c.off;
     return w;
-}
-
-int check_enc_args(const tpx_vae_encoder* h, const void* x, const void* dst, int P, const void* ws, size_t ws_bytes, const char* what) {
-    TPX_CHECK(h != nullptr && x != nullptr && dst != nullptr && ws != nullptr, TPX_ERR_ARG, "%s: null argument", what);
-    TPX_CHECK(h->finalized, TPX_ERR_STATE, "%s: weights not finalized (load the encoder tensors first)", what);
-    TPX_CHECK(P > 0, TPX_ERR_SHAPE, "%s: empty batch", what);
-    const size_t need = carve_ews(P, nullptr).total;
-    TPX_CHECK(ws_bytes >= need, TPX_ERR_ARG, "%s: workspace too small (%zu < %zu)", what, ws_bytes, need);
-    TPX_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, TPX_ERR_ARG, "%s: workspace must be 256-B aligned", what);
-    return TPX_OK;
 }
 
 // The encode schedule (Encoder.forward + quant_conv, vae3d_dib.py:310-327, :431-433).  stop < 0 runs it to the end and writes the
 // moments; stop = TPX_VAE_ENC_STAGE_* ends after that stage and copies its channels-last fp16 activation into `tap`.
 // Launches: conv_in 1, 8^3 block 4 + 4, downsample 2, 32 -> 256 block 5, 256 blocks 4 each, attention 4, norm_out 1, conv_out 1: 34.
 int enc_run(tpx_vae_encoder* h, const void* x, int x_dtype, void* out, int out_dtype, int P, int stop, void* tap, void* ws, cudaStream_t st) {
-    EncWs w = carve_ews(P, static_cast<uint8_t*>(ws));
+    EncWs w = carve_ews(P, ws);
     const int C0 = h->C0, C1 = h->C1;
     const BlockScratch sc{w.T1, w.T2, w.Q, w.K, w.V};
     int rc;
-#define TPX_RC(call) do { rc = (call); if (rc != TPX_OK) return rc; } while (0)
-#define TPX_TAP(stage, act, S3, C)                                                                                                   \
-    do {                                                                                                                             \
-        if (stop == (stage)) {                                                                                                       \
-            TPX_CUDA(cudaMemcpyAsync(tap, act, static_cast<size_t>(P) * (S3) * (C) * sizeof(__half), cudaMemcpyDeviceToDevice, st)); \
-            return TPX_OK;                                                                                                           \
-        }                                                                                                                            \
-    } while (0)
     __half *X = w.A, *X2 = w.B;
     TPX_RC(launch_vae_enc_conv_in(x, x_dtype, h->Win, h->bin, P, X, st));
     TPX_TAP(TPX_VAE_ENC_STAGE_CONV_IN, X, 512, C0);
@@ -451,7 +315,7 @@ int enc_run(tpx_vae_encoder* h, const void* x, int x_dtype, void* out, int out_d
     TPX_TAP(TPX_VAE_ENC_STAGE_DOWN1_RES1, X, 64, C1);
     TPX_RC(resnet_block(h->res[4], 4, X, X2, sc, P, st));
     TPX_TAP(TPX_VAE_ENC_STAGE_MID_RES0, X, 64, C1);
-    TPX_RC(attention_block(VaeAttn{h->ang, h->anb, h->Wqkv, h->Wap, h->bap, h->heads}, X, X2, sc, P, C1, st));
+    TPX_RC(attention_block(h->attn, X, X2, sc, P, C1, st));
     TPX_TAP(TPX_VAE_ENC_STAGE_MID_ATTN, X, 64, C1);
     TPX_RC(resnet_block(h->res[5], 4, X, X2, sc, P, st));
     TPX_TAP(TPX_VAE_ENC_STAGE_MID_RES1, X, 64, C1);
@@ -484,71 +348,28 @@ int tpx_vae_create(const tpx_vae_config* c, tpx_vae** out) {
     TPX_CHECK(c->attn_heads > 0 && c->ch_mid % c->attn_heads == 0 && (c->ch_mid / c->attn_heads) == 32, TPX_ERR_SHAPE, "vae_create: attention head dim must be 32");
     TPX_DEVICE_GUARD();
     tpx_vae* h = new tpx_vae();
-    h->C0 = c->ch_mid; h->C1 = c->ch_out; h->Cout = c->out_channels; h->heads = c->attn_heads;
-    carve(h, nullptr);
-    cudaError_t e = cudaMalloc(&h->store, h->store_halves * 2);
-    if (e != cudaSuccess) { delete h; return cuda_fail(e, "cudaMalloc(vae parameter store)"); }
-    e = cudaMemset(h->store, 0, h->store_halves * 2);
-    if (e != cudaSuccess) { cudaFree(h->store); delete h; return cuda_fail(e, "cudaMemset(vae parameter store)"); }
-    carve(h, h->store);
-    auto& r = h->required;
-    for (const char* k : {"post_quant_conv.weight", "post_quant_conv.bias", "decoder.conv_in.weight", "decoder.conv_in.bias", "decoder.norm_out.weight",
-                          "decoder.norm_out.bias", "decoder.conv_out.weight", "decoder.conv_out.bias", "decoder.up_blocks.0.upsample.weight",
-                          "decoder.up_blocks.0.upsample.bias", "decoder.mid_block.attns.0.norm.weight", "decoder.mid_block.attns.0.norm.bias",
-                          "decoder.mid_block.attns.0.attn.qkv.weight", "decoder.mid_block.attns.0.attn.proj.weight",
-                          "decoder.mid_block.attns.0.attn.proj.bias"})
-        r.emplace_back(k);
-    for (int i = 0; i < 6; ++i) {
-        for (const char* k : {"norm1.weight", "norm1.bias", "conv1.weight", "conv1.bias", "norm2.weight", "norm2.bias", "conv2.weight", "conv2.bias"})
-            r.emplace_back(std::string(kResPrefix[i]) + k);
-        if (h->res[i].Wsc != nullptr) { r.emplace_back(std::string(kResPrefix[i]) + "shortcut.weight"); r.emplace_back(std::string(kResPrefix[i]) + "shortcut.bias"); }
-    }
-    h->seen.assign(r.size(), 0);
+    h->C0 = c->ch_mid; h->C1 = c->ch_out; h->Cout = c->out_channels;
+    h->params.ignored = {"encoder.", "quant_conv."};   // not on the decode path
+    const int heads = c->attn_heads;
+    const int rc = h->params.create(kSlotAlign, [h, heads](ParamStore& s) { declare_decoder(h, s, heads); });
+    if (rc != TPX_OK) { delete h; return rc; }
     *out = h;
     return TPX_OK;
 }
 
-void tpx_vae_destroy(tpx_vae* h) {
-    if (h == nullptr) return;
-    if (h->store != nullptr) cudaFree(h->store);
-    delete h;
-}
+void tpx_vae_destroy(tpx_vae* h) { delete h; }
 
 int tpx_vae_set_weight(tpx_vae* h, const char* ref_key, const void* dev_ptr, int dtype, const int64_t* shape, int ndim, void* stream) {
-    TPX_CHECK(h != nullptr && ref_key != nullptr && dev_ptr != nullptr && shape != nullptr, TPX_ERR_ARG, "vae_set_weight: null argument");
-    const std::string key(ref_key);
-    if (key.rfind("encoder.", 0) == 0 || key.rfind("quant_conv.", 0) == 0) return 1;  // not on the decode path
-    VSlot s;
-    if (!find_vslot(h, key, &s)) { set_error("vae_set_weight: unexpected key '%s'", ref_key); return TPX_ERR_KEY; }
-    bool ok = ndim == static_cast<int>(s.shape.size());
-    long long n = 1;
-    for (int i = 0; ok && i < ndim; ++i) { ok = shape[i] == s.shape[i]; n *= shape[i]; }
-    TPX_CHECK(ok, TPX_ERR_SHAPE, "vae_set_weight: size mismatch for %s", ref_key);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int rc = TPX_OK;
-    switch (s.kind) {
-        case SK_PLAIN: rc = launch_to_half(dev_ptr, dtype, s.ptr, n, st); break;
-        case SK_CONV3: rc = launch_pack_conv3(dev_ptr, dtype, s.ptr, s.a, s.b, 0, st); break;
-        case SK_CONV3_T: rc = launch_pack_conv3(dev_ptr, dtype, s.ptr, s.a, s.b, 1, st); break;   // rows >= Cout stay zero
-        case SK_CONVT2: rc = launch_pack_convt2(dev_ptr, dtype, s.ptr, s.a, s.b, st); break;
-        case SK_BIAS_REP8: {
-            rc = launch_to_half(dev_ptr, dtype, s.ptr, n, st);   // first C entries, then replicated for the 8 output offsets
-            if (rc == TPX_OK) { rep8_kernel<<<(8 * s.a + 255) / 256, 256, 0, st>>>(s.ptr, s.ptr, s.a); rc = cudaGetLastError() == cudaSuccess ? TPX_OK : TPX_ERR_CUDA; }
-            break;
-        }
-    }
-    if (rc != TPX_OK) return rc;
-    for (size_t i = 0; i < h->required.size(); ++i)
-        if (h->required[i] == key) h->seen[i] = 1;
-    h->finalized = false;
-    return TPX_OK;
+    TPX_CHECK(h != nullptr, TPX_ERR_ARG, "vae_set_weight: null argument");
+    return h->params.set("vae_set_weight", ref_key, dev_ptr, dtype, shape, ndim, static_cast<cudaStream_t>(stream));
 }
 
 int tpx_vae_finalize(tpx_vae* h, void* stream) {
     (void)stream;
     TPX_CHECK(h != nullptr, TPX_ERR_ARG, "vae_finalize: null handle");
-    for (size_t i = 0; i < h->required.size(); ++i) TPX_CHECK(h->seen[i], TPX_ERR_STATE, "vae_finalize: missing key '%s' in state_dict", h->required[i].c_str());
-    h->finalized = true;
+    const int rc = h->params.complete("vae_finalize");
+    if (rc != TPX_OK) return rc;
+    h->params.finalized = true;
     return TPX_OK;
 }
 
@@ -558,14 +379,14 @@ size_t tpx_vae_workspace_bytes(const tpx_vae* h, int P) {
 }
 
 int tpx_vae_decode(tpx_vae* h, const void* z, int z_dtype, void* out, int out_dtype, int P, void* ws, size_t ws_bytes, void* stream) {
-    const int rc = check_run_args(h, z, out, P, ws, ws_bytes, "vae_decode");
+    const int rc = check_run_args(h, tpx_vae_workspace_bytes, z, out, P, ws, ws_bytes, "vae_decode");
     if (rc != TPX_OK) return rc;
     TPX_CHECK(out_dtype == TPX_DTYPE_F32 || out_dtype == TPX_DTYPE_F16, TPX_ERR_ARG, "vae_decode: bad output dtype %d", out_dtype);
     return vae_run(h, z, z_dtype, out, out_dtype, P, -1, nullptr, ws, static_cast<cudaStream_t>(stream));
 }
 
 int tpx_vae_debug_stage(tpx_vae* h, const void* z, int z_dtype, int P, int stage, void* tap_f16, void* ws, size_t ws_bytes, void* stream) {
-    const int rc = check_run_args(h, z, tap_f16, P, ws, ws_bytes, "vae_debug_stage");
+    const int rc = check_run_args(h, tpx_vae_workspace_bytes, z, tap_f16, P, ws, ws_bytes, "vae_debug_stage");
     if (rc != TPX_OK) return rc;
     TPX_CHECK(stage >= TPX_VAE_STAGE_CONV_IN && stage <= TPX_VAE_STAGE_NORM_OUT, TPX_ERR_ARG, "vae_debug_stage: bad stage %d", stage);
     return vae_run(h, z, z_dtype, nullptr, TPX_DTYPE_F16, P, stage, tap_f16, ws, static_cast<cudaStream_t>(stream));
@@ -590,64 +411,27 @@ int tpx_vae_encoder_create(const tpx_vae_config* c, tpx_vae_encoder** out) {
     TPX_CHECK(c->attn_heads > 0 && c->ch_mid % c->attn_heads == 0 && (c->ch_mid / c->attn_heads) == 32, TPX_ERR_SHAPE, "vae_encoder_create: attention head dim must be 32");
     TPX_DEVICE_GUARD();
     tpx_vae_encoder* h = new tpx_vae_encoder();
-    h->heads = c->attn_heads;
-    carve_enc(h, nullptr);
-    cudaError_t e = cudaMalloc(&h->store, h->store_halves * 2);
-    if (e != cudaSuccess) { delete h; return cuda_fail(e, "cudaMalloc(vae encoder parameter store)"); }
-    e = cudaMemset(h->store, 0, h->store_halves * 2);
-    if (e != cudaSuccess) { cudaFree(h->store); delete h; return cuda_fail(e, "cudaMemset(vae encoder parameter store)"); }
-    carve_enc(h, h->store);
-    auto& r = h->required;
-    for (const char* k : {"encoder.conv_in.weight", "encoder.conv_in.bias", "encoder.down_blocks.0.downsample.weight", "encoder.down_blocks.0.downsample.bias",
-                          "encoder.mid_block.attns.0.norm.weight", "encoder.mid_block.attns.0.norm.bias", "encoder.mid_block.attns.0.attn.qkv.weight",
-                          "encoder.mid_block.attns.0.attn.proj.weight", "encoder.mid_block.attns.0.attn.proj.bias", "encoder.norm_out.weight",
-                          "encoder.norm_out.bias", "encoder.conv_out.weight", "encoder.conv_out.bias", "quant_conv.weight", "quant_conv.bias"})
-        r.emplace_back(k);
-    for (int i = 0; i < 6; ++i) {
-        for (const char* k : {"norm1.weight", "norm1.bias", "conv1.weight", "conv1.bias", "norm2.weight", "norm2.bias", "conv2.weight", "conv2.bias"})
-            r.emplace_back(std::string(kEncResPrefix[i]) + k);
-        if (h->res[i].Wsc != nullptr) { r.emplace_back(std::string(kEncResPrefix[i]) + "shortcut.weight"); r.emplace_back(std::string(kEncResPrefix[i]) + "shortcut.bias"); }
-    }
-    h->seen.assign(r.size(), 0);
+    h->params.ignored = {"decoder.", "post_quant_conv."};   // not on the encode path
+    const int heads = c->attn_heads;
+    const int rc = h->params.create(kSlotAlign, [h, heads](ParamStore& s) { declare_encoder(h, s, heads); });
+    if (rc != TPX_OK) { delete h; return rc; }
     *out = h;
     return TPX_OK;
 }
 
-void tpx_vae_encoder_destroy(tpx_vae_encoder* h) {
-    if (h == nullptr) return;
-    if (h->store != nullptr) cudaFree(h->store);
-    delete h;
-}
+void tpx_vae_encoder_destroy(tpx_vae_encoder* h) { delete h; }
 
 int tpx_vae_encoder_set_weight(tpx_vae_encoder* h, const char* ref_key, const void* dev_ptr, int dtype, const int64_t* shape, int ndim, void* stream) {
-    TPX_CHECK(h != nullptr && ref_key != nullptr && dev_ptr != nullptr && shape != nullptr, TPX_ERR_ARG, "vae_encoder_set_weight: null argument");
-    const std::string key(ref_key);
-    if (key.rfind("decoder.", 0) == 0 || key.rfind("post_quant_conv.", 0) == 0) return 1;  // not on the encode path
-    ESlot s;
-    if (!find_eslot(h, key, &s)) { set_error("vae_encoder_set_weight: unexpected key '%s'", ref_key); return TPX_ERR_KEY; }
-    bool ok = ndim == static_cast<int>(s.shape.size());
-    long long n = 1;
-    for (int i = 0; ok && i < ndim; ++i) { ok = shape[i] == s.shape[i]; n *= shape[i]; }
-    TPX_CHECK(ok, TPX_ERR_SHAPE, "vae_encoder_set_weight: size mismatch for %s", ref_key);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int rc = TPX_OK;
-    switch (s.kind) {
-        case EK_PLAIN: rc = launch_to_half(dev_ptr, dtype, s.ptr, n, st); break;
-        case EK_CONV3: rc = launch_pack_conv3(dev_ptr, dtype, s.ptr, static_cast<int>(s.shape[0]), static_cast<int>(s.shape[1]), 0, st); break;
-        case EK_CONV3_S2D: rc = launch_pack_conv3_s2d(dev_ptr, dtype, s.ptr, static_cast<int>(s.shape[0]), static_cast<int>(s.shape[1]), st); break;
-    }
-    if (rc != TPX_OK) return rc;
-    for (size_t i = 0; i < h->required.size(); ++i)
-        if (h->required[i] == key) h->seen[i] = 1;
-    h->finalized = false;
-    return TPX_OK;
+    TPX_CHECK(h != nullptr, TPX_ERR_ARG, "vae_encoder_set_weight: null argument");
+    return h->params.set("vae_encoder_set_weight", ref_key, dev_ptr, dtype, shape, ndim, static_cast<cudaStream_t>(stream));
 }
 
 int tpx_vae_encoder_finalize(tpx_vae_encoder* h, void* stream) {
     (void)stream;
     TPX_CHECK(h != nullptr, TPX_ERR_ARG, "vae_encoder_finalize: null handle");
-    for (size_t i = 0; i < h->required.size(); ++i) TPX_CHECK(h->seen[i], TPX_ERR_STATE, "vae_encoder_finalize: missing key '%s' in state_dict", h->required[i].c_str());
-    h->finalized = true;
+    const int rc = h->params.complete("vae_encoder_finalize");
+    if (rc != TPX_OK) return rc;
+    h->params.finalized = true;
     return TPX_OK;
 }
 
@@ -657,14 +441,14 @@ size_t tpx_vae_encoder_workspace_bytes(const tpx_vae_encoder* h, int P) {
 }
 
 int tpx_vae_encode(tpx_vae_encoder* h, const void* x, int x_dtype, void* moments_out, int out_dtype, int P, void* ws, size_t ws_bytes, void* stream) {
-    const int rc = check_enc_args(h, x, moments_out, P, ws, ws_bytes, "vae_encode");
+    const int rc = check_run_args(h, tpx_vae_encoder_workspace_bytes, x, moments_out, P, ws, ws_bytes, "vae_encode");
     if (rc != TPX_OK) return rc;
     TPX_CHECK(out_dtype == TPX_DTYPE_F32 || out_dtype == TPX_DTYPE_F16, TPX_ERR_ARG, "vae_encode: bad output dtype %d", out_dtype);
     return enc_run(h, x, x_dtype, moments_out, out_dtype, P, -1, nullptr, ws, static_cast<cudaStream_t>(stream));
 }
 
 int tpx_vae_encode_debug_stage(tpx_vae_encoder* h, const void* x, int x_dtype, int P, int stage, void* tap_f16, void* ws, size_t ws_bytes, void* stream) {
-    const int rc = check_enc_args(h, x, tap_f16, P, ws, ws_bytes, "vae_encode_debug_stage");
+    const int rc = check_run_args(h, tpx_vae_encoder_workspace_bytes, x, tap_f16, P, ws, ws_bytes, "vae_encode_debug_stage");
     if (rc != TPX_OK) return rc;
     TPX_CHECK(stage >= TPX_VAE_ENC_STAGE_CONV_IN && stage <= TPX_VAE_ENC_STAGE_NORM_OUT, TPX_ERR_ARG, "vae_encode_debug_stage: bad stage %d", stage);
     return enc_run(h, x, x_dtype, nullptr, TPX_DTYPE_F16, P, stage, tap_f16, ws, static_cast<cudaStream_t>(stream));

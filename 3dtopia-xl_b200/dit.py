@@ -168,21 +168,8 @@ class DiT(nn.Module):
         lib = _lib.lib()
         if self._sd is None:
             self._sd = self._default_init()
-        dev = self._handle_device
         released = self._resident_only
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr()
-            keep = []
-            for k, v in self._sd.items():
-                t = v.detach()
-                if t.dtype not in (torch.float16, torch.float32):
-                    t = t.float()
-                t = t.to(dev, non_blocking=True).contiguous()
-                keep.append(t)
-                shape = (C.c_int64 * t.dim())(*t.shape)
-                _lib.check(lib.tpx_dit_set_weight(self._handle, k.encode(), t.data_ptr(), _lib.dtype_tag(t), shape, t.dim(), st), f"set_weight({k})")
-            _lib.check(lib.tpx_dit_finalize(self._handle, st), "tpx_dit_finalize")
-            torch.cuda.current_stream().synchronize()
+        _lib.upload(self._handle, lib.tpx_dit_set_weight, lib.tpx_dit_finalize, self._sd.items(), self._handle_device)
         self._cond_key, self._cond_ref = None, None
         self._ts_key = None                        # the C library dropped its timestep table with the first set_weight
         if released:                               # re-ingested after a device move of a released model: release again

@@ -143,20 +143,7 @@ class VAE(nn.Module):
 
     def _ingest(self):
         lib = _lib.lib()
-        dev = self._handle_device
-        with torch.cuda.device(dev):
-            st = _lib.stream_ptr()
-            keep = []
-            for k, v in self._sd.items():
-                t = v.detach()
-                if t.dtype not in (torch.float16, torch.float32):
-                    t = t.float()
-                t = t.to(dev, non_blocking=True).contiguous()
-                keep.append(t)
-                shape = (C.c_int64 * t.dim())(*t.shape)
-                _lib.check(lib.tpx_vae_set_weight(self._handle, k.encode(), t.data_ptr(), _lib.dtype_tag(t), shape, t.dim(), st), f"set_weight({k})")
-            _lib.check(lib.tpx_vae_finalize(self._handle, st), "tpx_vae_finalize")
-            torch.cuda.current_stream().synchronize()
+        _lib.upload(self._handle, lib.tpx_vae_set_weight, lib.tpx_vae_finalize, self._sd.items(), self._handle_device)
 
     def _destroy_handle(self):
         if self.__dict__.get("_handle") is not None:
@@ -192,14 +179,16 @@ class VAE(nn.Module):
             z = z.float()
         return z.contiguous()
 
-    def _workspace(self, lib, P: int):
-        """(256-B aligned address, bytes) of the decode scratch for P primitives; the buffer is kept for the next call of the same size."""
-        nbytes = lib.tpx_vae_workspace_bytes(self._handle, P)
-        ws = self._ws.get(P)
+    def _workspace(self, lib, P: int, encoder: bool = False):
+        """(256-B aligned address, bytes) of the decode scratch for P primitives, or of the encode scratch with `encoder`; the buffer
+        is kept for the next call of the same size."""
+        cache, nbytes = ((self._enc_ws, lib.tpx_vae_encoder_workspace_bytes(self._enc_handle, P)) if encoder
+                         else (self._ws, lib.tpx_vae_workspace_bytes(self._handle, P)))
+        ws = cache.get(P)
         if ws is None:
-            self._ws.clear()
+            cache.clear()
             ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=self._handle_device)
-            self._ws[P] = ws
+            cache[P] = ws
         return (ws.data_ptr() + 255) & ~255, nbytes
 
     def decode(self, x: torch.Tensor) -> torch.Tensor:
@@ -261,22 +250,11 @@ class VAE(nn.Module):
         h = C.c_void_p()
         with torch.cuda.device(dev):
             _lib.check(lib.tpx_vae_encoder_create(C.byref(cfg), C.byref(h)), "tpx_vae_encoder_create")
-            try:
-                st = _lib.stream_ptr()
-                keep = []
-                for k in shapes:
-                    t = self._extra[k].detach()
-                    if t.dtype not in (torch.float16, torch.float32):
-                        t = t.float()
-                    t = t.to(dev, non_blocking=True).contiguous()
-                    keep.append(t)
-                    shape = (C.c_int64 * t.dim())(*t.shape)
-                    _lib.check(lib.tpx_vae_encoder_set_weight(h, k.encode(), t.data_ptr(), _lib.dtype_tag(t), shape, t.dim(), st), f"encoder set_weight({k})")
-                _lib.check(lib.tpx_vae_encoder_finalize(h, st), "tpx_vae_encoder_finalize")
-                torch.cuda.current_stream().synchronize()     # the staged tensors in `keep` are read by the repack kernels
-            except Exception:
-                lib.tpx_vae_encoder_destroy(h)
-                raise
+        try:
+            _lib.upload(h, lib.tpx_vae_encoder_set_weight, lib.tpx_vae_encoder_finalize, ((k, self._extra[k]) for k in shapes), dev)
+        except Exception:
+            lib.tpx_vae_encoder_destroy(h)
+            raise
         self._enc_handle = h
         return h
 
@@ -295,15 +273,6 @@ class VAE(nn.Module):
             raise ValueError(f"x is on {x.device}, the module on {self._handle_device}")
         return x.detach().contiguous(), self._encoder()
 
-    def _enc_workspace(self, lib, h, P: int):
-        nbytes = lib.tpx_vae_encoder_workspace_bytes(h, P)
-        ws = self._enc_ws.get(P)
-        if ws is None:
-            self._enc_ws.clear()
-            ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=self._handle_device)
-            self._enc_ws[P] = ws
-        return (ws.data_ptr() + 255) & ~255, nbytes
-
     def encode(self, x: torch.Tensor) -> DiagonalGaussianDistribution:
         """VAE.encode (vae3d_dib.py:431-435): x [P,6,8,8,8] fp32 / fp16 on the module's device -> the posterior over quant_conv(encoder(x))
         [P,2,4,4,4] in x's dtype (computed in fp16 with fp32 accumulation, as under autocast).  Enqueued on the current stream."""
@@ -313,7 +282,7 @@ class VAE(nn.Module):
         out = torch.empty(P, 2 * self.latent_channels, 4, 4, 4, dtype=x.dtype, device=x.device)
         if P > 0:
             with torch.cuda.device(x.device):
-                base, nbytes = self._enc_workspace(lib, h, P)
+                base, nbytes = self._workspace(lib, P, encoder=True)
                 _lib.check(lib.tpx_vae_encode(h, x.data_ptr(), _lib.dtype_tag(x), out.data_ptr(), _lib.dtype_tag(out), P, base, nbytes,
                                               _lib.stream_ptr()), "tpx_vae_encode")
         return DiagonalGaussianDistribution(out)
@@ -330,7 +299,7 @@ class VAE(nn.Module):
         tap = torch.empty(P, *self.ENC_STAGE_SHAPES[stage], dtype=torch.float16, device=x.device)
         if P > 0:
             with torch.cuda.device(x.device):
-                base, nbytes = self._enc_workspace(lib, h, P)
+                base, nbytes = self._workspace(lib, P, encoder=True)
                 _lib.check(lib.tpx_vae_encode_debug_stage(h, x.data_ptr(), _lib.dtype_tag(x), P, stage, tap.data_ptr(), base, nbytes,
                                                           _lib.stream_ptr()), "tpx_vae_encode_debug_stage")
         return tap
