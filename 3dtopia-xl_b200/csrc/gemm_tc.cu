@@ -183,6 +183,54 @@ static int make_output_maps(const GemmProblem& p, GemmArgs& a, const CUtensorMap
     return rc;
 }
 
+// Every instantiated (tile width, k-block, A mode, epilogue); a combination not listed has no kernel.
+#define TPX_GEMM_INSTANCES(X) \
+    /* DiT (every tile width x every DiT epilogue, so any hidden size that is a multiple of 128 works); 128 / 144: ping-pong schedule */ \
+    X(128, 64, AMODE_LINEAR, EPI_STORE) \
+    X(128, 64, AMODE_LINEAR, EPI_GELU) \
+    X(128, 64, AMODE_LINEAR, EPI_HEADS) \
+    X(128, 64, AMODE_LINEAR, EPI_GATED) \
+    X(144, 64, AMODE_LINEAR, EPI_STORE) \
+    X(144, 64, AMODE_LINEAR, EPI_GELU) \
+    X(144, 64, AMODE_LINEAR, EPI_HEADS) \
+    X(144, 64, AMODE_LINEAR, EPI_GATED) \
+    X(192, 64, AMODE_LINEAR, EPI_STORE) \
+    X(192, 64, AMODE_LINEAR, EPI_GELU) \
+    X(192, 64, AMODE_LINEAR, EPI_HEADS) \
+    X(192, 64, AMODE_LINEAR, EPI_GATED) \
+    X(256, 64, AMODE_LINEAR, EPI_STORE) \
+    X(256, 64, AMODE_LINEAR, EPI_GELU) \
+    X(256, 64, AMODE_LINEAR, EPI_HEADS) \
+    X(256, 64, AMODE_LINEAR, EPI_GATED) \
+    /* VAE */ \
+    X(256, 64, AMODE_CONV3, EPI_STORE) \
+    X(256, 64, AMODE_CONV3, EPI_RESID_SCALE) \
+    X(256, 64, AMODE_LINEAR, EPI_RESID_SCALE) \
+    X(32, 64, AMODE_CONV3, EPI_STORE) \
+    X(32, 64, AMODE_LINEAR, EPI_STORE) \
+    X(32, 32, AMODE_CONV3, EPI_STORE) \
+    X(32, 32, AMODE_CONV3, EPI_RESID_SCALE) \
+    X(16, 32, AMODE_CONV3, EPI_NCDHW) \
+    /* VAE encoder: conv1 of the 32 -> 256 block at 4^3 and its K = 32 shortcut; conv_out (2 of 16 rows) + quant_conv */ \
+    X(256, 32, AMODE_CONV3, EPI_STORE) \
+    X(256, 32, AMODE_LINEAR, EPI_STORE) \
+    X(16, 64, AMODE_CONV3, EPI_MOMENTS)
+
+static bool gemm_has_kernel(int bn, int bk, int amode, int epi) {
+#define TPX_HAS(BN_, BK_, AM_, EP_) \
+    if (bn == BN_ && bk == BK_ && amode == AM_ && epi == EP_) return true;
+    TPX_GEMM_INSTANCES(TPX_HAS)
+#undef TPX_HAS
+    return false;
+}
+
+// k-block depth: 32-channel conv operands load 64-B rows; a linear K of 32 does too where a BK = 32 kernel exists for its tile and
+// epilogue (the VAE encoder's 1x1 shortcut), and otherwise runs the BK = 64 kernel, the TMA zero-filling columns 32..63 of each row.
+static int gemm_bk(const GemmProblem& p) {
+    if (p.a_mode == AMODE_CONV3) return p.conv_C == 32 ? 32 : 64;
+    return p.K == 32 && gemm_has_kernel(p.BN, 32, p.a_mode, p.epi) ? 32 : 64;
+}
+
 template <int BN, int BK, int AMODE, int EPI>
 static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& td, const CUtensorMap& te, const GemmArgs& a,
                       cudaStream_t stream) {
@@ -205,8 +253,9 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const CUtens
 int launch_gemm(const GemmProblem& p, cudaStream_t stream) {
     TPX_CHECK(p.M > 0 && p.N > 0 && p.K > 0, TPX_ERR_SHAPE, "gemm: empty problem %d x %d x %d", p.M, p.N, p.K);
     TPX_CHECK(p.N % 8 == 0 && p.K % 8 == 0, TPX_ERR_SHAPE, "gemm: N (%d) and K (%d) must be multiples of 8", p.N, p.K);
-    // 32-channel operands (conv input or a linear K of 32, the encoder's 1x1 shortcut) load 64-B rows; everything else 128-B rows
-    const int bk = (p.a_mode == AMODE_CONV3 ? p.conv_C == 32 : p.K == 32) ? 32 : 64;
+    const int bk = gemm_bk(p);
+    TPX_CHECK(gemm_has_kernel(p.BN, bk, p.a_mode, p.epi), TPX_ERR_SHAPE, "gemm: no kernel instantiated for BN=%d BK=%d amode=%d epi=%d", p.BN, bk,
+              p.a_mode, p.epi);
     ProfScope prof(p.a_mode == AMODE_CONV3 ? PROF_CONV_GEMM : PROF_GEMM, stream);
     GemmArgs a = p.args;
     a.M = p.M;
@@ -233,47 +282,32 @@ int launch_gemm(const GemmProblem& p, cudaStream_t stream) {
 
 #define TPX_CASE(BN_, BK_, AM_, EP_) \
     if (p.BN == BN_ && bk == BK_ && p.a_mode == AM_ && p.epi == EP_) return launch_one<BN_, BK_, AM_, EP_>(ta, tb, tc, td, te, a, stream);
-    // DiT (every tile width x every DiT epilogue, so any hidden size that is a multiple of 128 works); 128 / 144: ping-pong schedule
-    TPX_CASE(128, 64, AMODE_LINEAR, EPI_STORE)
-    TPX_CASE(128, 64, AMODE_LINEAR, EPI_GELU)
-    TPX_CASE(128, 64, AMODE_LINEAR, EPI_HEADS)
-    TPX_CASE(128, 64, AMODE_LINEAR, EPI_GATED)
-    TPX_CASE(144, 64, AMODE_LINEAR, EPI_STORE)
-    TPX_CASE(144, 64, AMODE_LINEAR, EPI_GELU)
-    TPX_CASE(144, 64, AMODE_LINEAR, EPI_HEADS)
-    TPX_CASE(144, 64, AMODE_LINEAR, EPI_GATED)
-    TPX_CASE(192, 64, AMODE_LINEAR, EPI_STORE)
-    TPX_CASE(192, 64, AMODE_LINEAR, EPI_GELU)
-    TPX_CASE(192, 64, AMODE_LINEAR, EPI_HEADS)
-    TPX_CASE(192, 64, AMODE_LINEAR, EPI_GATED)
-    TPX_CASE(256, 64, AMODE_LINEAR, EPI_STORE)
-    TPX_CASE(256, 64, AMODE_LINEAR, EPI_GELU)
-    TPX_CASE(256, 64, AMODE_LINEAR, EPI_HEADS)
-    TPX_CASE(256, 64, AMODE_LINEAR, EPI_GATED)
-    // VAE
-    TPX_CASE(256, 64, AMODE_CONV3, EPI_STORE)
-    TPX_CASE(256, 64, AMODE_CONV3, EPI_RESID_SCALE)
-    TPX_CASE(256, 64, AMODE_LINEAR, EPI_RESID_SCALE)
-    TPX_CASE(32, 64, AMODE_CONV3, EPI_STORE)
-    TPX_CASE(32, 64, AMODE_LINEAR, EPI_STORE)
-    TPX_CASE(32, 32, AMODE_CONV3, EPI_STORE)
-    TPX_CASE(32, 32, AMODE_CONV3, EPI_RESID_SCALE)
-    TPX_CASE(16, 32, AMODE_CONV3, EPI_NCDHW)
-    // VAE encoder: conv1 of the 32 -> 256 block at 4^3 and its K = 32 shortcut; conv_out (2 of 16 rows) + quant_conv
-    TPX_CASE(256, 32, AMODE_CONV3, EPI_STORE)
-    TPX_CASE(256, 32, AMODE_LINEAR, EPI_STORE)
-    TPX_CASE(16, 64, AMODE_CONV3, EPI_MOMENTS)
+    TPX_GEMM_INSTANCES(TPX_CASE)
 #undef TPX_CASE
-    set_error("gemm: no kernel instantiated for BN=%d BK=%d amode=%d epi=%d", p.BN, bk, p.a_mode, p.epi);
+    set_error("gemm: no kernel instantiated for BN=%d BK=%d amode=%d epi=%d", p.BN, bk, p.a_mode, p.epi);   // unreachable: checked above
     return TPX_ERR_SHAPE;
 }
 
-int gemm_linear(const __half* A, int lda, const __half* W, int M, int N, int K, int epi, const GemmArgs& args, int tile_n, cudaStream_t st) {
-    GemmProblem p{};
+// The problem of a linear GEMM, with the checks launch_gemm makes before it touches anything: a bad shape or tile width fails here,
+// before any launch (the head-split entry clears its outputs only after this).
+static int linear_problem(const __half* A, int lda, const __half* W, int M, int N, int K, int epi, const GemmArgs& args, int tile_n, GemmProblem& p) {
+    p = GemmProblem{};
     p.A = A; p.a_mode = AMODE_LINEAR; p.lda = lda; p.W = W; p.M = M; p.N = N; p.K = K;
     p.epi = epi; p.args = args;
     TPX_CHECK(tile_n >= 0, TPX_ERR_ARG, "gemm: tile width %d (0 = automatic, or one of the instantiated widths)", tile_n);
+    TPX_CHECK(M > 0 && N > 0 && K > 0, TPX_ERR_SHAPE, "gemm: empty problem %d x %d x %d", M, N, K);
+    TPX_CHECK(N % 8 == 0 && K % 8 == 0, TPX_ERR_SHAPE, "gemm: N (%d) and K (%d) must be multiples of 8", N, K);
     p.BN = tile_n > 0 ? tile_n : gemm_pick_bn(p);
+    const int bk = gemm_bk(p);
+    TPX_CHECK(gemm_has_kernel(p.BN, bk, p.a_mode, p.epi), TPX_ERR_SHAPE, "gemm: no kernel instantiated for BN=%d BK=%d amode=%d epi=%d", p.BN, bk,
+              p.a_mode, p.epi);
+    return TPX_OK;
+}
+
+int gemm_linear(const __half* A, int lda, const __half* W, int M, int N, int K, int epi, const GemmArgs& args, int tile_n, cudaStream_t st) {
+    GemmProblem p;
+    const int rc = linear_problem(A, lda, W, M, N, K, epi, args, tile_n, p);
+    if (rc != TPX_OK) return rc;
     return launch_gemm(p, st);
 }
 
@@ -315,9 +349,18 @@ int tpx_linear_heads(const void* A, int lda, const void* W, const void* bias, vo
     a.split_cols = split_cols; a.Dh = Dh; a.DhP = DhP; a.H = H; a.Nseq = n_seq_tokens;
     a.vt_which_plus1 = transposed_which >= 0 ? transposed_which + 1 : 0;
     a.vt_ld = transposed_ld;
-    if (Dh % 24 == 0 && n_seq_tokens % 32 == 0 && n_seq_tokens > 0 && M % n_seq_tokens == 0) {
-        // bulk-store epilogue: it writes the Dh real columns only, so the padding is cleared here (the DiT forward clears its
-        // workspace once per call instead)
+    TPX_CHECK(n_seq_tokens > 0 && M % n_seq_tokens == 0, TPX_ERR_SHAPE, "linear_heads: M (%d) must be a whole number of %d-token sequences", M,
+              n_seq_tokens);
+    TPX_CHECK(transposed_which < 0 || transposed_ld >= n_seq_tokens, TPX_ERR_SHAPE, "linear_heads: transposed row length %d < %d tokens", transposed_ld,
+              n_seq_tokens);
+    const bool bulk = Dh % 24 == 0 && n_seq_tokens % 32 == 0;
+    a.heads_tma = bulk ? 1 : 0;
+    GemmProblem p;
+    const int rc = linear_problem(static_cast<const __half*>(A), lda, static_cast<const __half*>(W), M, N, K, EPI_HEADS, a, tile_n, p);
+    if (rc != TPX_OK) return rc;
+    if (bulk) {
+        // bulk-store epilogue: it writes the Dh real columns of the n_seq tokens only, so the padding is cleared here (the DiT forward
+        // clears its workspace once per call instead).  The per-thread epilogue writes the padding itself.
         void* outs[3] = {out0, out1, out2};
         const size_t per = static_cast<size_t>(M / n_seq_tokens) * H * n_seq_tokens * DhP * 2;
         for (int w = 0; w < N / split_cols && w < 3; ++w) {
@@ -325,9 +368,8 @@ int tpx_linear_heads(const void* A, int lda, const void* W, const void* bias, vo
             const size_t bytes = w == transposed_which ? static_cast<size_t>(M / n_seq_tokens) * H * DhP * transposed_ld * 2 : per;
             TPX_CUDA(cudaMemsetAsync(outs[w], 0, bytes, static_cast<cudaStream_t>(stream)));
         }
-        a.heads_tma = 1;
     }
-    return gemm_linear(static_cast<const __half*>(A), lda, static_cast<const __half*>(W), M, N, K, EPI_HEADS, a, tile_n, static_cast<cudaStream_t>(stream));
+    return launch_gemm(p, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

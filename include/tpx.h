@@ -212,7 +212,11 @@ int tpx_vae_encode_debug_stage(tpx_vae_encoder* h, const void* x_dev, int x_dtyp
 /* ------------------------------------------------------------------------------------------------------------
  * Per-kernel entry points (unit parity tests; each is one launch of one hot-path kernel)
  * ---------------------------------------------------------------------------------------------------------- */
-/* out[M,N] fp16 = act(A[M,K] W[N,K]^T + bias) ; act: 0 none (optionally * post_scale, re-rounded), 1 GELU-tanh.  tile_n: 0 = auto. */
+/* out[M,N] fp16 = act(A[M,K] W[N,K]^T + bias) ; act: 0 none (optionally * post_scale, re-rounded), 1 GELU-tanh.  tile_n: 0 = auto.
+ * For the three linear entries: K % 8 == 0 and N % 8 == 0 (any K tail is zero-filled by the TMA, K = 32 included); lda, ldo, ldx are
+ * row strides in elements with 16-B aligned rows, and only columns < K of A and [M, N] of the output are touched.  An explicit tile_n
+ * with no kernel for the epilogue (128 / 144 / 192 / 256 for every epilogue; 32 for tpx_linear with act 0 only) is TPX_ERR_SHAPE, before any
+ * launch. */
 int tpx_linear(const void* A_f16, int lda, const void* W_f16, const void* bias_f16, void* out_f16, int ldo, int M, int N, int K, int act,
                float post_scale, int tile_n, void* stream);
 /* xres[M,N] fp32 += h(gate[(row/rows_per_batch)%gate_batches, :] * h(A W^T + bias))   (DiTBlock residual, dit_crossattn.py:55-57) */
@@ -220,15 +224,18 @@ int tpx_linear_gated(const void* A_f16, int lda, const void* W_f16, const void* 
                      int rows_per_batch, float* xres, int ldx, int M, int N, int K, int tile_n, void* stream);
 /* Column-split + head-split store: col -> (which = col / split_cols, head, d); row -> (b = row / n_seq_tokens, n);
  * out{which}[b, head, n, DhP] (zero padded).  post_scale applies to which == 0 (attention.py:105).  The column group
- * `transposed_which` (-1 = none) is stored transposed as [b, head, DhP, transposed_ld] (tokens contiguous): the V operand
- * layout of tpx_attention_tc. */
+ * `transposed_which` (-1 = none) is stored transposed as [b, head, DhP, transposed_ld] (tokens contiguous, transposed_ld >= n_seq_tokens):
+ * the V operand layout of tpx_attention_tc.  M must be a whole number of sequences.  Its token columns [n_seq_tokens, transposed_ld):
+ * when Dh % 24 == 0 and n_seq_tokens % 32 == 0 (the 24-column bulk-store epilogue) every output is cleared first, so they are zero;
+ * otherwise they are left as the caller had them (tpx_attention_tc only needs them finite). */
 int tpx_linear_heads(const void* A_f16, int lda, const void* W_f16, const void* bias_f16, void* out0, void* out1, void* out2, int M, int N, int K,
                      int split_cols, int H, int Dh, int DhP, int n_seq_tokens, float post_scale, int tile_n, int transposed_which, int transposed_ld,
                      void* stream);
 /* y = LN(x; eps) * h(1 + scale) + shift -> fp16   (modulate(norm(x), shift, scale), utils.py:19-20) */
 int tpx_ln_modulate(float* x, int rows, int D, float eps, const void* shift_f16, const void* scale_f16, int mod_bstride, int rows_per_batch,
                     int mod_batches, void* out_f16, const void* pre_gate_f16, const void* pre_const_f16, int pre_row0, void* stream);
-/* memory_efficient_attention contract (attention.py:54,109): q [B,H,Nq,DhP], k/v [B,H,Nk,DhP] -> out [B,Nq,H*Dh] */
+/* memory_efficient_attention contract (attention.py:54,109): q [B,H,Nq,DhP], k/v [B,H,Nk,DhP] -> out [B,Nq,H*Dh].  Padding: q k^T runs
+ * over all DhP columns, so q and k columns d >= Dh must be zero; v columns d >= Dh never reach the output (any value, NaN included). */
 int tpx_attention(const void* q, const void* k, const void* v, void* out, int B, int H, int Nq, int Nk, int Dh, int DhP, float scale, void* stream);
 /* Same contract on the wgmma path (Dh == 72, the released model's head size, or 64): q,k [B,H,N,80]; vT = V transposed
  * [B,H,80,NkPad], NkPad % 8 == 0.  q / k columns d >= Dh must be zero (q k^T runs over all 80); vT rows d >= Dh and key columns
