@@ -13,19 +13,13 @@ from tpxl_b200 import mesh
 
 from test_decimate_host import MESHES, fin_and_pinch
 from test_gpu_mesh import _shell_module
+from parity import same_mesh
 
 pytestmark = pytest.mark.gpu
 
 
 def _cuda(V, F):
     return torch.from_numpy(np.ascontiguousarray(V, np.float32)).cuda(), torch.from_numpy(np.ascontiguousarray(F, np.int64)).cuda()
-
-
-def _same(got, want, what=""):
-    v, f = got
-    assert v.dtype == torch.float32 and f.dtype == torch.int64
-    assert torch.equal(f.cpu(), torch.from_numpy(want[1])), f"{what}: faces differ ({f.shape[0]} vs {len(want[1])})"
-    assert np.array_equal(v.cpu().numpy().view(np.int32), want[0].view(np.int32)), f"{what}: vertex bytes differ"
 
 
 def _clean(v, f, v_pct, repair=True):
@@ -37,10 +31,10 @@ def _clean(v, f, v_pct, repair=True):
 def test_clean_matches_oracle(name, v_pct):
     V, F, _ = MESHES[name]()
     dv, df = _cuda(V, F)
-    _same(mesh._weld(dv, df, v_pct / 100), oc.weld(V, F, v_pct / 100), f"{name} weld")
+    same_mesh(mesh._weld(dv, df, v_pct / 100), oc.weld(V, F, v_pct / 100), f"{name} weld")
     want = oc.clean_mesh(V, F, v_pct, 8, 5, True)
     got = _clean(dv, df, v_pct)
-    _same(got, want, f"{name} clean")
+    same_mesh(got, want, f"{name} clean")
     side = torch.cuda.Stream()
     again = _clean(dv, df, v_pct)
     side.wait_stream(torch.cuda.current_stream())
@@ -55,8 +49,8 @@ def test_clean_matches_oracle(name, v_pct):
 
 def test_repair_fin_pinch_and_numpy():
     for Vm, Fm, _ in fin_and_pinch():
-        _same(mesh._repair(*_cuda(Vm, Fm)), oc.repair(Vm, Fm), "repair")
-        _same(_clean(*_cuda(Vm, Fm), 1), oc.clean_mesh(Vm, Fm, 1, 8, 5, True), "clean")
+        same_mesh(mesh._repair(*_cuda(Vm, Fm)), oc.repair(Vm, Fm), "repair")
+        same_mesh(_clean(*_cuda(Vm, Fm), 1), oc.clean_mesh(Vm, Fm, 1, 8, 5, True), "clean")
     V, F, _ = MESHES["torus"]()
     G = np.concatenate([F, F[:5, ::-1], [[F[7, 0], F[7, 0], F[7, 2]]]])  # duplicates of either winding and a repeated index
     v, f = _clean(V, G, 1)                                               # numpy in, numpy out
@@ -80,7 +74,7 @@ def test_adversarial_sizes_complete():
     v, f = mesh._weld(*_cuda(V, F), 1.01)
     assert v.shape[0] == 0 and f.shape[0] == 0
     Vs, Fs, _ = MESHES["sphere"]()                                      # r below every edge: no merges
-    _same(mesh._weld(*_cuda(Vs, Fs), 1e-7), (Vs, Fs), "no merge")
+    same_mesh(mesh._weld(*_cuda(Vs, Fs), 1e-7), (Vs, Fs), "no merge")
 
 
 def test_shell_r128_matches_oracle():
@@ -90,8 +84,8 @@ def test_shell_r128_matches_oracle():
     info = {}
     w = mesh._weld(v0, f0, 0.01, info)
     want_w = oc.weld(V, F, 0.01)
-    _same(w, want_w, "shell weld")
-    _same(mesh._repair(*w), oc.repair(*want_w), "shell repair")
+    same_mesh(w, want_w, "shell weld")
+    same_mesh(mesh._repair(*w), oc.repair(*want_w), "shell repair")
     print(f"R=128: F {len(F)} -> welded {len(want_w[1])} in {info['rounds']} rounds")
 
 

@@ -9,19 +9,13 @@ from tpxl_b200 import _lib, mesh
 
 from test_decimate_host import MESHES, fin_and_pinch
 from test_gpu_mesh import _shell_module
+from parity import same_mesh
 
 pytestmark = pytest.mark.gpu
 
 
 def _cuda(V, F):
     return torch.from_numpy(np.ascontiguousarray(V, np.float32)).cuda(), torch.from_numpy(np.ascontiguousarray(F, np.int64)).cuda()
-
-
-def _same(got, want):
-    v, f = got
-    assert v.dtype == torch.float32 and f.dtype == torch.int64
-    assert torch.equal(f.cpu(), torch.from_numpy(want[1])), f"faces differ ({f.shape[0]} vs {len(want[1])})"
-    assert np.array_equal(v.cpu().numpy().view(np.int32), want[0].view(np.int32)), "vertex bytes differ"
 
 
 @pytest.mark.parametrize("name", sorted(MESHES))
@@ -32,7 +26,7 @@ def test_decimate_matches_oracle(name):
     for T in (len(F) // 2, len(F) // 10, 1):
         want = od.decimate(V, F, T)
         got = mesh.decimate(dv, df, T)
-        _same(got, want)
+        same_mesh(got, want)
         again = mesh.decimate(dv, df, T)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -44,12 +38,12 @@ def test_decimate_matches_oracle(name):
 
 def test_fixed_vertices_and_small_cases_match_oracle():
     for Vm, Fm, _ in fin_and_pinch():
-        _same(mesh.decimate(*_cuda(Vm, Fm), len(Fm) // 5), od.decimate(Vm, Fm, len(Fm) // 5))
+        same_mesh(mesh.decimate(*_cuda(Vm, Fm), len(Fm) // 5), od.decimate(Vm, Fm, len(Fm) // 5))
     tet_v = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0], [0, 0, 1]], np.float32)
     tet_f = np.array([[0, 2, 1], [0, 1, 3], [0, 3, 2], [1, 2, 3]])
-    _same(mesh.decimate(*_cuda(tet_v, tet_f), 0), (tet_v, tet_f))
+    same_mesh(mesh.decimate(*_cuda(tet_v, tet_f), 0), (tet_v, tet_f))
     V, F, _ = MESHES["sphere"]()
-    _same(mesh.decimate(*_cuda(V, F), len(F)), (V, F))
+    same_mesh(mesh.decimate(*_cuda(V, F), len(F)), (V, F))
     v, f = mesh.decimate(V, F, len(F) // 3)                              # numpy in, numpy out
     want = od.decimate(V, F, len(F) // 3)
     assert v.dtype == np.float64 and f.dtype == np.int64
@@ -67,7 +61,7 @@ def test_component_filter_matches_oracle(name):
     for mf, md in ((8, 0.05), (int(sizes[sizes > 0].min()) + 1, 0.0), (0, 0.4), (0, 2.0)):
         want = od.remove_small_components(V, F, mf, md)
         got = mesh.remove_small_components(dv, df, mf, md)
-        _same(got, want)
+        same_mesh(got, want)
         assert all(torch.equal(a, b) for a, b in zip(got, mesh.remove_small_components(dv, df, mf, md)))
     # many small pieces: the two spheres plus copies of a tiny tetrahedron, interleaved in face order
     tet_v = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0], [0, 0, 1]], np.float32) * 0.01
@@ -77,7 +71,7 @@ def test_component_filter_matches_oracle(name):
         Fs.append(np.array([[0, 2, 1], [0, 1, 3], [0, 3, 2], [1, 2, 3]]) + sum(len(x) for x in Vs[:-1]))
     Vc, Fc = np.concatenate(Vs), np.concatenate(Fs)
     perm = np.random.default_rng(1).permutation(len(Fc))
-    _same(mesh.remove_small_components(*_cuda(Vc, Fc[perm]), 8, 0.05), od.remove_small_components(Vc, Fc[perm], 8, 0.05))
+    same_mesh(mesh.remove_small_components(*_cuda(Vc, Fc[perm]), 8, 0.05), od.remove_small_components(Vc, Fc[perm], 8, 0.05))
 
 
 def test_invalid_input_raises():

@@ -32,6 +32,7 @@ from oracle import dinov2 as odn
 from oracle.dit import Policy, r16
 from tpxl_b200 import _lib
 from gpu_util import st
+import parity
 
 pytestmark = pytest.mark.gpu
 d = importlib.import_module("tpxl_b200.dinov2")
@@ -104,61 +105,23 @@ CASES = {
 
 
 # ---- partitions and the bound -----------------------------------------------------------------------------------------------------
-def _reduce(t, how, Dh=DH):
-    """Sum of t [S, N, C] over each partition: 1-D tensor of the partitions."""
-    S, N, C = t.shape
-    if how == "image":
-        return t.sum((1, 2))
-    if how == "block":
-        blk = torch.arange(N, device=t.device) // 128
-        return torch.zeros(S, int(blk[-1]) + 1, dtype=t.dtype, device=t.device).index_add_(1, blk, t.sum(2)).flatten()
-    if how == "channel":
-        return t.sum((0, 1))
-    if how == "class":
-        return t[:, 0].sum(1)
-    if how == "head":
-        return t.reshape(S, N, C // Dh, Dh).sum((1, 3)).flatten()
-    raise ValueError(how)
-
-
-def _ratios(ours, pol, ref, how):
-    den = _reduce(ref ** 2, how).sqrt().clamp_min(1e-30)
-    return _reduce((ours - ref) ** 2, how).sqrt() / den, _reduce((pol - ref) ** 2, how).sqrt() / den
-
-
-def _rejects(ours, pol, ref, how) -> bool:
-    o, p = _ratios(ours, pol, ref, how)
-    return bool((o > 2.5 * p + 1e-4).any())
+PARTS = {"image": parity.sequence, "block": parity.block(128), "channel": parity.channel,
+         "class": parity.tokens(torch.tensor([0] + [-1] * (NT - 1))), "head": parity.head(DH)}
 
 
 def _check(key, ours, pol, ref, parts):
-    """ours / pol / ref fp64 [S, N, C]: ours <= 2.5 x policy + 1e-4 in relative L2 against exact, per partition."""
-    assert ours.shape == ref.shape == pol.shape, (key, ours.shape, pol.shape, ref.shape)
-    assert torch.isfinite(ours).all(), key
+    """ours / pol / ref fp64 [S, N, C] against the bound (tests/parity.py) per partition named in parts; the worst ratios go to WORST."""
     worst = WORST.setdefault(key, {})
-    for how in parts:
-        o, p = _ratios(ours, pol, ref, how)
-        bad = o > 2.5 * p + 1e-4
-        assert not bool(bad.any()), (f"{key}: {how} partitions {bad.nonzero().flatten().tolist()[:8]} exceed the bound: ours "
-                                     f"{o[bad][:8].tolist()} vs policy {p[bad][:8].tolist()}")
-        worst[how] = max(worst.get(how, 0.0), float((o / (2.5 * p + 1e-4)).max()))
-
-
-def _ulp16(v):
-    """fp16 spacing at |v| (2^-24 in the subnormal range)."""
-    return torch.exp2(torch.floor(torch.log2(v.abs().clamp_min(2.0 ** -14))) - 10)
+    for how, r in parity.check(f"{key}", ours, pol, ref, {h: PARTS[h] for h in parts}).items():
+        worst[how] = max(worst.get(how, 0.0), r)
 
 
 def _check_elementwise(key, ours, pol, extra=0.0):
     """|ours - pol| <= 1 fp16 ulp of the policy's value + extra (the fp32 round-off the kernel's reduction may carry)."""
-    err = (ours.double() - pol).abs()
-    tol = _ulp16(pol) + extra
-    bad = err > tol
-    assert not bool(bad.any()), (f"{key}: {int(bad.sum())} elements off the policy by more than an ulp, e.g. at "
-                                 f"{bad.nonzero()[:4].tolist()}: {ours.double()[bad][:4].tolist()} vs {pol[bad][:4].tolist()}")
+    r, off = parity.check_elementwise(f"{key}", ours, pol, parity.ulp16(pol) + extra)
     w = WORST.setdefault(key, {})
-    w["element"] = max(w.get("element", 0.0), float((err / tol).max()))
-    w["elements off"] = w.get("elements off", 0) + int((err > 0).sum())
+    w["element"] = max(w.get("element", 0.0), r)
+    w["elements off"] = w.get("elements off", 0) + off
 
 
 def _ln_extra(x, m):
@@ -307,12 +270,13 @@ def test_bound_rejects_one_percent_errors():
                                          ("channel", k1, "mlp inc", "channel", (slice(None), slice(None), 517)),
                                          ("class token", k1, "attn inc", "class", (slice(None), 0))):
         ours, pol, ref = kept[tap]
-        assert not _rejects(ours, pol, ref, how)
+        parts = {how: PARTS[how]}
+        assert not parity.rejects(ours, pol, ref, parts)
         bad = ours.clone()
         bad[region] *= 1.01
-        o, p = _ratios(bad, pol, ref, how)
-        print(f"1 % on one {what} ({tap}): worst {how} partition at {float((o / (2.5 * p + 1e-4)).max()):.1f} x the bound")
-        assert _rejects(bad, pol, ref, how), what
+        o, p = parity.ratios(bad, pol, ref, PARTS[how])
+        print(f"1 % on one {what} ({tap}): worst {how} partition at {float((o / parity.bound(p)).max()):.1f} x the bound")
+        assert parity.rejects(bad, pol, ref, parts), what
 
 
 # ---- kernel unit tests at the encoder's shapes --------------------------------------------------------------------------------------
@@ -338,15 +302,15 @@ def test_gelu_erf_every_finite_fp16_value():
     assert x.numel() == 63488
     ours, ref = _gelu_run(x), _gelu_ref(x)
     err = (ours.double() - ref).abs()
-    assert bool((err <= _ulp16(ref)).all()), x[err > _ulp16(ref)][:8].tolist()
+    assert bool((err <= parity.ulp16(ref)).all()), x[err > parity.ulp16(ref)][:8].tolist()
     print(f"gelu_erf: {int((err > 0).sum())} of {x.numel()} finite fp16 inputs one ulp off h(gelu_fp64(x)), the rest exact")
     g = torch.Generator(device=DEV).manual_seed(11)
     x8 = (torch.randn(8, generator=g, device=DEV) * 3).half()
-    assert bool(((_gelu_run(x8).double() - _gelu_ref(x8)).abs() <= _ulp16(_gelu_ref(x8))).all())
+    assert bool(((_gelu_run(x8).double() - _gelu_ref(x8)).abs() <= parity.ulp16(_gelu_ref(x8))).all())
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     nbig = sms * 8 * 256 * 8 + 8 * 1001                # more than one grid-stride sweep: the loop wraps
     xb = (torch.randn(nbig, generator=g, device=DEV) * 3).half()
-    assert bool(((_gelu_run(xb).double() - _gelu_ref(xb)).abs() <= _ulp16(_gelu_ref(xb))).all())
+    assert bool(((_gelu_run(xb).double() - _gelu_ref(xb)).abs() <= parity.ulp16(_gelu_ref(xb))).all())
 
 
 def test_ln_modulate_d768_offset_rows():
@@ -466,8 +430,8 @@ def test_linear_gated_layerscale(K, M):
     # the fp32 accumulation may round h(acc + b) the other way where acc lies within its round-off of a rounding boundary; the gate
     # then multiplies a value one ulp away
     budget = K * 2.0 ** -24 * (A.double().abs() @ W.double().abs().t() + b.double().abs())
-    near_tie = _ulp16(r16(acc)) / 2 - (acc - r16(acc)).abs() <= budget
-    extra = (budget + near_tie * _ulp16(r16(acc))) * gate.double().abs() + 2.0 ** -23 * x.double().abs()
+    near_tie = parity.ulp16(r16(acc)) / 2 - (acc - r16(acc)).abs() <= budget
+    extra = (budget + near_tie * parity.ulp16(r16(acc))) * gate.double().abs() + 2.0 ** -23 * x.double().abs()
     _check_elementwise(("unit", f"linear_gated K {K}"), x.double() - x0.double(), inc, extra)
 
 

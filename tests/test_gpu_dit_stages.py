@@ -23,6 +23,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import parity
 import tpxl_b200
 from oracle import dit as od
 from tpxl_b200 import _lib, synth
@@ -109,44 +110,19 @@ def _inputs(c, B, seed):
 
 
 # ---- partitions and the bound ---------------------------------------------------------------------------------------------------------
-def _reduce(t, how, Dh=None):
-    """Sum of t [S, N, C] over each partition: 1-D tensor of the partitions."""
-    S, N, C = t.shape
-    if how == "row":
-        return t.sum(2).flatten()
-    if how == "sequence":
-        return t.sum((1, 2))
-    if how == "block":
-        blk = torch.arange(N, device=t.device) // 128
-        return torch.zeros(S, int(blk[-1]) + 1, dtype=t.dtype, device=t.device).index_add_(1, blk, t.sum(2)).flatten()
-    if how == "channel":
-        return t.sum((0, 1))
-    if how == "head":
-        return t.reshape(S, N, C // Dh, Dh).sum((1, 3)).flatten()
-    raise ValueError(how)
+PARTS = {"row": parity.row, "sequence": parity.sequence, "block": parity.block(128), "channel": parity.channel}
 
 
-def _ratios(ours, pol, ref, how, Dh=None):
-    """Per partition: relative L2 of ours and of the policy against exact."""
-    den = _reduce(ref ** 2, how, Dh).sqrt().clamp_min(1e-30)
-    return _reduce((ours - ref) ** 2, how, Dh).sqrt() / den, _reduce((pol - ref) ** 2, how, Dh).sqrt() / den
-
-
-def _rejects(ours, pol, ref, how, Dh=None) -> bool:
-    o, p = _ratios(ours, pol, ref, how, Dh)
-    return bool((o > 2.5 * p + 1e-4).any())
+def _parts(names, Dh=None):
+    """The partitions named: PARTS, and "head" for the attention output's Dh-wide heads."""
+    return {h: parity.head(Dh) if h == "head" else PARTS[h] for h in names}
 
 
 def _check(key, ours, pol, ref, parts, Dh=None):
-    """ours / pol / ref fp64 [S, N, C]: ours <= 2.5 x policy + 1e-4 in relative L2 against exact, per partition."""
-    assert ours.shape == ref.shape == pol.shape, (key, ours.shape, ref.shape)
+    """ours / pol / ref fp64 [S, N, C] against the bound (tests/parity.py) per partition named in parts; the worst ratios go to WORST."""
     worst = WORST.setdefault(key, {})
-    for how in parts:
-        o, p = _ratios(ours, pol, ref, how, Dh)
-        bad = o > 2.5 * p + 1e-4
-        assert not bool(bad.any()), (f"{key}: {how} partitions {bad.nonzero().flatten().tolist()[:8]} exceed the bound: ours "
-                                     f"{o[bad][:8].tolist()} vs policy {p[bad][:8].tolist()}")
-        worst[how] = max(worst.get(how, 0.0), float((o / (2.5 * p + 1e-4)).max()))
+    for how, r in parity.check(f"{key}", ours, pol, ref, _parts(parts, Dh)).items():
+        worst[how] = max(worst.get(how, 0.0), r)
 
 
 INC_PARTS = ("sequence", "block", "channel")
@@ -166,13 +142,10 @@ def _check_with_null_half(key, ours, pol, ref, B):
     if ours.shape[0] == B:
         return
     m_o, m_p, m_e = (a[B:].mean(1) for a in (ours, pol, ref))
-    ulp = torch.exp2(torch.floor(torch.log2(m_p.abs().clamp_min(2.0 ** -14))) - 10)        # fp16 spacing at the policy's value
-    tol = 2 * ulp + 2.5 * (m_p - m_e).pow(2).mean(1, keepdim=True).sqrt() + 1e-4 * m_e.pow(2).mean(1, keepdim=True).sqrt()
-    err = (m_o - m_p).abs()
-    bad = err > tol
-    assert not bool(bad.any()), (f"{key}: null-half channel means {bad.nonzero().tolist()[:8]} off the policy's by {err[bad][:8].tolist()} "
-                                 f"(allowed {tol[bad][:8].tolist()})")
-    WORST.setdefault(key, {})["null-half channel mean"] = float((err / tol).max())
+    tol = (2 * parity.ulp16(m_p) + parity.K_POLICY * (m_p - m_e).pow(2).mean(1, keepdim=True).sqrt()
+           + parity.FLOOR * m_e.pow(2).mean(1, keepdim=True).sqrt())
+    worst, _ = parity.check_elementwise(f"{key}: null-half channel means", m_o, m_p, tol)
+    WORST.setdefault(key, {})["null-half channel mean"] = worst
 
 
 # ---- oracle pieces on the kernel's taps ------------------------------------------------------------------------------------------------
@@ -343,12 +316,13 @@ def test_bound_rejects_one_percent_errors():
                                    ("128-token block", "cross", "block", (0, slice(640, 768))),
                                    ("channel", "mlp", "channel", (slice(None), slice(None), 517))):
         ours, pol, ref = kept[tap]
-        assert not _rejects(ours, pol, ref, how, Dh)
+        parts = _parts((how,), Dh)
+        assert not parity.rejects(ours, pol, ref, parts)
         bad = ours.clone()
         bad[region] *= 1.01
-        o, p = _ratios(bad, pol, ref, how, Dh)
-        print(f"1 % on one {what} ({tap}): worst {how} partition at {float((o / (2.5 * p + 1e-4)).max()):.1f} x the bound")
-        assert _rejects(bad, pol, ref, how, Dh), what
+        o, p = parity.ratios(bad, pol, ref, parts[how])
+        print(f"1 % on one {what} ({tap}): worst {how} partition at {float((o / parity.bound(p)).max()):.1f} x the bound")
+        assert parity.rejects(bad, pol, ref, parts), what
 
 
 def test_timestep_table_rows_against_fp64():

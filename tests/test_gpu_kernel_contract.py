@@ -25,6 +25,7 @@ import torch
 from oracle import contract as C
 from tpxl_b200 import _lib
 from gpu_util import st
+import parity
 
 pytestmark = pytest.mark.gpu
 
@@ -345,27 +346,13 @@ def attention_ref(q, k, v, scale):
     return o, bound, pol
 
 
-def ulp16_t(x):
-    return torch.exp2(torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14))) - 10)
-
-
 def check_attention(got, o, bound, pol, what):
-    """got [B, Nq, H, Dh] against o [B, H, Nq, Dh]."""
+    """got [B, Nq, H, Dh] against o [B, H, Nq, Dh]: per element, and per (b, head, 64-row query tile) against the policy."""
     got = got.double().permute(0, 2, 1, 3)
-    assert torch.isfinite(got).all(), f"{what}: non-finite output"
-    err = (got - o).abs()
-    lim = ulp16_t(o) + bound
-    frac = float((err / lim).max())
-    assert frac <= 1.0, f"{what}: per-element bound exceeded by {frac:.3f}x"
-    worst = 0.0
+    frac, _ = parity.check_elementwise(f"{what}: per element", got, o, parity.ulp16(o) + bound)
     B, H, Nq, Dh = o.shape
-    for t0 in range(0, Nq, 64):
-        sl = slice(t0, t0 + 64)
-        den = o[:, :, sl].norm(dim=(-1, -2)).clamp_min(1e-30)
-        ours = (got[:, :, sl] - o[:, :, sl]).norm(dim=(-1, -2)) / den
-        poli = (pol[:, :, sl] - o[:, :, sl]).norm(dim=(-1, -2)) / den
-        assert bool((ours <= 2.5 * poli + 1e-4).all()), f"{what}: query tile {t0}: {float(ours.max()):.3e} vs policy {float(poli.max()):.3e}"
-        worst = max(worst, float((ours / (2.5 * poli + 1e-4)).max()))
+    worst = parity.check(f"{what}: per query tile", *(t.reshape(B * H, Nq, Dh) for t in (got, pol, o)),
+                         {"query tile": parity.block(64)})["query tile"]
     print(f"\n{what}: worst element at {frac:.3f} of its bound, worst query tile at {worst:.3f}")
 
 

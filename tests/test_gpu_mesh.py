@@ -6,10 +6,10 @@ import numpy as np
 import pytest
 import torch
 
-import oracle
 import tpxl_b200
 from oracle import mesh as omesh
 from tpxl_b200 import _lib, mesh
+from parity import is_fp32_tie
 
 pytestmark = pytest.mark.gpu
 SHAPES = [(2, 2, 2), (3, 5, 7), (17, 31, 9), (64, 64, 64), (130, 97, 66), (128, 128, 128)]
@@ -119,18 +119,6 @@ def test_sdf_grid_and_extract_mesh_match_the_chunked_reference_path(R):
     assert err <= 2e-6, err
 
 
-def _is_fp32_tie(p, srt, S):
-    """As tests/test_gpu_primsdf.py: the two best primitives, or the two best voxels of the nearest primitive, tie within fp32."""
-    d = (p[None] - srt[:, 1:4]).norm(dim=1)
-    order = d.argsort()
-    if len(order) > 1 and float(d[order[1]] - d[order[0]]) < 4e-7 * float(d[order[0]]):
-        return True
-    k = int(order[0])
-    cand = srt[k, 1:4][None] + srt[k, 0] * oracle.primsdf.local_grid(S).double()
-    dv = (p[None] - cand).norm(dim=1).sort().values
-    return float(dv[1] - dv[0]) < 4e-7 * float(dv[0])
-
-
 def test_sdf_grid_matches_reference_fixture(golden_dir):
     fx = np.load(os.path.join(golden_dir, "primsdf_grid.npz"))
     K, R = fx["srt"].shape[0], fx["grid"].shape[0]
@@ -144,7 +132,7 @@ def test_sdf_grid_matches_reference_fixture(golden_dir):
     xx = torch.linspace(-1, 1, R).double()
     srt = torch.from_numpy(fx["srt"]).double()
     for i, j, k in zip(*np.nonzero(bad)):
-        assert _is_fp32_tie(torch.stack([xx[i], xx[j], xx[k]]), srt, 8), (i, j, k, got[i, j, k], fx["grid"][i, j, k])
+        assert is_fp32_tie(torch.stack([xx[i], xx[j], xx[k]]), srt, 8), (i, j, k, got[i, j, k], fx["grid"][i, j, k])
     # the exhaustive path (no binned lists) gives the same grid
     lib = _lib.lib()
     srt_d, feat_d = m.srt_param.data.contiguous(), m.feat_param.data.contiguous()

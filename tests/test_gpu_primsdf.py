@@ -8,6 +8,7 @@ import torch
 import oracle
 import tpxl_b200
 from tpxl_b200 import _lib
+from parity import is_fp32_tie
 
 pytestmark = pytest.mark.gpu
 TOL = dict(rtol=2e-5, atol=2e-5)   # fp32 throughout; differences are summation order / fma contraction only
@@ -33,18 +34,6 @@ def test_matches_reference_fixture(golden_dir):
     np.testing.assert_allclose(tr["sdf"].cpu().numpy()[fx["covered"]], fx["sdf"][fx["covered"]], **TOL)
 
 
-def _is_fp32_tie(p, srt, S):
-    """True if the two best primitives, or the two best voxels of the nearest primitive, tie to within fp32 resolution."""
-    d = (p[None] - srt[:, 1:4]).norm(dim=1)
-    order = d.argsort()
-    if len(order) > 1 and float(d[order[1]] - d[order[0]]) < 4e-7 * float(d[order[0]]):
-        return True
-    k = int(order[0])
-    cand = srt[k, 1:4][None] + srt[k, 0] * oracle.primsdf.local_grid(S).double()
-    dv = (p[None] - cand).norm(dim=1).sort().values
-    return float(dv[1] - dv[0]) < 4e-7 * float(dv[0])
-
-
 @pytest.mark.parametrize("K,S,n", [(1, 8, 257), (1500, 8, 3001), (2048, 8, 1000), (64, 4, 513)])
 def test_matches_oracle(K, S, n):
     """Ragged sizes; K > one staging chunk (1024); the shipped K=2048; another primitive resolution."""
@@ -62,7 +51,7 @@ def test_matches_oracle(K, S, n):
     # candidates are closer than fp32 can tell apart, which one wins is rounding, not algorithm.  Only such points may differ.
     assert bad.mean() <= 0.01, f"{bad.sum()} of {n} sdf values differ"
     for i in np.nonzero(bad)[0]:
-        assert _is_fp32_tie(x[i].double(), srt.double(), S), f"point {i}: kernel {float(out['sdf'][i])} oracle {float(ref['sdf'][i])}"
+        assert is_fp32_tie(x[i].double(), srt.double(), S), f"point {i}: kernel {float(out['sdf'][i])} oracle {float(ref['sdf'][i])}"
 
 
 def test_voxel_centres_reproduce_the_voxels():

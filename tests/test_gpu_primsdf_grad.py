@@ -1,7 +1,7 @@
 """-m gpu: PrimSDF(differentiable=True) backward (tpx_primsdf_query_backward) against the reference fixture and fp64 autograd.
 
 Bounds per gradient tensor, as for the ray-march backward: relative L2 <= 1e-4 and cosine >= 1 - 1e-6 (fp32 kernel, fp32 atomics).
-In eval mode, uncovered points whose nearest primitive or nearest voxel is an fp32 tie (_is_fp32_tie, as in test_gpu_primsdf.py)
+In eval mode, uncovered points whose nearest primitive or nearest voxel is an fp32 tie (tests/parity.py is_fp32_tie)
 take no part: their upstream gradient is zeroed on both sides (the gradient is linear in it).
 Measured on one H100 80GB HBM3 (700 W): worst 3.1e-5 relative L2 against the fixture (grad_srt of the primsdf.npz scene; the
 fixture is the reference's own fp32 CPU arithmetic), 8.4e-6 against fp64 autograd (K = 5000, S = 4); 1 - cosine <= 4.8e-10.
@@ -15,6 +15,7 @@ import torch
 import oracle
 import tpxl_b200
 from oracle import primsdf_grad as pg
+from parity import is_fp32_tie
 from test_primsdf_grad_host import GRADS, scene, want
 
 pytestmark = pytest.mark.gpu
@@ -39,22 +40,11 @@ def _kernel_grads(m, x, G, need=(True, True, True)):
     return out.detach(), dict(zip(GRADS, [None if t.grad is None else t.grad.cpu() for t in (x, m.srt_param, m.feat_param)]))
 
 
-def _is_fp32_tie(p, srt, S):
-    d = (p[None] - srt[:, 1:4]).norm(dim=1)
-    order = d.argsort()
-    if len(order) > 1 and float(d[order[1]] - d[order[0]]) < 4e-7 * float(d[order[0]]):
-        return True
-    k = int(order[0])
-    cand = srt[k, 1:4][None] + srt[k, 0] * oracle.primsdf.local_grid(S).double()
-    dv = (p[None] - cand).norm(dim=1).sort().values
-    return float(dv[1] - dv[0]) < 4e-7 * float(dv[0])
-
-
 def _tie_mask(x, srt, S):
     """Uncovered points with an fp32 tie in the eval-mode fill."""
     xd, sd = x.double(), srt.double()
     cov = ((1 - ((xd[:, None] - sd[None, :, 1:4]) / sd[None, :, :1]).abs().amax(-1)) > 0).any(1)
-    return torch.tensor([bool(not c and _is_fp32_tie(p, sd, S)) for p, c in zip(xd, cov)], dtype=torch.bool)
+    return torch.tensor([bool(not c and is_fp32_tie(p, sd, S)) for p, c in zip(xd, cov)], dtype=torch.bool)
 
 
 def _compare(got, ref, tag):

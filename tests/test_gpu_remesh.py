@@ -10,6 +10,7 @@ from tpxl_b200 import _lib, mesh
 
 from test_decimate_host import MESHES
 from test_gpu_mesh import _shell_module
+from parity import same_mesh
 from test_remesh_host import _closed_oriented, _euler_per_component, _mean_edge, _shares
 
 pytestmark = pytest.mark.gpu
@@ -17,13 +18,6 @@ pytestmark = pytest.mark.gpu
 
 def _cuda(V, F):
     return torch.from_numpy(np.ascontiguousarray(V, np.float32)).cuda(), torch.from_numpy(np.ascontiguousarray(F, np.int64)).cuda()
-
-
-def _same(got, want, what=""):
-    v, f = got
-    assert v.dtype == torch.float32 and f.dtype == torch.int64
-    assert torch.equal(f.cpu(), torch.from_numpy(want[1])), f"{what}: faces differ ({f.shape[0]} vs {len(want[1])})"
-    assert np.array_equal(v.cpu().numpy().view(np.int32), want[0].view(np.int32)), f"{what}: vertex bytes differ"
 
 
 @pytest.mark.parametrize("name", sorted(MESHES))
@@ -35,7 +29,7 @@ def test_remesh_matches_oracle(name, scale, iterations):
     want = orm.remesh(V, F, L, iterations)
     dv, df = _cuda(V, F)
     got = mesh.remesh(dv, df, L, iterations)
-    _same(got, want, f"{name} L={L:.4g} it={iterations}")
+    same_mesh(got, want, f"{name} L={L:.4g} it={iterations}")
     side = torch.cuda.Stream()
     again = mesh.remesh(dv, df, L, iterations)
     side.wait_stream(torch.cuda.current_stream())

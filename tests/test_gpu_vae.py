@@ -14,6 +14,7 @@ import oracle
 import tpxl_b200
 from tpxl_b200 import _lib, synth
 from gpu_util import rel_l2, st
+import parity
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -56,7 +57,7 @@ def test_decode_against_reference_fixture(golden_dir):
     print(r)
     assert out.dtype == torch.float32 and out16.dtype == torch.float16 and out.shape == (4, 6, 8, 8, 8) and out.is_contiguous()
     assert r["ours_vs_ref32"] < 1e-2 and r["half_io"] < 1e-2
-    assert r["ours_vs_ref32"] < 2.5 * r["oracle16_vs_ref32"] + 1e-4
+    assert r["ours_vs_ref32"] < parity.bound(r["oracle16_vs_ref32"])
     out.mul_(2)   # caller mutates the result in place (inference.py:345-346): must be a fresh, writable tensor
 
 

@@ -20,6 +20,7 @@ from oracle import vae as ov
 from oracle.dit import Policy
 from tpxl_b200 import _lib, synth
 from gpu_util import rel_l2, st
+import parity
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -51,39 +52,11 @@ def _stage(k: int, sd, x, pol: Policy):
     return ov._convT(pol, x, sd[d + "conv_out.weight"], sd[d + "conv_out.bias"], stride=1, padding=1)
 
 
-def _to_ncdhw(tap):
-    P, S3, C = tap.shape
-    S = round(S3 ** (1 / 3))
-    return tap.reshape(P, S, S, S, C).permute(0, 4, 1, 2, 3)
-
-
-def _to_cl(x):
-    P, C = x.shape[:2]
-    return x.permute(0, 2, 3, 4, 1).reshape(P, -1, C)
-
-
-def _voxel_class(S: int):
-    """[S^3] int: number of coordinates on the volume's boundary (3 corner, 2 edge, 1 face, 0 interior), voxel v = (z*S + y)*S + x."""
-    i = torch.arange(S, device=DEV)
-    b = ((i == 0) | (i == S - 1)).long()
-    return (b[:, None, None] + b[None, :, None] + b[None, None, :]).reshape(-1)
-
-
 def _check_against_bound(name, ours, pol, ref):
-    """ours / pol / ref: [P, S^3, C] fp64.  Relative L2 against ref, per primitive, per voxel class and per channel."""
-    e2, p2, r2 = (ours - ref) ** 2, (pol - ref) ** 2, ref ** 2
-    cls = _voxel_class(round(ref.shape[1] ** (1 / 3)))
-    splits = {"primitive": lambda t: t.sum((1, 2)), "channel": lambda t: t.sum((0, 1)),
-              "class": lambda t: torch.stack([t[:, cls == c].sum() for c in range(4)])}
-    worst = {}
-    for how, red in splits.items():
-        den = red(r2).sqrt().clamp_min(1e-30)
-        o, p = red(e2).sqrt() / den, red(p2).sqrt() / den
-        bad = o > 2.5 * p + 1e-4
-        assert not bool(bad.any()), (f"{name}: {how} {bad.nonzero().flatten().tolist()[:8]} exceed the bound: ours {o[bad][:8].tolist()} "
-                                     f"vs policy {p[bad][:8].tolist()}")
-        worst[how] = float((o / (2.5 * p + 1e-4)).max())
-    return worst
+    """ours / pol / ref: [P, S^3, C] fp64.  The bound (tests/parity.py) per primitive, per channel and per voxel class (how many
+    coordinates lie on the volume's boundary)."""
+    cls = parity.boundary_count(round(ref.shape[1] ** (1 / 3)))
+    return parity.check(name, ours, pol, ref, {"primitive": parity.sequence, "channel": parity.channel, "class": parity.pooled(cls)})
 
 
 @pytest.fixture(scope="module")
@@ -127,15 +100,15 @@ def test_stage_local_parity(decoder, P, zdt):
                     assert torch.equal(vae.debug_stage(z[idx].contiguous(), k), tap[idx]), k
             else:
                 outs = {dt: _decode_raw(vae, z, dt) for dt in (torch.float32, torch.float16)}
-            ref = _to_cl(_stage(k, sd, prev, f64))
-            pol = _to_cl(_stage(k, sd, prev, f16))
+            ref = parity.to_cl(_stage(k, sd, prev, f64))
+            pol = parity.to_cl(_stage(k, sd, prev, f16))
             if k < N_STAGES:
                 print(f"stage {k}: activation rms {float(got.pow(2).mean().sqrt()):.3f}")
                 worst[k] = _check_against_bound(f"stage {k}", got, pol, ref)
-                prev = _to_ncdhw(got)
+                prev = parity.to_ncdhw(got)
             else:
                 for dt, o in outs.items():
-                    worst[f"out {dt}"] = _check_against_bound(f"decode output {dt}", _to_cl(o[idx].double()), pol, ref)
+                    worst[f"out {dt}"] = _check_against_bound(f"decode output {dt}", parity.to_cl(o[idx].double()), pol, ref)
     print({k: {h: round(v, 3) for h, v in w.items()} for k, w in worst.items()})
 
 
@@ -187,8 +160,8 @@ def test_upsample_one_hot_fills_its_sub_lattice(decoder, synth_sd, ci, co, abc):
     z = z_all[:3].contiguous()
     vae = _one_hot_decoder(synth_sd, "decoder.up_blocks.0.upsample.weight", (ci, co, *abc))
     with torch.no_grad():
-        x = _to_ncdhw(vae.debug_stage(z, 5))
-        u = _to_ncdhw(vae.debug_stage(z, 6))
+        x = parity.to_ncdhw(vae.debug_stage(z, 5))
+        u = parity.to_ncdhw(vae.debug_stage(z, 6))
     want = torch.zeros_like(u)
     a, b, c = abc
     want[:, co, a::2, b::2, c::2] = x[:, ci]
@@ -205,7 +178,7 @@ def test_conv_out_one_hot_is_a_flipped_shift(decoder, synth_sd, ci, co, tap, odt
     z = z_all[:3].contiguous()
     vae = _one_hot_decoder(synth_sd, "decoder.conv_out.weight", (ci, co, *tap))
     with torch.no_grad():
-        x = _to_ncdhw(vae.debug_stage(z, 9)).float()
+        x = parity.to_ncdhw(vae.debug_stage(z, 9)).float()
         out = _decode_raw(vae, z, odt).float()
     want = torch.zeros_like(out)
     kz, ky, kx = tap
@@ -226,7 +199,7 @@ def test_conv_in_one_hot_is_a_shift(decoder, synth_sd, co, tap, zdt):
     sd["post_quant_conv.weight"], sd["post_quant_conv.bias"] = torch.ones(1, 1, 1, 1, 1), torch.zeros(1)
     vae = _one_hot_decoder(sd, "decoder.conv_in.weight", (co, 0, *tap))
     with torch.no_grad():
-        got = _to_ncdhw(vae.debug_stage(z, 0))
+        got = parity.to_ncdhw(vae.debug_stage(z, 0))
     want = torch.zeros_like(got)
     kz, ky, kx = tap
     src = F.pad(z[:, 0].half(), (1, 1, 1, 1, 1, 1))
