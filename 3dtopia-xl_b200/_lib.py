@@ -179,6 +179,72 @@ def dtype_tag(t: torch.Tensor) -> int:
     raise TpxError(f"unsupported tensor dtype {t.dtype} (fp32 / fp16 only)")
 
 
+class Handle:
+    """Owner of one C handle, made by ``create(&cfg, &h)`` on `dev`.  ``ptr`` is what the C entries take, and ctypes passes the owner
+    itself as ``ptr`` (NULL once closed).  ``close()`` runs the given `destroy` at most once and never raises; dropping the owner closes
+    it, also at interpreter shutdown (nothing is looked up then)."""
+
+    def __init__(self, create, destroy, cfg, dev: torch.device):
+        self.ptr, self._destroy = None, destroy
+        h = C.c_void_p()
+        with torch.cuda.device(dev):
+            check(create(C.byref(cfg), C.byref(h)), create.__name__)
+        self.ptr = h
+
+    def close(self) -> None:
+        h, self.ptr = self.ptr, None
+        if h is not None:
+            try:
+                self._destroy(h)
+            except Exception:
+                pass
+
+    __del__ = close
+
+    @property
+    def _as_parameter_(self):
+        return self.ptr
+
+
+class Scratch:
+    """A device byte buffer that only grows: ``get(nbytes)`` returns (256-B aligned address, nbytes) inside it."""
+
+    def __init__(self, dev: torch.device):
+        self.dev, self.buf, self.addr = dev, None, 0
+
+    def get(self, nbytes: int) -> tuple[int, int]:
+        if self.buf is None or self.buf.numel() < nbytes + 256:
+            self.buf = None                     # the old buffer goes back to the allocator before the larger one is taken
+            self.buf = torch.empty(nbytes + 256, dtype=torch.uint8, device=self.dev)
+            self.addr = (self.buf.data_ptr() + 255) & ~255
+        return self.addr, nbytes
+
+
+def check_state_dict(owner: str, shapes, state_dict, strict: bool, ignore_prefixes=()) -> tuple[list, list]:
+    """The key and shape checks of nn.Module.load_state_dict against a (key -> shape) table: returns (missing, unexpected) and raises
+    torch's RuntimeError on a size mismatch, or on missing / unexpected keys when `strict`.  Keys under `ignore_prefixes` are never
+    unexpected."""
+    missing = [k for k in shapes if k not in state_dict]
+    unexpected = [k for k in state_dict if k not in shapes and not k.startswith(ignore_prefixes)]
+    errs = [f"size mismatch for {k}: copying a param with shape {tuple(state_dict[k].shape)}, expected {tuple(s)}"
+            for k, s in shapes.items() if k in state_dict and tuple(state_dict[k].shape) != tuple(s)]
+    if strict and (missing or unexpected):
+        errs.append(f"Missing key(s): {missing[:5]}{'...' if len(missing) > 5 else ''}; unexpected key(s): {unexpected[:5]}")
+    if errs:
+        raise RuntimeError(f"Error(s) in loading state_dict for {owner}:\n\t" + "\n\t".join(errs))
+    return missing, unexpected
+
+
+def read_checkpoint(path: str, key: str | None):
+    """``torch.load(path, map_location='cpu')[key]`` (the whole file when `key` is None), memory-mapped so that a tensor is read only
+    when it is used."""
+    try:
+        ck = torch.load(path, map_location="cpu", mmap=True, weights_only=True)
+    except (RuntimeError, ValueError, TypeError):      # legacy (non-zipfile) serialisation cannot be memory-mapped
+        ck = torch.load(path, map_location="cpu", weights_only=True)
+    return ck[key] if key is not None else ck
+
+
 def upload(handle, set_weight, finalize, tensors, dev: torch.device) -> None:
     """Load (key, tensor) pairs into a parameter handle on `dev` through its tpx_*_set_weight and tpx_*_finalize.  Each tensor is
     staged as a contiguous fp16 / fp32 copy on the device; the stream is synchronised before the staged copies are dropped, since

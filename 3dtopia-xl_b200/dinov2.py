@@ -86,12 +86,7 @@ class Dinov2Wrapper(nn.Module):
         state_dict = {k: v for k, v in state_dict.items() if "mask_token" not in k}      # dropped by the reference too (hub/backbones.py)
         if state_dict and not any(k.startswith("model.") for k in state_dict):           # a hub checkpoint of the bare ViT (no wrapper prefix)
             state_dict = {"model." + k: v for k, v in state_dict.items()}
-        missing = [k for k in self._shapes if k not in state_dict]
-        unexpected = [k for k in state_dict if k not in self._shapes]
-        bad = [k for k, shp in self._shapes.items() if k in state_dict and tuple(state_dict[k].shape) != tuple(shp)]
-        if bad or (strict and (missing or unexpected)):
-            raise RuntimeError(f"Error(s) in loading state_dict for Dinov2Wrapper: size mismatch {bad[:4]}, missing {missing[:4]}, "
-                               f"unexpected {unexpected[:4]}")
+        missing, unexpected = _lib.check_state_dict("Dinov2Wrapper", self._shapes, state_dict, strict)
         cur = self.state_dict()
         self._sd = OrderedDict((k, state_dict[k].detach() if k in state_dict else cur[k]) for k in self._shapes)
         self._dev_w = None

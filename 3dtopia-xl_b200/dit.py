@@ -50,14 +50,14 @@ class DiT(nn.Module):
         # one tiny real parameter so `.to(device)`, `next(model.parameters()).device` (gaussian_diffusion.py:669) work
         self._anchor = nn.Parameter(torch.zeros(1), requires_grad=False)
         self._sd: Optional["OrderedDict[str, torch.Tensor]"] = None
-        self._handle = None
+        self._handle: Optional[_lib.Handle] = None
         self._handle_device = None
-        self._ws: Dict[int, torch.Tensor] = {}
-        self._cond_ws: Optional[torch.Tensor] = None
+        self._ws: Dict[int, _lib.Scratch] = {}          # one per sequence count: debug_tap reads the one the last forward used
+        self._cond_ws: Optional[_lib.Scratch] = None
         self._cond_key = None
         self._resident_only = False                     # True once the host copy was released (release_state_dict / load_checkpoint)
         self._cond_ref: Optional[torch.Tensor] = None   # strong reference to the cached y: its address cannot be recycled while cached
-        self._ts_ws: Optional[torch.Tensor] = None      # timestep table (set_timesteps): modulation rows of a schedule's timesteps
+        self._ts_ws: Optional[_lib.Scratch] = None      # timestep table (set_timesteps): modulation rows of a schedule's timesteps
         self._ts_key: Optional[tuple] = None
         self.collapse_null_branch = True     # set False to run the null half through real cross-attention (tests)
 
@@ -110,27 +110,13 @@ class DiT(nn.Module):
         checkpoints such as model_sview_dit_fp16.pt are copied, never widened to fp32 modules), and with ``retain=False`` nothing but
         the packed store is kept.  The model must already be on its GPU (``.to('cuda')``)."""
         self._require_handle()
-        try:
-            ck = torch.load(path, map_location="cpu", mmap=True, weights_only=True)
-        except (RuntimeError, ValueError, TypeError):      # legacy (non-zipfile) serialisation cannot be memory-mapped
-            ck = torch.load(path, map_location="cpu", weights_only=True)
-        sd = ck[key] if key is not None else ck
-        out = self.load_state_dict(sd)                     # validates keys / shapes, ingests tensor by tensor
+        out = self.load_state_dict(_lib.read_checkpoint(path, key))      # validates keys / shapes, ingests tensor by tensor
         if not retain:
             self.release_state_dict()
         return out
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
-        missing = [k for k in self._shapes if k not in state_dict]
-        unexpected = [k for k in state_dict if k not in self._shapes]
-        errs = []
-        for k, shp in self._shapes.items():
-            if k in state_dict and tuple(state_dict[k].shape) != tuple(shp):
-                errs.append(f"size mismatch for {k}: copying a param with shape {tuple(state_dict[k].shape)}, expected {tuple(shp)}")
-        if strict and (missing or unexpected):
-            errs.append(f"Missing key(s): {missing[:5]}{'...' if len(missing) > 5 else ''}; unexpected key(s): {unexpected[:5]}")
-        if errs:
-            raise RuntimeError("Error(s) in loading state_dict for DiT:\n\t" + "\n\t".join(errs))
+        missing, unexpected = _lib.check_state_dict("DiT", self._shapes, state_dict, strict)
         base = self._sd if self._sd is not None else ((self._export_all() if self._resident_only and self._handle is not None else self._default_init()) if missing else OrderedDict())
         sd = OrderedDict()
         for k in self._shapes:
@@ -152,16 +138,13 @@ class DiT(nn.Module):
         if self._sd is None and self._resident_only and self._handle is not None:
             self._sd = self._export_all()          # moving a released model to another GPU: carry the packed values over
             torch.cuda.synchronize(self._handle_device)
-        self._destroy_handle()
+        self._handle = None                        # the old handle is freed before the new one is made
         cfg = _lib.DitConfig(self.seq_length, self.in_channels, self.out_channels, self.condition_channels, self.hidden_size, self.depth,
                              self.num_heads, self.mlp_hidden)
-        h = C.c_void_p()
-        with torch.cuda.device(dev):
-            _lib.check(lib.tpx_dit_create(C.byref(cfg), C.byref(h)), "tpx_dit_create")
-        self._handle, self._handle_device = h, dev
+        self._handle, self._handle_device = _lib.Handle(lib.tpx_dit_create, lib.tpx_dit_destroy, cfg, dev), dev
         self._ws.clear()
-        self._cond_ws, self._cond_key, self._cond_ref = None, None, None
-        self._ts_ws, self._ts_key = None, None
+        self._cond_ws, self._cond_key, self._cond_ref = _lib.Scratch(dev), None, None
+        self._ts_ws, self._ts_key = _lib.Scratch(dev), None
         self._ingest()
 
     def _ingest(self):
@@ -175,33 +158,16 @@ class DiT(nn.Module):
         if released:                               # re-ingested after a device move of a released model: release again
             self._sd = None
 
-    def _destroy_handle(self):
-        if self.__dict__.get("_handle") is not None:
-            try:
-                _lib.load_library().tpx_dit_destroy(self._handle)
-            except Exception:
-                pass
-            self.__dict__["_handle"] = None      # not nn.Module.__setattr__: this also runs at interpreter shutdown
-
-    def __del__(self):
-        self._destroy_handle()
-
     # ---- forward -------------------------------------------------------------------------------------------
     def _require_handle(self):
         if self._handle is None:
             raise _lib.TpxError("DiT is not on a CUDA device: call .to('cuda') first (this implementation has no CPU path)")
 
-    def _workspace(self, n_seq: int) -> torch.Tensor:
-        ws = self._ws.get(n_seq)
-        if ws is None:
-            nbytes = _lib.lib().tpx_dit_workspace_bytes(self._handle, n_seq)
-            ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=self._handle_device)
-            self._ws[n_seq] = ws
-        return ws
-
-    @staticmethod
-    def _aligned(t: torch.Tensor) -> int:
-        return (t.data_ptr() + 255) & ~255
+    def _workspace(self, n_seq: int):
+        """(aligned address, bytes) of the workspace of n_seq sequences."""
+        if n_seq not in self._ws:
+            self._ws[n_seq] = _lib.Scratch(self._handle_device)
+        return self._ws[n_seq].get(_lib.lib().tpx_dit_workspace_bytes(self._handle, n_seq))
 
     def _set_cond(self, y: torch.Tensor, with_null: bool):
         """(Re)compute the hoisted cross-attention K/V when the conditioning tensor changed.
@@ -218,10 +184,9 @@ class DiT(nn.Module):
             null = self._param("null_cond_embedding").to(self._handle_device, torch.float32)
             yy = torch.cat([yy, null.expand_as(yy)], dim=0).contiguous()
         n_cross, M = yy.shape[0], yy.shape[1]
-        nbytes = lib.tpx_dit_cond_bytes(self._handle, n_cross, M)
-        if self._cond_ws is None or self._cond_ws.numel() < nbytes + 256:
-            self._cond_ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=self._handle_device)
-        _lib.check(lib.tpx_dit_set_cond(self._handle, yy.data_ptr(), n_cross, M, self._aligned(self._cond_ws), nbytes, _lib.stream_ptr()), "tpx_dit_set_cond")
+        self._cond_key = None                      # the store is rewritten below, and may move
+        ws, nbytes = self._cond_ws.get(lib.tpx_dit_cond_bytes(self._handle, n_cross, M))
+        _lib.check(lib.tpx_dit_set_cond(self._handle, yy.data_ptr(), n_cross, M, ws, nbytes, _lib.stream_ptr()), "tpx_dit_set_cond")
         self._cond_key, self._cond_ref = key, y
 
     def set_timesteps(self, timesteps: Sequence[int], force: bool = False) -> None:
@@ -240,11 +205,10 @@ class DiT(nn.Module):
             nbytes = lib.tpx_dit_timesteps_bytes(self._handle, len(ts))
             if nbytes == 0:
                 raise _lib.TpxError(f"set_timesteps: {len(ts)} timesteps is outside what the table holds (1..4096)")
-            if self._ts_ws is None or self._ts_ws.numel() < nbytes + 256:
-                self._ts_ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=self._handle_device)
             self._ts_key = None
+            ws, nbytes = self._ts_ws.get(nbytes)
             arr = (C.c_int64 * len(ts))(*ts)
-            _lib.check(lib.tpx_dit_set_timesteps(self._handle, arr, len(ts), self._aligned(self._ts_ws), nbytes, _lib.stream_ptr()), "tpx_dit_set_timesteps")
+            _lib.check(lib.tpx_dit_set_timesteps(self._handle, arr, len(ts), ws, nbytes, _lib.stream_ptr()), "tpx_dit_set_timesteps")
         self._ts_key = ts
 
     def _prepare(self, x, t, y, use_cfg: int):
@@ -259,7 +223,6 @@ class DiT(nn.Module):
             raise _lib.TpxError(f"batch of {x.shape[0]} samples per forward: the H100 DiT handle runs 1..8 samples (2..16 sequences under CFG) per call; split larger batches")
         if use_cfg and self.cond_drop_prob <= 0:
             raise AttributeError("'DiT' object has no attribute 'null_cond_embedding'")   # as the reference would (dit_crossattn.py:208)
-        lib = _lib.lib()
         B = x.shape[0]
         xx = x.detach().to(self._handle_device, torch.float32).contiguous()
         tt = t.detach().to(self._handle_device, torch.int64).contiguous()
@@ -267,7 +230,7 @@ class DiT(nn.Module):
             raise ValueError(f"t must have shape [{B}], got {tuple(tt.shape)}")
         self._set_cond(y, with_null=(use_cfg == 2))
         n_seq = 2 * B if use_cfg else B
-        return xx, tt, n_seq, self._aligned(self._workspace(n_seq)), lib.tpx_dit_workspace_bytes(self._handle, n_seq)
+        return xx, tt, n_seq, *self._workspace(n_seq)
 
     def _run(self, x, t, y, use_cfg: int, cfg_scale: float, enable_amp: bool, t_host: Optional[int] = None):
         lib = _lib.lib()
@@ -341,7 +304,7 @@ class DiT(nn.Module):
                         "pre_cfg": ((count, N, self.out_channels), torch.float16)}[which]
         out = torch.empty(shape, dtype=dtype, device=self._handle_device)
         with torch.cuda.device(self._handle_device):
-            _lib.check(_lib.lib().tpx_dit_debug_tap(self._handle, self._aligned(self._workspace(n_seq)), n_seq, self.TAPS[which], count, out.data_ptr(),
+            _lib.check(_lib.lib().tpx_dit_debug_tap(self._handle, self._workspace(n_seq)[0], n_seq, self.TAPS[which], count, out.data_ptr(),
                                                     _lib.stream_ptr()), "tpx_dit_debug_tap")
         return out
 
@@ -349,9 +312,10 @@ class DiT(nn.Module):
         """The modulation rows [K, Ltot] fp16 that set_timesteps computed, one per timestep in its order (a view of the table)."""
         if self._ts_key is None:
             raise _lib.TpxError("debug_timestep_table: no timestep table (call set_timesteps)")
-        off = self._aligned(self._ts_ws) - self._ts_ws.data_ptr()       # the table opens the store (tpx_dit_set_timesteps)
+        ws = self._ts_ws
+        off = ws.addr - ws.buf.data_ptr()                                # the table opens the store (tpx_dit_set_timesteps)
         K, Ltot = len(self._ts_key), self.depth * 9 * self.hidden_size + 2 * self.hidden_size
-        return self._ts_ws[off:off + K * Ltot * 2].view(torch.float16).view(K, Ltot)
+        return ws.buf[off:off + K * Ltot * 2].view(torch.float16).view(K, Ltot)
 
     def debug_residual(self, n_seq: int) -> torch.Tensor:
         """fp32 residual stream [n_seq, N, D] left by the last forward (parity tests)."""

@@ -9,7 +9,6 @@ from ``load_state_dict`` and uploaded to a handle of their own on the first ``en
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 from collections import OrderedDict
 from typing import Optional
@@ -81,11 +80,11 @@ class VAE(nn.Module):
         self._anchor = nn.Parameter(torch.zeros(1), requires_grad=False)
         self._sd: Optional["OrderedDict[str, torch.Tensor]"] = None
         self._extra = OrderedDict()   # encoder.* / quant_conv.* tensors, kept only so state_dict() round-trips
-        self._handle = None
+        self._handle: Optional[_lib.Handle] = None
         self._handle_device = None
-        self._ws = {}
-        self._enc_handle = None     # created and filled on the first encode after load_state_dict / .to()
-        self._enc_ws = {}
+        self._ws: Optional[_lib.Scratch] = None
+        self._enc_handle: Optional[_lib.Handle] = None      # created and filled on the first encode after load_state_dict / .to()
+        self._enc_ws: Optional[_lib.Scratch] = None
 
     def state_dict(self, *args, **kwargs):
         if self._sd is None:
@@ -95,17 +94,10 @@ class VAE(nn.Module):
         return out
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
-        missing = [k for k in self._shapes if k not in state_dict]
-        unexpected = [k for k in state_dict if k not in self._shapes and not k.startswith(("encoder.", "quant_conv."))]
-        errs = [f"size mismatch for {k}: copying a param with shape {tuple(state_dict[k].shape)}, expected {tuple(s)}"
-                for k, s in self._shapes.items() if k in state_dict and tuple(state_dict[k].shape) != tuple(s)]
-        if strict and (missing or unexpected):
-            errs.append(f"Missing key(s): {missing[:5]}; unexpected key(s): {unexpected[:5]}")
-        if errs:
-            raise RuntimeError("Error(s) in loading state_dict for VAE:\n\t" + "\n\t".join(errs))
+        missing, unexpected = _lib.check_state_dict("VAE", self._shapes, state_dict, strict, _ENCODER_PREFIXES)
         self._sd = OrderedDict((k, state_dict[k].detach()) for k in self._shapes if k in state_dict)
         self._extra = OrderedDict((k, v) for k, v in state_dict.items() if k.startswith(_ENCODER_PREFIXES))
-        self._destroy_encoder()
+        self._enc_handle = None
         if self._handle is not None:
             self._ingest()
         return torch.nn.modules.module._IncompatibleKeys(missing, unexpected)
@@ -114,11 +106,7 @@ class VAE(nn.Module):
         """``vae.load_state_dict(torch.load(path, map_location='cpu')['model_state_dict'])`` (inference.py:257-258) from a memory-mapped
         file: only decoder.* / post_quant_conv.* tensors are read and uploaded; the encoder half of the checkpoint is never touched
         unless ``encoder=True``, which also keeps its encoder.* / quant_conv.* tensors for ``encode``."""
-        try:
-            ck = torch.load(path, map_location="cpu", mmap=True, weights_only=True)
-        except (RuntimeError, ValueError, TypeError):
-            ck = torch.load(path, map_location="cpu", weights_only=True)
-        sd = ck[key] if key is not None else ck
+        sd = _lib.read_checkpoint(path, key)
         return self.load_state_dict(OrderedDict((k, v) for k, v in sd.items() if encoder or not k.startswith(_ENCODER_PREFIXES)))
 
     def _apply(self, fn, recurse=True):
@@ -130,42 +118,16 @@ class VAE(nn.Module):
 
     def _create_handle(self, dev):
         lib = _lib.lib()
-        self._destroy_handle()
+        self._handle = self._enc_handle = None     # the old handles are freed before the new one is made
         cfg = _lib.VaeConfig(self.latent_channels, self.out_channels, self.up_channels[0], self.up_channels[1], 8)
-        h = C.c_void_p()
-        with torch.cuda.device(dev):
-            _lib.check(lib.tpx_vae_create(C.byref(cfg), C.byref(h)), "tpx_vae_create")
-        self._handle, self._handle_device = h, dev
-        self._ws.clear()
-        self._destroy_encoder()
+        self._handle, self._handle_device = _lib.Handle(lib.tpx_vae_create, lib.tpx_vae_destroy, cfg, dev), dev
+        self._ws, self._enc_ws = _lib.Scratch(dev), _lib.Scratch(dev)
         if self._sd is not None:
             self._ingest()
 
     def _ingest(self):
         lib = _lib.lib()
         _lib.upload(self._handle, lib.tpx_vae_set_weight, lib.tpx_vae_finalize, self._sd.items(), self._handle_device)
-
-    def _destroy_handle(self):
-        if self.__dict__.get("_handle") is not None:
-            try:
-                _lib.load_library().tpx_vae_destroy(self._handle)
-            except Exception:
-                pass
-            self.__dict__["_handle"] = None      # not nn.Module.__setattr__: this also runs at interpreter shutdown
-
-    def _destroy_encoder(self):
-        if self.__dict__.get("_enc_handle") is not None:
-            try:
-                _lib.load_library().tpx_vae_encoder_destroy(self._enc_handle)
-            except Exception:
-                pass
-            self.__dict__["_enc_handle"] = None
-        if "_enc_ws" in self.__dict__:
-            self._enc_ws.clear()
-
-    def __del__(self):
-        self._destroy_encoder()
-        self._destroy_handle()
 
     def _latents(self, x: torch.Tensor, what: str) -> torch.Tensor:
         if self._handle is None:
@@ -180,16 +142,10 @@ class VAE(nn.Module):
         return z.contiguous()
 
     def _workspace(self, lib, P: int, encoder: bool = False):
-        """(256-B aligned address, bytes) of the decode scratch for P primitives, or of the encode scratch with `encoder`; the buffer
-        is kept for the next call of the same size."""
-        cache, nbytes = ((self._enc_ws, lib.tpx_vae_encoder_workspace_bytes(self._enc_handle, P)) if encoder
-                         else (self._ws, lib.tpx_vae_workspace_bytes(self._handle, P)))
-        ws = cache.get(P)
-        if ws is None:
-            cache.clear()
-            ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=self._handle_device)
-            cache[P] = ws
-        return (ws.data_ptr() + 255) & ~255, nbytes
+        """(256-B aligned address, bytes) of the decode scratch for P primitives, or of the encode scratch with `encoder`."""
+        if encoder:
+            return self._enc_ws.get(lib.tpx_vae_encoder_workspace_bytes(self._enc_handle, P))
+        return self._ws.get(lib.tpx_vae_workspace_bytes(self._handle, P))
 
     def decode(self, x: torch.Tensor) -> torch.Tensor:
         """VAE.decode (vae3d_dib.py:437-440)."""
@@ -247,13 +203,11 @@ class VAE(nn.Module):
         lib = _lib.lib()
         dev = self._handle_device
         cfg = _lib.VaeConfig(self.latent_channels, self.in_channels, self.down_channels[1], self.down_channels[0], 8)
-        h = C.c_void_p()
-        with torch.cuda.device(dev):
-            _lib.check(lib.tpx_vae_encoder_create(C.byref(cfg), C.byref(h)), "tpx_vae_encoder_create")
+        h = _lib.Handle(lib.tpx_vae_encoder_create, lib.tpx_vae_encoder_destroy, cfg, dev)
         try:
             _lib.upload(h, lib.tpx_vae_encoder_set_weight, lib.tpx_vae_encoder_finalize, ((k, self._extra[k]) for k in shapes), dev)
         except Exception:
-            lib.tpx_vae_encoder_destroy(h)
+            h.close()
             raise
         self._enc_handle = h
         return h

@@ -190,10 +190,10 @@ def test_timestep_table_is_dropped_when_weights_change():
     assert not torch.equal(a, b) and torch.equal(b, c) and torch.equal(e, c)
     with pytest.raises(tpxl_b200._lib.TpxError):     # straight at the C ABI: a timestep outside the table is an error there, not a fallback
         lib = tpxl_b200._lib.lib()
-        ws = m._workspace(4)
+        ws, nbytes = m._workspace(4)
         out = torch.empty(2, 256, 136, dtype=torch.float16, device=DEV)
-        tpxl_b200._lib.check(lib.tpx_dit_forward_step(m._handle, x.data_ptr(), 7, 2, 1, 6.0, out.data_ptr(), m._aligned(ws),
-                                                      lib.tpx_dit_workspace_bytes(m._handle, 4), tpxl_b200._lib.stream_ptr()))
+        tpxl_b200._lib.check(lib.tpx_dit_forward_step(m._handle, x.data_ptr(), 7, 2, 1, 6.0, out.data_ptr(), ws, nbytes,
+                                                      tpxl_b200._lib.stream_ptr()))
 
 
 @pytest.mark.parametrize("ddim", [True, False])
