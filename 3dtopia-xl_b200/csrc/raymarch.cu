@@ -5,10 +5,11 @@
 // an sm_70 torch extension.  One kernel here does both:
 //   * ray set-up per pixel (origin / volradius, direction through the pinhole, slab range of the unit cube);
 //   * per warp (the reference's 8 x 4-pixel warp of an 8 x 16 block — the hit list is a per-warp object in the reference and so
-//     part of the result) the ASCENDING list of primitives whose box is hit by ANY ray of the warp, capped at 512 like the
-//     reference's shared-memory list.  The reference walks a trivial 4095-node tree whose boxes prune next to nothing for
-//     unsorted primitives; here the 32 lanes first cull the primitives' bounding spheres against the warp's ray cone (64
-//     sphere tests per lane) and only the survivors get the exact per-ray slab test;
+//     part of the result) the list of primitives whose box is hit by ANY ray of the warp, in the reference's tree order (ascending
+//     index rotated by 2^ceil(log2 K) - K; see the hit-list scan), capped at 512 like the reference's shared-memory list.  The
+//     reference walks a trivial (2K - 1)-node tree whose boxes prune next to nothing for unsorted primitives; here the 32 lanes first
+//     cull the primitives' bounding spheres against the warp's ray cone (64 sphere tests per lane at K = 2048) and only the
+//     survivors get the exact per-ray slab test;
 //   * the fixed-step march: start at the last step before the ray's first hit, visit the listed primitives at every step
 //     (strictly-inside test in the primitive's frame, trilinear channels-last sample, alpha faded by exp(-fadescale * sum |y|^fadeexp)
 //     with the fast-math intrinsics the reference is compiled with), additive alpha with saturation at 1.
@@ -118,13 +119,19 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
     for (int o = 16; o > 0; o >>= 1) cmin = fminf(cmin, __shfl_xor_sync(0xffffffffu, cmin, o));
     const float theta = acosf(fminf(cmin, 1.f)) + 1e-4f;
 
-    // ---- hit list (ray_subset_fixedbvh semantics: any ray of the warp, ascending index, first RM_MAXHIT) ----
+    // ---- hit list (ray_subset_fixedbvh semantics: any ray of the warp, the tree's leaf order, first RM_MAXHIT) ----
+    // The reference walks the implicit heap of build_accel(fixedorder=True) depth-first, left child first, and appends each leaf as it
+    // is reached; leaf node i is primitive i - (K - 1).  Left to right, the leaves are the deeper level's first, so the list order is
+    // ascending order rotated by r = 2^ceil(log2 K) - K: r, ..., K - 1, 0, ..., r - 1 (ascending when K is a power of two).  Scan
+    // position j visits primitive (j + r) mod K.  The order decides which primitives a warp over the cap keeps and which primitive a
+    // saturating step's colour comes from.
+    const int rot = (1 << (32 - __clz(a.K - 1))) - a.K;
     int nhit = 0;
     float rtmin = INFINITY, rtmax = -INFINITY;
     for (int k0 = 0; k0 < a.K; k0 += 32) {
-        const int kc = k0 + lane;
+        const int kc = k0 + lane + rot < a.K ? k0 + lane + rot : k0 + lane + rot - a.K;
         bool cand = false;
-        if (kc < a.K) {
+        if (k0 + lane < a.K) {
             const size_t o = static_cast<size_t>(n) * a.K + kc;
             const float3 v = ld3(a.primpos + o * 3) - raypos;
             const float3 s = ld3(a.primscale + o * 3);
@@ -141,7 +148,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
         while (m != 0) {
             const int b = __ffs(m) - 1;
             m &= m - 1;
-            const int k = k0 + b;
+            const int k = k0 + b + rot < a.K ? k0 + b + rot : k0 + b + rot - a.K;
             const Prim p = load_prim(a, n, k);
             // PrimTransfSRT::forward2 + slab test in the primitive's frame
             const float3 xmt = raypos - p.t;

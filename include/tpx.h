@@ -303,7 +303,9 @@ int tpx_primsdf_sdf_grid(const float* coords_dev, int R, const float* srt_dev, c
  * template channels-last [N,K,S,S,S,4]; primpos [N,K,3] ALREADY divided by volradius (as the reference passes it),
  * primrot [N,K,3,3], primscale [N,K,3]; camera as convert_camera_parameters returns it (campos [N,3] in world units,
  * camrot [N,3,3], focal [N,2] = diagonal of K[:2,:2], princpt [N,2]); pixel (w,h) -> ray through (w,h); stepsize = dt / volradius.
- * rgba_out [N,H,W,4] (the reference's rayrgba; RayMarcher permutes it to [N,4,H,W]).
+ * rgba_out [N,H,W,4] (the reference's rayrgba; RayMarcher permutes it to [N,4,H,W]).  Each 8 x 4-pixel warp visits the
+ * primitives whose box any of its rays meets, in the "fixedorder" tree's leaf order (ascending index rotated by
+ * 2^ceil(log2 K) - K, so ascending when K is a power of two), at most the first 512 of them.
  * ---------------------------------------------------------------------------------------------------------- */
 int tpx_raymarch_preview(const float* template_chlast, const float* primpos, const float* primrot, const float* primscale, const float* campos,
                          const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius, float stepsize,

@@ -6,15 +6,17 @@ a plain PyTorch implementation of the same forward pass as the arm its CUDA kern
 tests/golden/make_raymarch_golden.py EXECUTES that block from /root/reference on the CPU over a seeded scene and stores inputs + image
 in tests/golden/raymarch_ref.npz.  tests/test_oracle_golden.py holds `raymarch_dense` (the restatement of that block) to the fixture
 at 2.4e-7 and the kernel-shaped restatement `raymarch` at 1.3e-6, and additionally `raymarch` to `raymarch_dense` on a camera scene.
-What stays a reading of the sources without reference output behind it: the CUDA-only parts — the per-warp hit list with its 512-entry
-cap, the start-at-first-hit stepping and compute_raydirs' slab test.
+The CUDA-only parts (the per-warp hit list, its order and 512-entry cap, the start-at-first-hit stepping and compute_raydirs' slab
+test) have no pure-PyTorch counterpart; they are pinned by running the reference's own CUDA extensions on the GPU against the kernel
+(tests/test_gpu_raymarch_ref.py), and the list order by the reference's tree walk on the host (tests/test_raymarch_grad_host.py).
 
 Restates (file:line under /root/reference):
   * convert_camera_parameters            dva/ray_marcher.py:24-33
   * RayMarcher.forward                   dva/ray_marcher.py:142-229   (pixel grid, pos / volradius, dt / volradius, "fixedorder" BVH, chlast)
   * compute_raydirs_forward_kernel       dva/mvp/extensions/utils/utils_kernel.cu:15-55
   * ray_subset_fixedbvh                  dva/mvp/extensions/mvpraymarch/utils.h:728-824   (per-warp hit list: a primitive is listed if ANY ray of the
-                                          8x4-pixel warp hits its box; ascending index; at most maxhitboxes = 512; rtminmax from the ray's own hits)
+                                          8x4-pixel warp hits its box; in the tree's leaf order, fixedorder_visit; at most maxhitboxes = 512; rtminmax from the
+                                          ray's own hits)
   * raymarch_subset_forward_kernel       .../mvpraymarch_subset_kernel.h:14-101  (start at the first step before the first hit, fixed steps, stop
                                           after the last hit or at saturation)
   * PrimTransfSRT.forward / valid        .../primtransf.h:104-131      (y = (R^T-rows . (x - t)) * s, strictly inside (-1, 1)^3)
@@ -75,16 +77,21 @@ def _sample_chlast(tpl, y):
     return out
 
 
-def raymarch(raypos, raydir, stepsize, tminmax, template, primpos, primrot, primscale, fadescale=8.0, fadeexp=8.0, block=(8, 16), maxhitboxes=512):
-    """Kernel-shaped restatement for ONE batch element.  raypos/raydir [H,W,3], tminmax [H,W,2], template [K,D,H,W,4] channels-last,
-    primpos [K,3] (already / volradius), primrot [K,3,3], primscale [K,3].  Returns rgba [H,W,4]."""
+def fixedorder_visit(K: int) -> list[int]:
+    """The order in which ray_subset_fixedbvh lists primitives: its depth-first, left-first walk of build_accel(fixedorder=True)'s
+    implicit heap (node i has children 2i+1, 2i+2; leaf node i is primitive i - (K - 1)) reaches the leaves of the deeper level first,
+    so it is ascending order rotated by r = 2^ceil(log2 K) - K: [r, ..., K-1, 0, ..., r-1], ascending only when K is a power of two."""
+    r = (1 << (K - 1).bit_length()) - K
+    return [(j + r) % K for j in range(K)]
+
+
+def slab_hits(raypos, raydir, primpos, primrot, primscale):
+    """The exact per-ray test of ray_subset_fixedbvh: hit [K,H,W] (the ray's LINE meets primitive k's box; no t >= 0 condition) and
+    the ray's rtminmax over its hits, rt_min / rt_max [H,W] (+inf / -inf without one)."""
     H, W = raypos.shape[:2]
     K = primpos.shape[0]
-    bx, by = block
-    # ---- hit lists (ray_subset_fixedbvh, sync = true, sortboxes = false) ----
-    inf = float("inf")
-    rt_min = torch.full((H, W), inf)
-    rt_max = torch.full((H, W), -inf)
+    rt_min = torch.full((H, W), float("inf"))
+    rt_max = torch.full((H, W), -float("inf"))
     hit = torch.zeros(K, H, W, dtype=torch.bool)
     for k in range(K):
         r0 = _local(raypos, primpos[k], primrot[k], primscale[k])                       # forward2: origin with the translation ...
@@ -97,6 +104,15 @@ def raymarch(raypos, raydir, stepsize, tminmax, template, primpos, primrot, prim
         hit[k] = h
         rt_min = torch.where(h, torch.minimum(rt_min, trmin), rt_min)
         rt_max = torch.where(h, torch.maximum(rt_max, trmax), rt_max)
+    return hit, rt_min, rt_max
+
+
+def hit_lists(hit, block=(8, 16), maxhitboxes=512):
+    """hit [K,H,W] bool (the exact slab test per primitive and ray) -> (warp_id [H,W], listed [warps, K] bool, order): a primitive is
+    listed for a warp if ANY of its rays hits it and it is among the first maxhitboxes such primitives in `fixedorder_visit` order,
+    which is also the order the march visits them in."""
+    K, H, W = hit.shape
+    bx, by = block
     # warp of pixel (h, w): thread id in the (bx, by) block = (h % by) * bx + (w % bx); 32 threads per warp
     hh, ww = torch.meshgrid(torch.arange(H), torch.arange(W), indexing="ij")
     wpb = (bx * by) // 32
@@ -104,9 +120,22 @@ def raymarch(raypos, raydir, stepsize, tminmax, template, primpos, primrot, prim
     nw = int(warp_id.max()) + 1
     cnt = torch.zeros(nw, K, dtype=torch.int32)
     cnt.index_put_((warp_id.reshape(-1).repeat(K), torch.arange(K).repeat_interleave(H * W)), hit.reshape(-1).int(), accumulate=True)
-    listed = cnt > 0
-    over = listed.long().cumsum(1) > maxhitboxes                                      # first maxhitboxes in ascending index survive
-    listed = listed & ~over
+    order = fixedorder_visit(K)
+    listed = (cnt > 0)[:, order]
+    listed = listed & ~(listed.long().cumsum(1) > maxhitboxes)                      # the first maxhitboxes in visiting order survive
+    out = torch.zeros_like(listed)
+    out[:, order] = listed
+    return warp_id, out, order
+
+
+def raymarch(raypos, raydir, stepsize, tminmax, template, primpos, primrot, primscale, fadescale=8.0, fadeexp=8.0, block=(8, 16), maxhitboxes=512):
+    """Kernel-shaped restatement for ONE batch element.  raypos/raydir [H,W,3], tminmax [H,W,2], template [K,D,H,W,4] channels-last,
+    primpos [K,3] (already / volradius), primrot [K,3,3], primscale [K,3].  Returns rgba [H,W,4]."""
+    H, W = raypos.shape[:2]
+    K = primpos.shape[0]
+    # ---- hit lists (ray_subset_fixedbvh, sync = true, sortboxes = false) ----
+    hit, rt_min, rt_max = slab_hits(raypos, raydir, primpos, primrot, primscale)
+    warp_id, listed, order = hit_lists(hit, block, maxhitboxes)
     rt_min = torch.maximum(rt_min, tminmax[..., 0])
     rt_max = torch.minimum(rt_max, tminmax[..., 1])
     # ---- march ----
@@ -120,7 +149,7 @@ def raymarch(raypos, raydir, stepsize, tminmax, template, primpos, primrot, prim
     rgba = torch.zeros(H, W, 4)
     sat = torch.zeros(H, W, dtype=torch.bool)
     alive = ~nohit
-    active_k = [k for k in range(K) if bool(listed[:, k].any())]
+    active_k = [k for k in order if bool(listed[:, k].any())]
     while bool((alive & ~(t > rt_max + 1e-5) & ~sat).any()):
         for k in active_k:
             y0 = _local(pos, primpos[k], primrot[k], primscale[k])
@@ -137,6 +166,35 @@ def raymarch(raypos, raydir, stepsize, tminmax, template, primpos, primrot, prim
         t = t + stepsize
         pos = pos + raydir * stepsize
     return rgba
+
+
+def saturating_overlap(raypos, raydir, stepsize, tminmax, template, primpos, primrot, primscale, fadescale=8.0, fadeexp=8.0):
+    """[H,W] int: how many primitives a ray is inside of at the step where its accumulated alpha first reaches 1 (0 if it never does),
+    on raymarch_dense's steps.  Where this is 2 or more, the primitive visited first takes the step's remaining alpha and supplies the
+    ray's final colour, so the image depends on the visiting order; every other ray sums the same samples in any order."""
+    H, W = raypos.shape[:2]
+    K = primpos.shape[0]
+    acc = torch.zeros(H, W)
+    out = torch.zeros(H, W, dtype=torch.int64)
+    pos0, t0 = raypos + raydir * tminmax[..., 0:1], tminmax[..., 0]
+    step = 0
+    t, pos = t0.clone(), pos0.clone()
+    while bool((t < tminmax[..., 1]).any()):
+        live = (t < tminmax[..., 1]) & (out == 0)
+        n = torch.zeros(H, W, dtype=torch.int64)
+        add = torch.zeros(H, W)
+        for k in range(K):
+            y0 = _local(pos, primpos[k], primrot[k], primscale[k])
+            inside = ((y0 >= -1.0) & (y0 <= 1.0)).all(-1) & live
+            s = _sample_chlast(template[k], y0.clamp(-1, 1))
+            add = add + torch.where(inside, s[..., 3] * torch.exp(-fadescale * (y0.abs() ** fadeexp).sum(-1)) * stepsize, torch.zeros_like(add))
+            n = n + inside.long()
+        acc = acc + add
+        out = torch.where(live & (acc >= 1.0), n, out)
+        step += 1
+        t = t0 + stepsize * step
+        pos = pos0 + raydir * stepsize * step
+    return out
 
 
 def raymarch_dense(raypos, raydir, stepsize, tminmax, template, primpos, primrot, primscale, fadescale=8.0, fadeexp=8.0):

@@ -16,7 +16,7 @@ from __future__ import annotations
 
 import torch
 
-from .raymarch import _local, _sample_chlast, compute_raydirs, convert_camera_parameters
+from .raymarch import _local, _sample_chlast, compute_raydirs, convert_camera_parameters, hit_lists, slab_hits
 
 
 def compute_raydirs_at(campos, camrot, focal, princpt, pixelcoords, volradius: float):
@@ -41,30 +41,9 @@ def raymarch_grad(raypos, raydir, stepsize, tminmax, template, primpos, primrot,
     test divides by the ray direction in the primitive's frame, whose backward is 0 * inf = nan on a ray parallel to a box face."""
     H, W = raypos.shape[:2]
     K = primpos.shape[0]
-    bx, by = block
     with torch.no_grad():
-        rt_min = torch.full((H, W), float("inf"))
-        rt_max = torch.full((H, W), -float("inf"))
-        hit = torch.zeros(K, H, W, dtype=torch.bool)
-        for k in range(K):
-            r0 = _local(raypos, primpos[k], primrot[k], primscale[k])
-            rd = _local(raydir, torch.zeros(3), primrot[k], primscale[k])
-            ird = 1.0 / rd
-            t0, t1 = (-1.0 - r0) * ird, (1.0 - r0) * ird
-            trmin = torch.minimum(t0, t1).amax(-1)
-            trmax = torch.maximum(t0, t1).amin(-1)
-            h = trmin <= trmax
-            hit[k] = h
-            rt_min = torch.where(h, torch.minimum(rt_min, trmin), rt_min)
-            rt_max = torch.where(h, torch.maximum(rt_max, trmax), rt_max)
-        hh, ww = torch.meshgrid(torch.arange(H), torch.arange(W), indexing="ij")
-        wpb = (bx * by) // 32
-        warp_id = ((hh // by) * ((W + bx - 1) // bx) + (ww // bx)) * wpb + ((hh % by) * bx + (ww % bx)) // 32
-        nw = int(warp_id.max()) + 1
-        cnt = torch.zeros(nw, K, dtype=torch.int32)
-        cnt.index_put_((warp_id.reshape(-1).repeat(K), torch.arange(K).repeat_interleave(H * W)), hit.reshape(-1).int(), accumulate=True)
-        listed = cnt > 0
-        listed = listed & ~(listed.long().cumsum(1) > maxhitboxes)
+        hit, rt_min, rt_max = slab_hits(raypos, raydir, primpos, primrot, primscale)
+        warp_id, listed, order = hit_lists(hit, block, maxhitboxes)
         rt_min = torch.maximum(rt_min, tminmax[..., 0])
         rt_max = torch.minimum(rt_max, tminmax[..., 1])
         t = tminmax[..., 0].clone()
@@ -77,7 +56,7 @@ def raymarch_grad(raypos, raydir, stepsize, tminmax, template, primpos, primrot,
     rgba = torch.zeros(H, W, 4)
     sat = torch.zeros(H, W, dtype=torch.bool)
     alive = ~nohit
-    active_k = [k for k in range(K) if bool(listed[:, k].any())]
+    active_k = [k for k in order if bool(listed[:, k].any())]
     while bool((alive & ~(t > rt_max + 1e-5) & ~sat).any()):
         for k in active_k:
             y0 = _local(pos, primpos[k], primrot[k], primscale[k])

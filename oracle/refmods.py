@@ -72,6 +72,38 @@ def load() -> SimpleNamespace:
     return _cache
 
 
+def raymarcher_available() -> bool:
+    return stage_ref.raymarcher_staged()
+
+
+_rm_cache = None
+
+
+def load_raymarcher():
+    """-> the reference's ``dva.ray_marcher.RayMarcher`` over its own CUDA extensions (mvpraymarchlib, utilslib) built by
+    oracle/stage_ref.py.  ``dva`` is a generic top-level name, so it is imported with ``oracle/_ref`` first on ``sys.path`` and taken
+    out of ``sys.modules`` again, as ``load()`` does.  Raises FileNotFoundError when the extensions were not built."""
+    global _rm_cache
+    if _rm_cache is not None:
+        return _rm_cache
+    if not raymarcher_available():
+        raise FileNotFoundError("the reference's ray marcher is not built: run `python oracle/stage_ref.py` where a reference checkout exists")
+    taken = ("dva", "mvpraymarchlib", "utilslib")
+    saved = {k: v for k, v in sys.modules.items() if k.split(".")[0] in taken}
+    for k in saved:
+        del sys.modules[k]
+    sys.path.insert(0, stage_ref.DEST)
+    try:
+        from dva.ray_marcher import RayMarcher
+    finally:
+        sys.path.remove(stage_ref.DEST)
+        for k in [k for k in sys.modules if k.split(".")[0] in taken]:
+            del sys.modules[k]
+        sys.modules.update(saved)
+    _rm_cache = RayMarcher
+    return _rm_cache
+
+
 def build_dit(cfg: dict, state_dict: dict, device="cpu"):
     """Reference DiT with the given (reference-keyed) parameters, fp32 modules as inference.py:254-265 builds them."""
     ref = load()

@@ -14,6 +14,15 @@ What is staged (byte-identical copies, sha256 recorded in ``oracle/_ref/MANIFEST
 Nothing else of the reference is needed on this path.  The one un-vendored dependency, ``xformers.ops``
 (models/attention.py:17; unpinned, README.md:67), is NOT staged or copied from anywhere: ``oracle/refmods.py``
 restates its contract with ``torch.nn.functional.scaled_dot_product_attention``.
+
+The ray marcher's preview (``dva.ray_marcher.RayMarcher``) is staged too, so the ``-m gpu`` suite can run the reference's own CUDA
+extensions as the oracle of csrc/raymarch.cu:
+    dva/__init__.py, dva/ray_marcher.py, dva/mvp/extensions/{mvpraymarch/mvpraymarch.py, utils/utils.py}   (byte-identical)
+and its two torch extensions are compiled FROM THE CHECKOUT (no source is copied) into oracle/_ref/build/, in parallel, with the
+flags of their own setup.py except that ``-arch=sm_70`` becomes ``-gencode arch=compute_90a,code=sm_90a``; each ``.so`` is then
+placed beside its wrapper, where ``from . import mvpraymarchlib`` / ``from . import utilslib`` find it.  The host compile gets
+``-DNDEBUG``: utils.cpp:67 and :113 assert on a ``size()`` that ``std::optional`` does not have, and the reference's setup.py build
+never compiles those asserts because setuptools passes Python's CFLAGS, which carry ``-DNDEBUG``.
 """
 from __future__ import annotations
 
@@ -21,6 +30,7 @@ import hashlib
 import json
 import os
 import shutil
+import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -31,26 +41,74 @@ FILES = [
     "models/diffusion/__init__.py", "models/diffusion/diffusion_utils.py", "models/diffusion/gaussian_diffusion.py",
     "models/diffusion/respace.py", "models/diffusion/timestep_sampler.py", "utils/typing.py",
 ]
+RAYMARCH_FILES = [
+    "dva/__init__.py", "dva/ray_marcher.py", "dva/mvp/extensions/mvpraymarch/mvpraymarch.py", "dva/mvp/extensions/utils/utils.py",
+]
+SM90A = ["-gencode", "arch=compute_90a,code=sm_90a"]
+# name -> (directory under the checkout, sources, nvcc flags of its setup.py with the arch replaced)
+EXTENSIONS = {
+    "mvpraymarchlib": ("dva/mvp/extensions/mvpraymarch", ["mvpraymarch.cpp", "mvpraymarch_kernel.cu", "bvh.cu"],
+                       ["-use_fast_math", *SM90A, "-std=c++17", "-lineinfo"]),
+    "utilslib": ("dva/mvp/extensions/utils", ["utils.cpp", "utils_kernel.cu"], [*SM90A, "-std=c++14", "-lineinfo"]),
+}
+_BUILD = """
+import sys
+from torch.utils.cpp_extension import load
+name, build_dir, flags, *sources = sys.argv[1:]
+load(name=name, sources=sources, extra_cflags=["-DNDEBUG"], extra_cuda_cflags=flags.split(), build_directory=build_dir, verbose=False)
+"""
+
+
+def _sha(path: str) -> str:
+    with open(path, "rb") as f:
+        return hashlib.sha256(f.read()).hexdigest()
 
 
 def stage(src: str = DEFAULT_SRC, dest: str = DEST) -> dict:
     if not os.path.isdir(src):
         raise FileNotFoundError(f"{src} not found: pass the path of a reference checkout")
     manifest = {"source": src, "files": {}}
-    for rel in FILES:
+    for rel in FILES + RAYMARCH_FILES:
         s, d = os.path.join(src, rel), os.path.join(dest, rel)
         os.makedirs(os.path.dirname(d), exist_ok=True)
         shutil.copyfile(s, d)
-        manifest["files"][rel] = hashlib.sha256(open(d, "rb").read()).hexdigest()
+        manifest["files"][rel] = _sha(d)
+    manifest["extensions"] = build_raymarch_extensions(src, dest)
     with open(os.path.join(dest, "MANIFEST.json"), "w") as f:
         json.dump(manifest, f, indent=1, sort_keys=True)
     return manifest
+
+
+def build_raymarch_extensions(src: str = DEFAULT_SRC, dest: str = DEST) -> dict:
+    """Compile mvpraymarchlib and utilslib side by side (one process each) and place each .so beside its staged wrapper.
+    Returns {placed .so (relative to dest): its nvcc flags}."""
+    jobs = {}
+    for name, (rel, sources, flags) in EXTENSIONS.items():
+        build_dir = os.path.join(dest, "build", name)
+        os.makedirs(build_dir, exist_ok=True)
+        cmd = [sys.executable, "-c", _BUILD, name, build_dir, " ".join(flags), *[os.path.join(src, rel, s) for s in sources]]
+        jobs[name] = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    placed = {}
+    for name, p in jobs.items():
+        log = p.communicate()[0]
+        if p.returncode != 0:
+            raise RuntimeError(f"building the reference's {name} failed:\n{log[-4000:]}")
+        rel, _, flags = EXTENSIONS[name]
+        so = os.path.join(rel, name + ".so")
+        shutil.copyfile(os.path.join(dest, "build", name, name + ".so"), os.path.join(dest, so))
+        placed[so] = " ".join(flags)
+    return placed
 
 
 def staged(dest: str = DEST) -> bool:
     return all(os.path.exists(os.path.join(dest, rel)) for rel in FILES)
 
 
+def raymarcher_staged(dest: str = DEST) -> bool:
+    sos = [os.path.join(rel, name + ".so") for name, (rel, _, _) in EXTENSIONS.items()]
+    return all(os.path.exists(os.path.join(dest, rel)) for rel in RAYMARCH_FILES + sos)
+
+
 if __name__ == "__main__":
     m = stage(sys.argv[1] if len(sys.argv) > 1 else DEFAULT_SRC)
-    print(f"staged {len(m['files'])} reference files under {DEST}")
+    print(f"staged {len(m['files'])} reference files and built {len(m['extensions'])} extensions under {DEST}")

@@ -332,12 +332,17 @@ def test_raymarch_restatement_agrees_with_the_reference_torch_marcher():
     assert rel < 2e-2, rel
 
 
-def test_raymarch_oracle_matches_the_reference_torch_marcher_fixture(golden_dir):
+def test_raymarch_oracle_matches_the_reference_torch_marcher_fixture_on_order_free_rays(golden_dir):
     """tests/golden/raymarch_ref.npz holds the image the REFERENCE's own pure-PyTorch ray-marcher (the block its gradcheck script runs
     against the CUDA kernel, mvpraymarch.py:391-475) produced for a seeded scene; tests/golden/make_raymarch_golden.py executed that
     block from /root/reference on the CPU.  Both oracle restatements are held to it: `raymarch_dense` (the same algorithm) tightly,
     `raymarch` (the CUDA kernel's structure, which the GPU test compares the kernel with) up to float rounding on this scene, whose
-    rays carry their own [tmin, tmax] so the two formulations take the same steps."""
+    rays carry their own [tmin, tmax] so the two formulations take the same steps.
+
+    The pure-PyTorch marcher visits primitives in ascending index; the CUDA kernel, and so `raymarch`, in the "fixedorder" tree's
+    leaf order (here K = 6: 2, 3, 4, 5, 0, 1).  With its visiting order set to ascending, `raymarch` matches the fixture on every ray,
+    so the order is the only difference.  In the tree order it differs only on rays whose saturating step is inside two or more
+    primitives (the first visited supplies the colour); on all other rays, saturating ones among them, it matches to float rounding."""
     import torch
     from oracle import raymarch as rmo
     d = np.load(os.path.join(golden_dir, "raymarch_ref.npz"))
@@ -348,8 +353,19 @@ def test_raymarch_oracle_matches_the_reference_torch_marcher_fixture(golden_dir)
     assert float((ref[..., 3] > 0).float().mean()) > 0.5 and float((ref[..., 3] >= 1 - 1e-6).float().mean()) > 0.1   # covered and saturating rays
     dense = rmo.raymarch_dense(*args)
     assert float((dense - ref).abs().max()) < 5e-6, float((dense - ref).abs().max())
+    with pytest.MonkeyPatch.context() as mp:
+        mp.setattr(rmo, "fixedorder_visit", lambda K: list(range(K)))
+        ascending = rmo.raymarch(*args)
+    assert float((ascending - ref).abs().max()) < 2e-5, float((ascending - ref).abs().max())
     kern = rmo.raymarch(*args)
-    assert float((kern - ref).abs().max()) < 2e-5, float((kern - ref).abs().max())
+    overlap = rmo.saturating_overlap(*args)
+    order_free = overlap < 2
+    err = (kern - ref).abs().amax(-1)
+    print(f"rays whose saturating step overlaps primitives: {int((~order_free).sum())} of {order_free.numel()}, "
+          f"differing there {int((err[~order_free] >= 2e-5).sum())}, worst {float(err.max()):.2e}")
+    assert bool((err[order_free] < 2e-5).all()), float(err[order_free].max())
+    assert float(order_free.float().mean()) > 0.5 and int((overlap == 1).sum()) > 0     # most rays, saturating ones among them, still compared
+    assert int((err[~order_free] >= 2e-5).sum()) > 0                                    # and the tree order does show on this scene
 
 
 def test_inference_glue_matches_the_reference_statements(golden_dir):
