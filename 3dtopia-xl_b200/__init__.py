@@ -9,7 +9,7 @@ import types
 
 from . import synth  # noqa: F401
 from . import _lib  # noqa: F401
-from . import bake, diffusion, dinov2, dit, mesh, pipeline, primsdf, ray_marcher, shard, unwrap, vae  # noqa: F401
+from . import bake, diffusion, dinov2, dit, mesh, pipeline, primsdf, ray_marcher, shard, unwrap, vae, visualize  # noqa: F401
 from .diffusion import SpacedDiffusion, create_diffusion  # noqa: F401
 from .dit import DiT  # noqa: F401
 from .pipeline import LatentCodec, PrimXPipeline  # noqa: F401
@@ -23,7 +23,8 @@ __version__ = "0.1.0"
 def install(mcubes: bool = False, nvdiffrast: bool = False, uv_unwrap: bool = False, meshutils: bool = False) -> None:
     """Make the reference's import paths resolve to this implementation, so ``inference.py`` / ``app.py`` run
     unchanged:  ``models.dit_crossattn`` -> dit, ``models.vae3d_dib`` -> vae, ``models.diffusion`` -> diffusion,
-    ``models.primsdf`` -> primsdf, ``models.conditioner.image_dinov2`` -> dinov2, ``dva.ray_marcher`` -> ray_marcher.
+    ``models.primsdf`` -> primsdf, ``models.conditioner.image_dinov2`` -> dinov2, ``dva.ray_marcher`` -> ray_marcher,
+    ``dva.visualize`` -> visualize.
     (Equivalent to editing ``class_name`` in configs/inference_dit.yml:32,53; see INTEGRATION.md.)  If the reference's
     ``models`` package is importable it is imported first so its other members (conditioner, primsdf) keep working.
     ``mcubes=True`` also binds ``sys.modules["mcubes"]`` to a module whose ``marching_cubes`` is the GPU one of ``mesh``, so
@@ -52,9 +53,14 @@ def install(mcubes: bool = False, nvdiffrast: bool = False, uv_unwrap: bool = Fa
     # the preview renderer: ``from dva.ray_marcher import RayMarcher`` (inference.py:12) resolves here, so the reference's sm_70
     # ray-march extensions (dva/mvp/extensions/*) need not be built at all
     sys.modules["dva.ray_marcher"] = ray_marcher
+    # and the preview renders: ``from dva.visualize import visualize_primvolume, visualize_video_primvolume`` (inference.py:15,
+    # app.py:18) resolves to the device drop-in; the reference's own dva.visualize also imports over this ray_marcher, whose
+    # generate_colored_boxes it needs
+    sys.modules["dva.visualize"] = visualize
     try:
         import dva as ref_dva
         setattr(ref_dva, "ray_marcher", ray_marcher)
+        setattr(ref_dva, "visualize", visualize)
     except Exception:
         pass
     if mcubes:

@@ -14,6 +14,8 @@ _lock = threading.Lock()
 _lib = None
 
 DTYPE_F32, DTYPE_F16 = 0, 1
+LAYOUT_NCDHW, LAYOUT_CHLAST = 0, 1          # tpx_colored_boxes
+PAYLOAD_RGB, PAYLOAD_MAT = 0, 1            # tpx_primvolume_payload
 _vp, _i, _f, _sz, _i64 = C.c_void_p, C.c_int, C.c_float, C.c_size_t, C.c_int64
 
 
@@ -89,6 +91,9 @@ SIGNATURES = {
     "tpx_raymarch_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _f, _i, _vp, _vp, _vp, _vp]),
     "tpx_raymarch_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                    _vp]),
+    "tpx_raymarch_preview_views": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _f, _f, _f, _vp, _vp]),
+    "tpx_colored_boxes": (_i, [_vp, _i, _i, _i, _f, _i, _vp, _vp]),
+    "tpx_primvolume_payload": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "tpx_mc_workspace_bytes": (_sz, [_i64, _i64, _i64]),
     "tpx_mc_count": (_i, [_vp, _i64, _i64, _i64, _f, _vp, _sz, _vp, _vp]),
     "tpx_mc_emit": (_i, [_vp, _i64, _i64, _i64, _f, _f, _f, _f, _f, _f, _f, _vp, _sz, _vp, _vp, _vp]),

@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libtpx_b200.so")
-SOURCES = ["runtime.cu", "gemm_tc.cu", "elementwise.cu", "attention.cu", "attention_tc.cu", "vae_kernels.cu", "conv_halo.cu", "primsdf.cu", "marching_cubes.cu", "texture_bake.cu", "mesh_simplify.cu", "mesh_remesh.cu", "uv_unwrap.cu", "raymarch.cu", "conditioner.cu", "dit.cu", "vae.cu"]
+SOURCES = ["runtime.cu", "gemm_tc.cu", "elementwise.cu", "attention.cu", "attention_tc.cu", "vae_kernels.cu", "conv_halo.cu", "primsdf.cu", "marching_cubes.cu", "texture_bake.cu", "mesh_simplify.cu", "mesh_remesh.cu", "uv_unwrap.cu", "raymarch.cu", "visualize.cu", "conditioner.cu", "dit.cu", "vae.cu"]
 HEADERS = ["tpx_common.cuh", "gemm_tc.cuh", "kernels.cuh", "mesh_common.cuh", "mc_tables.cuh", "bake_interp.cuh", os.path.join("..", "..", "include", "tpx.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr"]

@@ -22,6 +22,8 @@
 //   * the 15 transform partials are summed over the warp with shuffles (all 32 lanes visit the same primitive at the same step) and
 //     lanes 0..14 each issue one reduction.
 // Subsampled rays (ray_subsample_factor > 1): output pixel (j, i) traces the ray through image pixel (x0 + stride j, y0 + stride i).
+// Views (tpx_raymarch_preview_views): image n reads primitive set n / views and camera n, so a turntable of one primitive set is one
+// launch over one template.
 #include "kernels.cuh"
 
 namespace tpx {
@@ -52,6 +54,7 @@ struct RayMarchArgs {
     float* grad_pos;         // [N, K, 3]
     float* grad_rot;         // [N, K, 3, 3]
     float* grad_scale;       // [N, K, 3]
+    int views;               // image n marches primitive set n / views (the [N, K, ...] arrays above hold N / views sets)
 };
 
 struct Prim {
@@ -83,7 +86,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
     const int lin = threadIdx.y * RM_BX + threadIdx.x;
     const int warp = lin >> 5, lane = lin & 31;
     int w = blockIdx.x * RM_BX + threadIdx.x, h = blockIdx.y * RM_BY + threadIdx.y;
-    const int n = blockIdx.z;
+    const int n = blockIdx.z, np = n / a.views;   // image (camera, output) and primitive set
     const bool live = w < a.W && h < a.H;
     w = min(w, a.W - 1);
     h = min(h, a.H - 1);                 // threads outside the image march a duplicate of the border ray (as in the reference)
@@ -132,7 +135,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
         const int kc = k0 + lane + rot < a.K ? k0 + lane + rot : k0 + lane + rot - a.K;
         bool cand = false;
         if (k0 + lane < a.K) {
-            const size_t o = static_cast<size_t>(n) * a.K + kc;
+            const size_t o = static_cast<size_t>(np) * a.K + kc;
             const float3 v = ld3(a.primpos + o * 3) - raypos;
             const float3 s = ld3(a.primscale + o * 3);
             const float rad = sqrtf(1.f / (s.x * s.x) + 1.f / (s.y * s.y) + 1.f / (s.z * s.z)) * 1.001f + 1e-6f;   // bounding sphere of the rotated box
@@ -149,7 +152,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
             const int b = __ffs(m) - 1;
             m &= m - 1;
             const int k = k0 + b + rot < a.K ? k0 + b + rot : k0 + b + rot - a.K;
-            const Prim p = load_prim(a, n, k);
+            const Prim p = load_prim(a, np, k);
             // PrimTransfSRT::forward2 + slab test in the primitive's frame
             const float3 xmt = raypos - p.t;
             const float3 r0 = (p.r0 * xmt.x + p.r1 * xmt.y + p.r2 * xmt.z) * p.s;
@@ -169,7 +172,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
     }
     __syncwarp();
     for (int j = lane; j < min(nhit, RM_CACHE); j += 32) {
-        const Prim p = load_prim(a, n, s_list[warp][j]);
+        const Prim p = load_prim(a, np, s_list[warp][j]);
         float* d = s_prim[warp][j];
         d[0] = p.t.x; d[1] = p.t.y; d[2] = p.t.z; d[3] = p.r0.x; d[4] = p.r0.y; d[5] = p.r0.z; d[6] = p.r1.x; d[7] = p.r1.y; d[8] = p.r1.z;
         d[9] = p.r2.x; d[10] = p.r2.y; d[11] = p.r2.z; d[12] = p.s.x; d[13] = p.s.y; d[14] = p.s.z;
@@ -209,7 +212,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
                 p.t = make_float3(d[0], d[1], d[2]); p.r0 = make_float3(d[3], d[4], d[5]); p.r1 = make_float3(d[6], d[7], d[8]);
                 p.r2 = make_float3(d[9], d[10], d[11]); p.s = make_float3(d[12], d[13], d[14]);
             } else {
-                p = load_prim(a, n, k);
+                p = load_prim(a, np, k);
             }
             const float3 xmt = pos - p.t;
             const float3 y = (p.r0 * xmt.x + p.r1 * xmt.y + p.r2 * xmt.z) * p.s;
@@ -225,7 +228,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
                 const float ix = (y.x + 1.f) * 0.5f * hs, iy = (y.y + 1.f) * 0.5f * hs, iz = (y.z + 1.f) * 0.5f * hs;
                 const int x0 = min(static_cast<int>(floorf(ix)), S - 2), y0 = min(static_cast<int>(floorf(iy)), S - 2), z0 = min(static_cast<int>(floorf(iz)), S - 2);
                 const float ax = ix - x0, ay = iy - y0, az = iz - z0;
-                const float4* tp = reinterpret_cast<const float4*>(a.tpl) + (static_cast<size_t>(n) * a.K + k) * S * S * S + (z0 * S + y0) * S + x0;
+                const float4* tp = reinterpret_cast<const float4*>(a.tpl) + (static_cast<size_t>(np) * a.K + k) * S * S * S + (z0 * S + y0) * S + x0;
                 float4 smp = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
                 for (int c = 0; c < 8; ++c) {
@@ -252,7 +255,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
                     float3 dy = make_float3(cf * __powf(fabsf(y.x), fe1) * (y.x > 0.f ? 1.f : -1.f), cf * __powf(fabsf(y.y), fe1) * (y.y > 0.f ? 1.f : -1.f),
                                             cf * __powf(fabsf(y.z), fe1) * (y.z > 0.f ? 1.f : -1.f));
                     const float4 g = make_float4(wgt_rgb * dL.x, wgt_rgb * dL.y, wgt_rgb * dL.z, dla * fade);
-                    float4* gtp = reinterpret_cast<float4*>(a.grad_tpl) + (static_cast<size_t>(n) * a.K + k) * S * S * S + (z0 * S + y0) * S + x0;
+                    float4* gtp = reinterpret_cast<float4*>(a.grad_tpl) + (static_cast<size_t>(np) * a.K + k) * S * S * S + (z0 * S + y0) * S + x0;
                     float gx = 0.f, gy = 0.f, gz = 0.f;
 #pragma unroll
                     for (int c = 0; c < 8; ++c) {
@@ -292,7 +295,7 @@ __global__ void __launch_bounds__(RM_BX * RM_BY) raymarch_kernel(const RayMarchA
                     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
                     if (lane == i) mine = v;
                 }
-                const size_t o = static_cast<size_t>(n) * a.K + k;
+                const size_t o = static_cast<size_t>(np) * a.K + k;
                 float* dst = lane < 3 ? a.grad_scale + o * 3 + lane : lane < 12 ? a.grad_rot + o * 9 + (lane - 3) : a.grad_pos + o * 3 + (lane - 12);
                 if (lane < 15 && mine != 0.f) atomicAdd(dst, mine);
             }
@@ -313,6 +316,7 @@ int raymarch_check(const RayMarchArgs& a, int H, int W) {
     TPX_CHECK(a.N > 0 && a.K > 0 && a.S >= 2 && a.S <= 64 && H > 0 && W > 0 && a.N <= 65535, TPX_ERR_SHAPE, "raymarch: bad geometry (N %d K %d S %d %d x %d)", a.N,
               a.K, a.S, H, W);
     TPX_CHECK(a.stride >= 1 && a.H >= 1 && a.W >= 1, TPX_ERR_SHAPE, "raymarch: stride %d leaves a %d x %d image of %d x %d", a.stride, a.H, a.W, H, W);
+    TPX_CHECK(a.views >= 1 && a.N % a.views == 0, TPX_ERR_SHAPE, "raymarch: %d views do not divide %d images", a.views, a.N);
     TPX_CHECK(a.stepsize > 0.f && a.volradius > 0.f, TPX_ERR_ARG, "raymarch: step size and volume radius must be positive");
     TPX_CHECK((reinterpret_cast<uintptr_t>(a.tpl) & 15) == 0, TPX_ERR_ARG, "raymarch: template must be 16-B aligned");
     return TPX_OK;
@@ -341,12 +345,24 @@ extern "C" int tpx_raymarch_preview(const float* tpl, const float* primpos, cons
                                 nullptr, out, nullptr, stream);
 }
 
+extern "C" int tpx_raymarch_preview_views(const float* tpl, const float* primpos, const float* primrot, const float* primscale, const float* campos,
+                                          const float* camrot, const float* focal, const float* princpt, int N, int views, int K, int S, int H, int W,
+                                          float volradius, float stepsize, float fadescale, float fadeexp, float* out, void* stream) {
+    const RayMarchArgs a{tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, out, N, K, S, H, W, volradius, stepsize, fadescale, fadeexp,
+                         1, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, views};
+    TPX_CHECK(out != nullptr, TPX_ERR_ARG, "raymarch: null argument");
+    if (const int rc = raymarch_check(a, H, W)) return rc;
+    TPX_CHECK((reinterpret_cast<uintptr_t>(out) & 15) == 0, TPX_ERR_ARG, "raymarch: output must be 16-B aligned");
+    TPX_DEVICE_GUARD();
+    return raymarch_launch<false>(a, stream);
+}
+
 extern "C" int tpx_raymarch_forward(const float* tpl, const float* primpos, const float* primrot, const float* primscale, const float* campos,
                                     const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius,
                                     float stepsize, float fadescale, float fadeexp, int stride, const int* offsets, float* out, float* raysat_out, void* stream) {
     const int h = stride >= 1 ? H / stride : 0, w = stride >= 1 ? W / stride : 0;
     const RayMarchArgs a{tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, out, N, K, S, h, w, volradius, stepsize, fadescale, fadeexp,
-                         stride, offsets, raysat_out, nullptr, nullptr, nullptr, nullptr, nullptr};
+                         stride, offsets, raysat_out, nullptr, nullptr, nullptr, nullptr, nullptr, 1};
     TPX_CHECK(out != nullptr, TPX_ERR_ARG, "raymarch: null argument");
     if (const int rc = raymarch_check(a, H, W)) return rc;
     TPX_CHECK((reinterpret_cast<uintptr_t>(out) & 15) == 0, TPX_ERR_ARG, "raymarch: output must be 16-B aligned");
@@ -360,7 +376,7 @@ extern "C" int tpx_raymarch_backward(const float* tpl, const float* primpos, con
                                      const float* grad_rgba, float* grad_tpl, float* grad_primpos, float* grad_primrot, float* grad_primscale, void* stream) {
     const int h = stride >= 1 ? H / stride : 0, w = stride >= 1 ? W / stride : 0;
     const RayMarchArgs a{tpl, primpos, primrot, primscale, campos, camrot, focal, princpt, nullptr, N, K, S, h, w, volradius, stepsize, fadescale, fadeexp,
-                         stride, offsets, const_cast<float*>(raysat), grad_rgba, grad_tpl, grad_primpos, grad_primrot, grad_primscale};
+                         stride, offsets, const_cast<float*>(raysat), grad_rgba, grad_tpl, grad_primpos, grad_primrot, grad_primscale, 1};
     TPX_CHECK(raysat != nullptr && grad_rgba != nullptr && grad_tpl != nullptr && grad_primpos != nullptr && grad_primrot != nullptr && grad_primscale != nullptr,
               TPX_ERR_ARG, "raymarch: null argument");
     if (const int rc = raymarch_check(a, H, W)) return rc;

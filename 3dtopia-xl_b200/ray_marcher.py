@@ -12,9 +12,13 @@ a ``torch.autograd.Function`` (the reference's ``MVPRaymarch``, mvpraymarch.py:7
 arrive in the caller's layout, units and dtype.  The camera gets no gradient, as in the reference.  Otherwise the no-grad preview runs.
 ``ray_subsample_factor > 1`` marches every f-th pixel from a per-image offset: drawn as ``subsample_pixel_coords`` draws it in training,
 ``f // 2`` in eval (dva/ray_marcher.py:33-73, 174-190).
+
+``generate_colored_boxes`` (dva/ray_marcher.py:232-279, what ``dva.visualize`` imports beside ``RayMarcher``) builds the box template
+in one launch (tpx_colored_boxes); ``march_views`` marches many cameras of one primitive set in one launch for ``tpxl_b200.visualize``.
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -26,6 +30,63 @@ def convert_camera_parameters(Rt: torch.Tensor, K: torch.Tensor):
     R = Rt[:, :3, :3]
     t = -R.permute(0, 2, 1).bmm(Rt[:, :3, 3].unsqueeze(2)).squeeze(2)
     return dict(campos=t, camrot=R, focal=K[:, :2, :2], princpt=K[:, :2, 2])
+
+
+def march_camera(RT: torch.Tensor, K: torch.Tensor, dev) -> tuple:
+    """(campos, camrot, focal, princpt) as the march reads them, computed on `dev` from extrinsics [B,3,4] and intrinsics [B,3,3] by
+    the reference's torch statements (convert_camera_parameters, then the focal diagonal), fp32 and contiguous."""
+    with torch.no_grad():
+        cam = convert_camera_parameters(RT.to(dev).float(), K.to(dev).float())
+        f32 = lambda t: t.to(dev).float().contiguous()  # noqa: E731
+        return f32(cam["campos"]), f32(cam["camrot"]), f32(torch.diagonal(cam["focal"], dim1=1, dim2=2)), f32(cam["princpt"])
+
+
+def march_views(tpl: torch.Tensor, pos: torch.Tensor, rot: torch.Tensor, scale: torch.Tensor, cam, views: int, H: int, W: int, volradius: float,
+                stepsize: float, fadescale: float, fadeexp: float) -> torch.Tensor:
+    """No-grad preview march of `views` cameras per primitive set in one launch (tpx_raymarch_preview_views): tpl [N,K,S,S,S,4] fp32
+    channels-last, pos [N,K,3] (/ volradius), rot [N,K,3,3], scale [N,K,3], ``cam`` = march_camera's four tensors for N * views
+    cameras, set-major (camera n belongs to set n // views) -> rgba [N * views, H, W, 4].  Each image is tpx_raymarch_preview's."""
+    N, K, S = tpl.shape[0], tpl.shape[1], tpl.shape[2]
+    out = torch.empty(N * views, H, W, 4, dtype=torch.float32, device=tpl.device)
+    with torch.cuda.device(tpl.device):
+        _lib.check(_lib.lib().tpx_raymarch_preview_views(tpl.data_ptr(), pos.data_ptr(), rot.data_ptr(), scale.data_ptr(), *[c.data_ptr() for c in cam],
+                                                         N * views, views, K, S, H, W, float(volradius), float(stepsize), float(fadescale), float(fadeexp),
+                                                         out.data_ptr(), _lib.stream_ptr()), "tpx_raymarch_preview_views")
+    return out
+
+
+def box_colors(K: int, seed: int = 123456) -> torch.Tensor:
+    """The per-primitive colours of generate_colored_boxes: ``np.random.seed(seed)`` then ``np.random.rand(K, 3) * 255.0`` rounded to
+    fp32 [K,3] on the host.  The draws are the 3 K scalar ``np.random.rand()`` calls of the reference's loop, in its order, and numpy's
+    global generator is left where the reference leaves it."""
+    np.random.seed(seed)
+    return torch.from_numpy((np.random.rand(K, 3) * 255.0).astype(np.float32))
+
+
+def colored_boxes(N: int, K: int, S: int, colors: torch.Tensor, alpha: float, chlast: bool, device) -> torch.Tensor:
+    """tpx_colored_boxes: the lit box template for N copies of K primitives of S^3 with `colors` [K,3] fp32 -> [N,K,S,S,S,4] when
+    `chlast` (the march's layout), else [N,K,4,S,S,S] (the reference's)."""
+    shape = (N, K, S, S, S, 4) if chlast else (N, K, 4, S, S, S)
+    out = torch.empty(shape, dtype=torch.float32, device=device)
+    colors = colors.to(device=device, dtype=torch.float32).contiguous()
+    with torch.cuda.device(out.device):
+        _lib.check(_lib.lib().tpx_colored_boxes(colors.data_ptr(), N, K, S, float(alpha), _lib.LAYOUT_CHLAST if chlast else _lib.LAYOUT_NCDHW,
+                                                out.data_ptr(), _lib.stream_ptr()), "tpx_colored_boxes")
+    return out
+
+
+def generate_colored_boxes(template: torch.Tensor, prim_rot: torch.Tensor, alpha: float = 10000.0, seed: int = 123456) -> torch.Tensor:
+    """dva/ray_marcher.py:232-279 in one launch: a [N,K,4,S,S,S] template of the shape (not the values) of `template`, every primitive a
+    box of one random colour shaded by a fixed light, alpha `alpha`.  Reseeds numpy's global generator with `seed` and draws the
+    colours as the reference does (box_colors).  `prim_rot` is unused, as in the reference."""
+    if template.dim() != 6 or template.shape[2] != 4 or not (template.shape[3] == template.shape[4] == template.shape[5]):
+        raise ValueError(f"template must be [N, K, 4, S, S, S], got {tuple(template.shape)}")
+    if template.dtype != torch.float32:
+        raise ValueError(f"template must be fp32 (the box template is computed in fp32), got {template.dtype}")
+    if not template.is_cuda:
+        raise _lib.TpxError("generate_colored_boxes runs on CUDA only (no CPU path)")
+    N, K, S = template.shape[0], template.shape[1], template.shape[-1]
+    return colored_boxes(N, K, S, box_colors(K, seed), alpha, False, template.device)
 
 
 def subsample_offsets(batch_size: int, ray_subsample_factor: int, training: bool) -> list[tuple[int, int]]:
@@ -122,10 +183,7 @@ class RayMarcher(nn.Module):
             raise ValueError(f"ray_subsample_factor {f} does not fit a {H} x {W} image")
         grad = torch.is_grad_enabled() and any(t.requires_grad for t in (prim_rgba, prim_pos, prim_rot, prim_scale))
         dev = prim_rgba.device
-        with torch.no_grad():
-            cam = convert_camera_parameters(RT.to(dev).float(), K.to(dev).float())
-            f32 = lambda t: t.to(dev).float().contiguous()  # noqa: E731
-            cam = (f32(cam["campos"]), f32(cam["camrot"]), f32(torch.diagonal(cam["focal"], dim1=1, dim2=2)), f32(cam["princpt"]))
+        cam = march_camera(RT, K, dev)
         if f > 1:
             offsets = subsample_offsets(int(B), f, self.training)
             pixel_coords = offset_pixel_coords(self.base_pixel_coords, offsets, f)

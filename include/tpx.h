@@ -338,6 +338,30 @@ int tpx_raymarch_backward(const float* template_chlast, const float* primpos, co
                           const float* camrot, const float* focal, const float* princpt, int N, int K, int S, int H, int W, float volradius, float stepsize,
                           float fadescale, float fadeexp, int stride, const int* offsets, const float* raysat, const float* grad_rgba,
                           float* grad_template, float* grad_primpos, float* grad_primrot, float* grad_primscale, void* stream);
+/* tpx_raymarch_preview for N images of N / views primitive sets: image n marches primitive set n / views (template, primpos, primrot,
+ * primscale hold N / views sets) through camera n (campos, camrot, focal, princpt hold N cameras).  views >= 1 divides N.  A
+ * turntable of V views of one set is one launch over one template, bit-identical to V tpx_raymarch_preview calls; views = 1 is
+ * tpx_raymarch_preview. */
+int tpx_raymarch_preview_views(const float* template_chlast, const float* primpos, const float* primrot, const float* primscale, const float* campos,
+                               const float* camrot, const float* focal, const float* princpt, int N, int views, int K, int S, int H, int W,
+                               float volradius, float stepsize, float fadescale, float fadeexp, float* rgba_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Preview payloads (dva/visualize.py), forward only.  All pointers device fp32, contiguous.
+ * tpx_colored_boxes: the box template of generate_colored_boxes (dva/ray_marcher.py:232-279) for N batch copies of K primitives of S^3
+ * (S >= 2): colors [K,3] (the caller's np.random.rand(K, 3) * 255.0 rounded to fp32); per voxel (z, y, x) the dominant-axis sign
+ * normal n of meshgrid(linspace(-1,1,S)^3) with its y and z negated, normalised (0 / 0 = NaN at a centre voxel whose coordinates are
+ * all 0, as in the reference), mult = max(sum(lightdir * n), 0.2) with lightdir = -3 / ||(-3,-3,-3)|| per axis and NaN kept, and
+ * rgb = colors[k] * (1.4f * mult), alpha = alpha, each an fp32 operation in the reference's order.  layout TPX_LAYOUT_NCDHW writes
+ * out [N,K,4,S,S,S] (the reference's); TPX_LAYOUT_CHLAST writes [N,K,S,S,S,4] (the march's template, 16-B aligned).
+ * tpx_primvolume_payload: recon_param [B,P,4+6 S^3] (LatentCodec.pack's layout: scale, pos[3], sdf S^3, tex 3 S^3, mat 2 S^3) ->
+ * out [B,P,S,S,S,4] channels-last (16-B aligned): alpha = exp(-(sdf * (1 / 0.005f))^2) * 255 (visualize.py:217-232, bit for bit
+ * with torch's CUDA ops); mode TPX_PAYLOAD_RGB colours tex * 255, TPX_PAYLOAD_MAT colours (0, roughness, metallic) * 255.
+ * ---------------------------------------------------------------------------------------------------------- */
+enum { TPX_LAYOUT_NCDHW = 0, TPX_LAYOUT_CHLAST = 1 };
+enum { TPX_PAYLOAD_RGB = 0, TPX_PAYLOAD_MAT = 1 };
+int tpx_colored_boxes(const float* colors, int N, int K, int S, float alpha, int layout, float* out, void* stream);
+int tpx_primvolume_payload(const float* recon_param, int B, int P, int S, int mode, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Marching cubes — the `mcubes.marching_cubes(grid, 0.0)` call of extract_texmesh (inference.py:106-124), which copies the SDF grid
