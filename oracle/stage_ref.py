@@ -23,6 +23,11 @@ flags of their own setup.py except that ``-arch=sm_70`` becomes ``-gencode arch=
 placed beside its wrapper, where ``from . import mvpraymarchlib`` / ``from . import utilslib`` find it.  The host compile gets
 ``-DNDEBUG``: utils.cpp:67 and :113 assert on a ``size()`` that ``std::optional`` does not have, and the reference's setup.py build
 never compiles those asserts because setuptools passes Python's CFLAGS, which carry ``-DNDEBUG``.
+
+The first and last stages of the image-to-SDF path are staged too (byte-identical), so the ``-m gpu`` suite can run them next to the
+kernels: the image conditioner ``models/conditioner/image_dinov2.py`` with the ``dinov2/{hub,models,layers}`` files its import reaches
+(CONDITIONER_FILES; torchvision is its one outside dependency), and ``models/primsdf.py`` (PRIMSDF_FILES; its ``trimesh`` import is unused
+on the query path and stubbed by the loader).  ``oracle/refmods.py`` builds them.
 """
 from __future__ import annotations
 
@@ -44,6 +49,14 @@ FILES = [
 RAYMARCH_FILES = [
     "dva/__init__.py", "dva/ray_marcher.py", "dva/mvp/extensions/mvpraymarch/mvpraymarch.py", "dva/mvp/extensions/utils/utils.py",
 ]
+CONDITIONER_FILES = [
+    "models/conditioner/image_dinov2.py", "models/conditioner/dinov2/__init__.py",
+    "models/conditioner/dinov2/hub/__init__.py", "models/conditioner/dinov2/hub/backbones.py", "models/conditioner/dinov2/hub/utils.py",
+    "models/conditioner/dinov2/models/__init__.py", "models/conditioner/dinov2/models/vision_transformer.py",
+    *[f"models/conditioner/dinov2/layers/{m}.py" for m in ("__init__", "attention", "block", "dino_head", "drop_path", "layer_scale", "mlp",
+                                                           "patch_embed", "swiglu_ffn")],
+]
+PRIMSDF_FILES = ["models/primsdf.py"]
 SM90A = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # name -> (directory under the checkout, sources, nvcc flags of its setup.py with the arch replaced)
 EXTENSIONS = {
@@ -68,7 +81,7 @@ def stage(src: str = DEFAULT_SRC, dest: str = DEST) -> dict:
     if not os.path.isdir(src):
         raise FileNotFoundError(f"{src} not found: pass the path of a reference checkout")
     manifest = {"source": src, "files": {}}
-    for rel in FILES + RAYMARCH_FILES:
+    for rel in FILES + RAYMARCH_FILES + CONDITIONER_FILES + PRIMSDF_FILES:
         s, d = os.path.join(src, rel), os.path.join(dest, rel)
         os.makedirs(os.path.dirname(d), exist_ok=True)
         shutil.copyfile(s, d)
@@ -107,6 +120,14 @@ def staged(dest: str = DEST) -> bool:
 def raymarcher_staged(dest: str = DEST) -> bool:
     sos = [os.path.join(rel, name + ".so") for name, (rel, _, _) in EXTENSIONS.items()]
     return all(os.path.exists(os.path.join(dest, rel)) for rel in RAYMARCH_FILES + sos)
+
+
+def conditioner_staged(dest: str = DEST) -> bool:
+    return all(os.path.exists(os.path.join(dest, rel)) for rel in CONDITIONER_FILES)
+
+
+def primsdf_staged(dest: str = DEST) -> bool:
+    return all(os.path.exists(os.path.join(dest, rel)) for rel in PRIMSDF_FILES)
 
 
 if __name__ == "__main__":

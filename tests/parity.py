@@ -170,6 +170,21 @@ def is_fp32_tie(p, srt, S):
     return float(dv[1] - dv[0]) < 4e-7 * float(dv[0])
 
 
+def fp32_ties(p, srt, S, chunk=2048):
+    """is_fp32_tie of every point of p [n, 3] at once, on p's device in p's dtype (pass fp64): [n] bool."""
+    grid = local_grid(S).to(srt)
+    out = []
+    for c in p.split(chunk):
+        d = (c[:, None] - srt[None, :, 1:4]).norm(dim=2)
+        near = d.topk(min(2, d.shape[1]), dim=1, largest=False)
+        tie = (near.values[:, 1] - near.values[:, 0] < 4e-7 * near.values[:, 0]) if d.shape[1] > 1 else torch.zeros_like(d[:, 0], dtype=torch.bool)
+        k = near.indices[:, 0]
+        cand = srt[k, 1:4][:, None] + srt[k, 0][:, None, None] * grid[None]
+        dv = (c[:, None] - cand).norm(dim=2).topk(2, dim=1, largest=False).values
+        out.append(tie | (dv[:, 1] - dv[:, 0] < 4e-7 * dv[:, 0]))
+    return torch.cat(out) if out else torch.zeros(0, dtype=torch.bool, device=p.device)
+
+
 def same_mesh(got, want, what=""):
     """got (vertices fp32, faces int64) tensors equal to want (vertices, faces) numpy arrays byte for byte."""
     v, f = got

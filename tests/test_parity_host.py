@@ -172,6 +172,23 @@ def test_is_fp32_tie():
     assert not parity.is_fp32_tie(g[0] + 0.3 * (g[1] - g[0]), one, S)
 
 
+def test_fp32_ties_is_is_fp32_tie_per_point():
+    """The batched form agrees with is_fp32_tie point by point: random points, constructed primitive and voxel ties, a negative
+    scale (the box and the voxel grid are mirrored, the candidates the same), and a single primitive."""
+    S = 8
+    g = torch.Generator().manual_seed(3)
+    srt = torch.cat([0.05 + 0.1 * torch.rand(40, 1, generator=g), torch.rand(40, 3, generator=g) * 1.6 - 0.8], 1).double()
+    srt[7, 0] *= -1
+    srt[1, 1:] = srt[0, 1:] + torch.tensor([0.3, 0.0, 0.0], dtype=torch.float64)
+    vox = srt[7, 1:] + srt[7, 0] * local_grid(S).double()
+    p = torch.cat([torch.rand(300, 3, generator=g).double() * 2.4 - 1.2,
+                   (srt[0, 1:] + torch.tensor([0.15, 0.02, -0.01], dtype=torch.float64))[None],     # equidistant from primitives 0 and 1
+                   ((vox[9] + vox[10]) / 2)[None] + 1e-9])
+    want = torch.tensor([parity.is_fp32_tie(q, srt, S) for q in p])
+    assert bool(want[-2]) and torch.equal(parity.fp32_ties(p, srt, S, chunk=64), want)
+    assert torch.equal(parity.fp32_ties(p, srt[:1], S), torch.tensor([parity.is_fp32_tie(q, srt[:1], S) for q in p]))
+
+
 def test_same_mesh_compares_bytes():
     V = np.array([[0.0, 1.0, 2.0], [3.0, 4.0, 5.0], [6.0, 7.0, 8.0]], np.float32)
     F = np.array([[0, 1, 2]], np.int64)
